@@ -22,6 +22,9 @@ The N = 1 line also carries: `roofline` (ResStack pair unit of SURVEY 8d), `cpu_
 bounded sample), `parity` (waveform error of each precision against that oracle output; out of tolerance FAILS the run),
 `workloads` (configs[1] vocoder-only latency, configs[4] 10 min long-form through VoiceFixer.restore_inmem in modes
 0/1/2, the 64-item batch) and `gpu_library_baseline` (the reference's op sequence through stock PyTorch on the same GPU).
+
+--dump-outputs DIR writes the waveforms the timed path computed in its last step to DIR/restored.npy (float32, (B, L);
+a seeded row sample when the batch exceeds 64 MB): the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -43,7 +46,7 @@ FLOP_PER_AUDIO_SEC = 118.44e9        # BASELINE.md §2: 1184.4 GFLOP per 10 s ut
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -90,7 +93,8 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16 rate; a power-capped card reaches less
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 def host_threads():
@@ -302,35 +306,21 @@ def wl_cli(precision, n_files=8, seconds=10.0):
             "jobs_wall_s": jobs_wall, "value": (n_files * seconds / jobs_wall) if jobs_wall else None, "unit": UNIT}
 
 
-def csrc_sha(files=None):
-    """Hash of CUDA sources (all of csrc/, or the listed files): an ncu traffic figure is only quoted when the kernel it was
-    captured from is built from the same sources as the one that just ran."""
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "voicefixer_b200", "csrc")
-    for f in sorted(files or os.listdir(d)):
-        h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()[:16]
-
-
 def roofline_from(rep, B, L_by_stack, precision, peaks, peaks_src, tot_ms):
     """SURVEY 8(d): the unit of the HBM-bound ResStack kernels is the PAIR -- read x once, write x' once,
-    2 * C * L * 4 bytes per item -- whether a pair is one fused launch or two.  `frac` uses that; the kernel-level
-    figures on the builder's own per-launch byte model (DESIGN.md 4) go under `other`."""
+    2 * C * L * 4 bytes per item -- whether a pair is one fused launch or two.  `frac` uses that; the kernel-level figures on the per-launch byte model of the
+    engine's profile go under `other`."""
     cands = []
     for j, C in ((3, 64), (2, 128), (1, 256), (0, 512)):
         fused = rep.get(f"voc.rs{j}.pair")
         c1, c2 = rep.get(f"voc.rs{j}.c1"), rep.get(f"voc.rs{j}.c2")
         if fused:
             ms_pair, n = fused["ms"] / fused["count"], fused["count"]
-            kname = ("resstack_pair3_kernel (one SM, residual stashed in TMEM)" if precision == "tf32" and C == 64
-                     else "resstack_pair_kernel" if C == 64 else "resstack_pair2_kernel (two-CTA cluster)")
-            kern = f"{kname} [voc.rs{j}.pair]"
+            kern = f"pair_fused_kernel [voc.rs{j}.pair]"
             flops, model_bytes = fused["flops"] / fused["count"], fused["bytes"] / fused["count"]
         elif c1 and c2:
             ms_pair, n = (c1["ms"] + c2["ms"]) / c2["count"], c2["count"]
-            kern = (f"conv_ts_kernel (weights in TMEM) + conv_gemm_tc_kernel for large dilations [voc.rs{j}.c1 + voc.rs{j}.c2]"
-                    if precision == "tf32" and C == 128 else f"conv_gemm_tc_kernel x2 [voc.rs{j}.c1 + voc.rs{j}.c2]")
+            kern = f"conv_gemm_wgmma_kernel x2 [voc.rs{j}.c1 + voc.rs{j}.c2]"
             flops = (c1["flops"] + c2["flops"]) / c2["count"]
             model_bytes = (c1["bytes"] + c2["bytes"]) / c2["count"]
         else:
@@ -343,18 +333,9 @@ def roofline_from(rep, B, L_by_stack, precision, peaks, peaks_src, tot_ms):
     dom = max(hbm or cands, key=lambda c: c["total_ms"])
     gbs = dom["pair_bytes"] / (dom["ms_pair"] * 1e-3) / 1e9
     tf = dom["flops"] / (dom["ms_pair"] * 1e-3) / 1e12
-    traffic, tnote = None, "no ncu capture of these sources committed"
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        ent = tj.get(f"{'bf16' if precision == 'fp16' else precision}:voc.rs{dom['j']}.pair:B{B}")       # fp16 moves bf16's bytes
-        if ent and ent.get("csrc_sha") == csrc_sha(ent.get("files")):
-            traffic, tnote = ent["dram_bytes_per_pair"], ent.get("source", "profiles/")
-        elif ent:
-            tnote = "capture in profiles/ncu_traffic.json is from older sources: not quoted"
     return {"bound": "hbm", "kernel": dom["kern"], "unit_of_work": f"ResStack pair, C = {dom['C']}, {B} x {L_by_stack[dom['j']]} positions",
             "achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
-            "traffic": traffic, "traffic_note": tnote, "peak_source": f"{peaks_src} (hbm_gbs)",
+            "peak_source": f"{peaks_src} (hbm_gbs)",
             "algorithmic_bytes_per_pair": dom["pair_bytes"], "algorithmic_flops_per_pair": dom["flops"],
             "pairs_in_step": dom["n"], "avg_pair_ms": dom["ms_pair"], "share_of_step": dom["total_ms"] / tot_ms,
             "other": {"builder_byte_model_gbs": dom["model_bytes"] / (dom["ms_pair"] * 1e-3) / 1e9,
@@ -469,11 +450,22 @@ def measure_batch(args, precision, rank, world, local, B, full=True):
         sampler.start()
     ms_step = timed(False, args.steps) / args.steps
     clocks = sampler.stop() if rank == 0 and full else None
+    if full and args.dump_outputs:
+        y = gplan(dev_out) if gplan is not None else dev_out          # what the caller of the path receives: all ranks' items
+        if rank == 0:
+            dump_outputs(args.dump_outputs, y)
+        del y
     l0 = eng.launch_count(); eng.restore(dev_in, mode=0, out=dev_out); torch.cuda.synchronize()
     launches = (eng.launch_count() - l0) * args.steps                  # graph replays bypass the library's counter
+    used_graph = graph is not None
+    if world == 1:
+        # the e2e path below is restore_batch with its own graph: drop this one, so that at most two step workspaces
+        # (the engine's and one graph's) are alive at a time -- 55 GB at 64 x 10 s
+        graph = None
+        torch.cuda.empty_cache()
     audio_per_step = world * B * args.seconds
     res = {"value": audio_per_step / (ms_step / 1e3), "ms_per_step": ms_step, "gpu_launches": launches, "clocks": clocks,
-           "ws_gb": ws_gb, "bcast_ms": bcast_ms, "graph": graph is not None}
+           "ws_gb": ws_gb, "bcast_ms": bcast_ms, "graph": used_graph}
     step(True)
     ms_e2e = timed(True, args.steps) / args.steps
     res["e2e"] = {"value": audio_per_step / (ms_e2e / 1e3), "unit": UNIT, "ms_per_step": ms_e2e,
@@ -493,6 +485,41 @@ def measure_batch(args, precision, rank, world, local, B, full=True):
     return res
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, out):
+    """The timed path's result of its last step, (B, L) float32; rows in a fixed seeded sample if it exceeds 64 MB (the
+    sample and its row indices together stay within 64 MB)."""
+    y = out.float().cpu().numpy()
+    os.makedirs(path, exist_ok=True)
+    if y.nbytes > DUMP_LIMIT_BYTES:
+        keep = max(1, DUMP_LIMIT_BYTES // (y.shape[1] * 4 + 8) - 1)
+        rows = np.sort(np.random.default_rng(0).choice(y.shape[0], keep, replace=False))
+        np.save(os.path.join(path, "restored_rows.npy"), rows.astype(np.float64))
+        y = y[rows]
+    np.save(os.path.join(path, "restored.npy"), y)
+
+
+def start_batch64(args):
+    """configs[3]'s per-GPU share (64 x 10 s) on one GPU, measured in a child process that runs first, on its own: its
+    54 GB (workspace and CUDA-graph workspace) fit an 80 GB card only without the headline engine's memory beside them."""
+    cmd = [sys.executable, os.path.abspath(__file__), "--batch", "64", "--precision", args.precision, "--steps",
+           str(max(3, min(args.steps, 8))), "--warmup", str(args.warmup), "--seconds", str(args.seconds), "--no-extras",
+           "--no-cpu-baseline"]
+    r = subprocess.run(cmd, capture_output=True, text=True, env=dict(os.environ, WORLD_SIZE="1", RANK="0", LOCAL_RANK="0"))
+    return r
+
+
+def finish_batch64(r):
+    try:
+        d = json.loads(r.stdout.strip().splitlines()[-1])
+        return {"workload": "64 x 10 s per GPU (configs[3]'s per-GPU share) on ONE GPU: the weak-scaling base of the N > 1 lines",
+                "value": d["value"], "ms_per_step": d["ms_per_step"], "e2e": d["e2e"]["value"]}
+    except Exception:
+        return {"error": f"rc {r.returncode}: {r.stderr[-500:]}"}
+
+
 def parity_of(eng, wav, ref, precision):
     y = eng.restore(torch.from_numpy(wav)[None].to(f"cuda:{eng.device}")).cpu().numpy().astype(np.float64)
     ref = np.asarray(ref, dtype=np.float64).reshape(y.shape)
@@ -510,7 +537,8 @@ def torch_gpu_result(args, B):
     from voicefixer_b200 import synthetic
     from oracle import vf_oracle as O
     dev = "cuda:0"
-    # fp32 NCHW activations of the reference layout: ~3 GB per 10 s item at the peak
+    # fp32 NCHW activations of the reference layout: ~3 GB per 10 s item at the peak, so at most 16 items on an 80 GB GPU
+    B = min(B, 16)
     ana = {k: v.to(dev) for k, v in synthetic.make_analysis_state(0).items()}
     voc = {k: v.to(dev) for k, v in synthetic.make_vocoder_state(1).items()}
     O.mel_weight = (lambda f: (lambda: f().to(dev)))(O.mel_weight)
@@ -571,6 +599,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the second precision mode, the workloads and the library baseline")
     ap.add_argument("--no-graph", action="store_true", help="launch the kernels of a step individually")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's waveforms to DIR/restored.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         if not args.batch:
@@ -593,6 +622,8 @@ def main():
     prec = args.precision
     peaks, peaks_src = measured_peaks()
 
+    extras = rank == 0 and world == 1 and not args.no_extras
+    b64 = start_batch64(args) if extras else None
     res = measure_batch(args, prec, rank, world, local, B)
     rep = res["rep"]
     tot_ms = sum(r["ms"] for r in rep.values())
@@ -603,7 +634,6 @@ def main():
     whole_tf = FLOP_PER_AUDIO_SEC * B * args.seconds / (res["ms_per_step"] * 1e-3) / 1e12
     roofline["whole_step"] = {"tflops": whole_tf, "frac_of_bf16_sustained": whole_tf / peaks["bf16_tflops_sustained"]}
 
-    extras = rank == 0 and world == 1 and not args.no_extras
     cpu_baseline, parity, modes, workloads, lib_base = None, None, {}, {}, None
     run = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
@@ -633,20 +663,14 @@ def main():
             workloads["stream"] = wl_stream(vf)
         except Exception as e:
             workloads["stream"] = {"error": f"{type(e).__name__}: {e}"}
-    # free the headline engine before the next ones
+    # free the headline engine (and the workspace its workloads grew) before the next ones
+    vf = None
     res.pop("vf"); res.pop("eng"); res.pop("rep")
     import gc
     gc.collect(); torch.cuda.empty_cache()
     if extras:
         a2 = argparse.Namespace(**vars(args)); a2.steps = max(3, min(args.steps, 8))
-        try:
-            r64 = measure_batch(a2, prec, rank, world, local, 64, full=False)
-            workloads["batch64_1gpu"] = {"workload": "64 x 10 s per GPU (configs[3]'s per-GPU share) on ONE GPU: the weak-scaling base of the N > 1 lines",
-                                         "value": r64["value"], "ms_per_step": r64["ms_per_step"], "e2e": r64["e2e"]["value"]}
-            del r64
-        except Exception as e:
-            workloads["batch64_1gpu"] = {"error": f"{type(e).__name__}: {e}"}
-        gc.collect(); torch.cuda.empty_cache()
+        workloads["batch64_1gpu"] = finish_batch64(b64)
         for other in [m for m in ("fp16", "bf16", "tf32") if m != prec][:2]:
             try:
                 r2 = measure_batch(a2, other, rank, world, local, B, full=False)
@@ -680,7 +704,7 @@ def main():
                                     f"({B} per GPU), mode 0, NCCL weight broadcast + waveform gather"),
                        "precision": prec, "global_batch": world * B,
                        "launch": "CUDA graph replay of the step's launch sequence" if res["graph"] else "individual launches",
-                       "l2": f"no flush needed: {res['ws_gb']:.1f} GB of activations per step >> 126 MB L2",
+                       "l2": f"no flush needed: {res['ws_gb']:.1f} GB of activations per step >> 50 MB L2",
                        "parallelism": f"batch-shard x{world}: 2 collectives -- NCCL weight broadcast {res['bcast_ms']:.1f} ms (once, start-up) "
                                       "and one waveform gather per step on a side stream" if world > 1 else "single GPU"},
             "e2e": res["e2e"], "gpu_launches": res["gpu_launches"], "clocks": res["clocks"], "roofline": roofline,

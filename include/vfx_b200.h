@@ -1,4 +1,4 @@
-/* vfx_b200.h — C ABI of the B200-native VoiceFixer restore() hot path.
+/* vfx_b200.h — C ABI of the H100-native VoiceFixer restore() hot path.
  *
  * The reference (haoheliu/voicefixer, pure Python/PyTorch) has no FFI; its boundary for this path
  * is five nn.Module.forward seams (SURVEY 8b).  Each entry point below replaces one of them and
@@ -32,13 +32,13 @@ enum vfx_status {
 
 /* Arithmetic of the convolution GEMMs.
  *   FP32: SIMT fp32 FMA (validation path, bit-for-bit deterministic).
- *   BF16: tcgen05 tensor-core MMA (kind::f16), bf16 operands and weights, fp32 accumulation in TMEM.
- *   TF32: tcgen05 tensor-core MMA (kind::tf32), fp32 storage with operands and weights rounded to tf32
+ *   BF16: wgmma tensor-core MMA, bf16 operands and weights, fp32 accumulation.
+ *   TF32: wgmma tensor-core MMA (tf32), fp32 storage with operands and weights rounded to tf32
  *         (round-to-nearest) by their producers, fp32 accumulation -- the arithmetic of the reference's own
  *         CUDA path (torch.backends.cudnn.allow_tf32 defaults to True; the reference's test/test.py:27-35
  *         compares that path with its CPU path).  Weights are registered in the FP32 layout.
- *   FP16: tcgen05 kind::f16 on fp16 operands and weights, fp32 accumulation: the SAME 10-bit mantissa as tf32 (so the same
- *         waveform parity) in 2-byte storage, i.e. the BF16 mode's memory traffic, kernels and speed -- at fp16's exponent
+ *   FP16: wgmma on fp16 operands and weights, fp32 accumulation: the SAME 10-bit mantissa as tf32 (so the same
+ *         waveform parity) in 2-byte storage, i.e. the BF16 mode's memory traffic and kernels -- at fp16's exponent
  *         range (|x| < 65504; smaller than 6e-5 loses relative precision).  Everything outside the GEMM operands stays fp32. */
 enum vfx_precision { VFX_PREC_FP32 = 0, VFX_PREC_BF16 = 1, VFX_PREC_TF32 = 2, VFX_PREC_FP16 = 3 };
 
@@ -49,7 +49,7 @@ const char* vfx_last_error(void);
 int vfx_version(void);
 
 /* ---- engine lifetime ------------------------------------------------------------------ */
-/* device >= 0: an engine on that sm_100a device.  device == -1: a planning-only engine that makes no
+/* device >= 0: an engine on that sm_90a device.  device == -1: a planning-only engine that makes no
  * CUDA call -- vfx_engine_set_tensor / vfx_engine_finalize validate a weight set (names and byte sizes)
  * and vfx_workspace_bytes* size the workspace on a host without a GPU; every launching entry point
  * refuses it with VFX_ERR_INVALID. */
@@ -60,13 +60,13 @@ int vfx_engine_destroy(vfx_engine* e);
  * against what the engine expects when it is first used).  Names and layouts: DESIGN.md §3.
  * Replaces torch.load + load_state_dict: voicefixer/base.py:15-30, voicefixer/vocoder/base.py:24-32. */
 int vfx_engine_set_tensor(vfx_engine* e, const char* name, const void* dev_ptr, size_t bytes);
-/* Engine options: "use_tc" (BF16 / TF32; 1 = tcgen05 kernel [default], 0 = SIMT cross-check on the same operands),
+/* Engine options: "use_tc" (BF16 / FP16 / TF32; 1 = wgmma kernel [default], 0 = SIMT cross-check on the same operands),
  * "profile" (0/1/2, see vfx_profile_report; 2 = one tag per shape / dilation),
- * "fuse_pair" (BF16: width-64 ResStack pairs as one fused kernel, default 1),
  * "tf32_stream" (TF32: vocoder residual streams as one encoded tensor, vfx_conv_desc.res_enc / raw_enc, default 1),
- * "fuse_pair3" (TF32: width-64 ResStack pairs as one fused kernel, residual stashed in tensor memory, default 1),
- * "fuse_pair2" (two-CTA cluster pipeline: 1 [default] = BF16 / FP16 width-128 ResStack pairs, 2 = also TF32 width 64 when
- *  "fuse_pair3" is 0 [no gain there], 0 = off). */
+ * "fuse_pair" (BF16 / FP16: width-64 ResStack pairs as one fused kernel, default 1),
+ * "fuse_pair3" (TF32: width-64 ResStack pairs as one fused kernel on the encoded stream, default 1),
+ * "fuse_pair2" (1 [default] = BF16 / FP16 width-128 ResStack pairs fused, 2 = also TF32 width 64 when "fuse_pair3" is 0,
+ *  0 = off). */
 int vfx_engine_set_option(vfx_engine* e, const char* key, int value);
 /* Number of CUDA kernels this library has launched in this process (bench.py's gpu_launches). */
 unsigned long long vfx_launch_count(void);
@@ -159,7 +159,7 @@ typedef struct vfx_conv_desc {
   const float* act_shift;   /* out_act = act(result * act_scale[n] + act_shift[n]) (fused eval-mode BN) */
   /* TF32 "encoded stream" (vocoder ResStacks in VFX_PREC_TF32): ONE fp32 tensor S serves both as the next convolution's
    * tf32 operand and as the lossless carrier of the fp32 residual stream:  S = bits(lrelu(x, enc_slope)) + 0x1000.
-   * kind::tf32 ignores the low 13 mantissa bits of an operand, so reading S as an operand yields exactly
+   * The tf32 tensor core ignores the low 13 mantissa bits of an operand, so reading S as an operand yields exactly
    * round-to-nearest-tf32(lrelu(x)); subtracting 0x1000 from the bits and inverting the (bijective) leaky ReLU gives x back.
    * res_enc: `residual` holds S, it is decoded before the add.  raw_enc: `out_raw` receives S of the result. */
   int res_enc, raw_enc;
@@ -169,18 +169,17 @@ typedef struct vfx_conv_desc {
 enum vfx_act { VFX_ACT_NONE = 0, VFX_ACT_LRELU = 1, VFX_ACT_ELU = 2,
                VFX_ACT_LRELU_XSINX = 3 /* v = lrelu(x, p); v + sin v */, VFX_ACT_SIGMOID = 4 };
 
-/* impl: 0 = SIMT, 1 = tcgen05 (BF16, TF32 or FP16). */
+/* impl: 0 = SIMT, 1 = wgmma tensor cores (BF16, TF32 or FP16). */
 int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream);
 
-/* Fused ResStack pair on tcgen05:
+/* Fused ResStack pair on the wgmma tensor cores:
  *   x' = x + conv2_{k3,d=1}( lrelu_0.01( conv1_{k3,dilation}( a ) + b1 ) ) + b2
- * ResStack.forward voicefixer/vocoder/model/modules.py:592-595 (layers :550-576).  The intermediate never leaves the chip.
- * Three implementations (impl: 0 = pick, 1 = one CTA per tile [16-bit operands], 2 = two-CTA cluster pipeline: conv1 on one SM,
- * conv2 on its neighbour, the intermediate crossing through an L2-resident scratch ring, 3 = one CTA per tile in tf32: the
- * residual rides in the operand boxes and is stashed in tensor memory, 8 bytes of HBM traffic per element):
- *   VFX_PREC_BF16 / VFX_PREC_FP16, C = 64 (impl 1), C = 128 (impl 2): a = lrelu_0.01(x) in the operand format [B][L][C]; x fp32 is read as the residual
- *     and, if write_raw, overwritten with x' (or written to x_out); out_act (optional, bf16, must not alias a) receives act(x').
- *   VFX_PREC_TF32, C = 64 (impl 3, or 2), stream_enc = 1: a == x == the encoded stream S (vfx_conv_desc.raw_enc), fp32 [B][L][C];
+ * ResStack.forward voicefixer/vocoder/model/modules.py:592-595 (layers :550-576).
+ * impl: 0, 1 or 3 = one kernel, the intermediate h kept in shared memory (no scratch needed); 2 = the two convolutions per
+ * block of rows with h in `scratch` (required for impl 2: vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned).
+ *   VFX_PREC_BF16 / VFX_PREC_FP16, C = 64 or 128: a = lrelu_0.01(x) in the operand format [B][L][C]; x fp32 is read as the residual
+ *     and, if write_raw, overwritten with x' (or written to x_out); out_act (optional, operand format, must not alias a) receives act(x').
+ *   VFX_PREC_TF32, C = 64, stream_enc = 1: a == x == the encoded stream S (vfx_conv_desc.raw_enc), fp32 [B][L][C];
  *     the result goes to x_out (required, aliasing neither input) as S' (stream_enc_out = 1) or as plain x' (0).
  * w1 / w2: [3][C][C] in the operand format, tap-major.  Other shapes return VFX_ERR_UNSUPPORTED. */
 typedef struct vfx_pair_desc {
@@ -191,12 +190,12 @@ typedef struct vfx_pair_desc {
   int B, L, C;
   int write_raw;
   void* out_act; int act; float act_param;
-  int precision;            /* vfx_precision: VFX_PREC_BF16 (0 is read as BF16 for compatibility) or VFX_PREC_TF32 */
-  int impl;
-  float* x_out;             /* NULL = in place over x (bf16 only) */
+  int precision;            /* vfx_precision: VFX_PREC_BF16 (0 is read as BF16 for compatibility), VFX_PREC_FP16 or VFX_PREC_TF32 */
+  int impl;                 /* see above */
+  float* x_out;             /* NULL = in place over x (16-bit modes only) */
   int stream_enc, stream_enc_out;
-  void* scratch;            /* impl 2: device scratch of vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned (the */
-  size_t scratch_bytes;     /* intermediate tile crosses from one SM to its neighbour through it; stays in L2)          */
+  void* scratch;            /* impl 2: device scratch of vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned: holds h */
+  size_t scratch_bytes;
 } vfx_pair_desc;
 size_t vfx_resstack_pair_scratch_bytes(void);
 int vfx_resstack_pair(const vfx_pair_desc* d, void* stream);

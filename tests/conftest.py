@@ -14,7 +14,7 @@ torch.set_num_threads(min(8, os.cpu_count() or 1))   # the CPU oracle oversubscr
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -206,9 +206,8 @@ def test_wav_loader_mono_mix_and_resample(tmp_path):
 
 @pytest.mark.parametrize("precision", ["bf16", "fp32"])
 def test_planning_only_engine_validates_weight_sets_and_sizes_workspace(states, precision):
-    """vfx_engine_create(device=-1): finalize + workspace planning without a GPU.  The 20 x 30 s bf16 figure is
-    the one the B200 run of round 1 reported for the same batch (profiles/r01_bench_longform_N1.json: 17.168495616 GB)
-    plus the 16 MiB scratch ring of round 2's two-CTA ResStack pair pipeline."""
+    """vfx_engine_create(device=-1): finalize + workspace planning without a GPU.  The 20 x 30 s bf16 figure is the
+    workspace a GPU run of the same batch allocates (17.168495616 GB): a change to the launch sequence's buffers shows here."""
     import ctypes
     from voicefixer_b200 import _lib
     from voicefixer_b200.engine import Planner
@@ -217,7 +216,7 @@ def test_planning_only_engine_validates_weight_sets_and_sizes_workspace(states, 
     full = dict(pack_analysis(states[0], precision), **voc)
     pl = Planner(full, precision)
     if precision == "bf16":
-        assert pl.workspace_bytes(20, 44100 * 30) == 17168495616 + (16 << 20)
+        assert pl.workspace_bytes(20, 44100 * 30) == 17168495616
     small, big = pl.workspace_bytes(1, 44100), pl.workspace_bytes(8, 441000)
     assert 0 < small < big and pl.workspace_bytes(8, 441000) == big            # deterministic
     assert pl.workspace_bytes(1, 1024) == 0 and pl.workspace_bytes(0, 44100) == 0

@@ -3,9 +3,9 @@
 The reference's acceptance test is FLAC in / FLAC out through librosa.load and soundfile.write
 (test/test.py:48-57,85-89; voicefixer/base.py:47-49; tools/wav.py:37).  The decoder is pinned by
 (a) a libFLAC-encoded excerpt of the reference's own test input with the PCM of its sibling .wav
-(tests/golden/flac_libflac_excerpt.npz, made by tests/golden/make_flac_golden.py), (b) when
-/root/reference is present, every .flac the reference ships, against the MD5 signature libFLAC
-stored in STREAMINFO, and (c) hashlib for the MD5 itself.  The encoder is pinned by the decoder."""
+(tests/golden/flac_libflac_excerpt.npz, made by tests/golden/make_flac_golden.py), (b) one whole .flac the
+reference ships (tests/golden/reference_p360_001_mic1.flac, its test/utterance/original/p360_001_mic1.flac), against
+the MD5 signature libFLAC stored in STREAMINFO, and (c) hashlib for the MD5 itself.  The encoder is pinned by the decoder."""
 import glob
 import hashlib
 import os
@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_UTT = "/root/reference/test/utterance"
+REF_FLAC = os.path.join(ROOT, "tests", "golden", "reference_p360_001_mic1.flac")
 
 
 def test_hostio_library_exports_every_declared_symbol():
@@ -140,26 +140,16 @@ def test_wavio_flac_follows_the_file_extension(tmp_path):
     assert m.shape == (60000,)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_UTT), reason="reference checkout not present (GPU box)")
-def test_decode_every_reference_flac_against_its_libflac_md5():
-    """All FLAC files the reference ships (inputs, targets, outputs): header fields, frame CRCs and the MD5
-    signature written by libFLAC; sample counts are the ones BASELINE.md quotes; original.flac == original.wav."""
-    from voicefixer_b200 import _hostio, wavio
-    files = sorted(glob.glob(os.path.join(REF_UTT, "*", "*.flac")))
-    assert len(files) >= 6
-    expect = {"original.flac": 132300, "p360_001_mic1.flac": 96076, "oracle.flac": 97902, "output_mode_0.flac": 132300,
-              "output_mode_1.flac": 132096, "output_mode_2.flac": 132300}
-    for f in files:
-        data = open(f, "rb").read()
-        info = _hostio.flac_info(data)
-        assert any(info.md5), f
-        pcm, sr, bps = _hostio.flac_decode(data)                     # raises on CRC / MD5 mismatch
-        assert (sr, bps, pcm.shape) == (44100, 16, (expect[os.path.basename(f)], 1)), f
-        assert hashlib.md5(pcm.astype("<i2").tobytes()).digest() == bytes(info.md5)
-    with wave.open(os.path.join(REF_UTT, "original", "original.wav"), "rb") as w:
-        ref = np.frombuffer(w.readframes(w.getnframes()), dtype="<i2")
-    got = wavio.load_mono(os.path.join(REF_UTT, "original", "original.flac"))
-    assert np.array_equal(got, ref.astype(np.float32) / 32768.0)
+def test_decode_reference_flac_against_its_libflac_md5():
+    """A whole FLAC file the reference ships (libFLAC-encoded input of its acceptance test): header fields, frame CRCs and
+    the MD5 signature written by libFLAC; the sample count is the one BASELINE.md quotes."""
+    from voicefixer_b200 import _hostio
+    data = open(REF_FLAC, "rb").read()
+    info = _hostio.flac_info(data)
+    assert any(info.md5)
+    pcm, sr, bps = _hostio.flac_decode(data)                         # raises on CRC / MD5 mismatch
+    assert (sr, bps, pcm.shape) == (44100, 16, (96076, 1))
+    assert hashlib.md5(pcm.astype("<i2").tobytes()).digest() == bytes(info.md5)
 
 
 # ------------------------------------------------------------------ decoder paths no available file reaches

@@ -1,9 +1,9 @@
-"""GPU tests of the fused ResStack pair kernel (vfx_resstack_pair: conv1 -> h on chip -> conv2 + residual, tcgen05)
-through the C ABI, against the same arithmetic spelled out with torch ops: bf16 operands (a, h, weights), fp32
+"""GPU tests of the ResStack pair entry point (vfx_resstack_pair: conv1 -> h in the caller's scratch -> conv2 + residual,
+on the tensor-core convolution) through the C ABI, against the same arithmetic spelled out with torch ops: bf16 operands (a, h, weights), fp32
 accumulation, fp32 residual stream.  Reference op: ResStack.forward voicefixer/vocoder/model/modules.py:592-595.
 
 Tolerances: fp32 output 1e-4 relative RMS (bf16 x bf16 products are exact in fp32; a rare bf16 rounding tie of the
-on-chip intermediate h may flip against torch's), activated bf16 output 4e-3 (one bf16 rounding)."""
+intermediate h may flip against torch's), activated bf16 output 4e-3 (one bf16 rounding)."""
 import ctypes
 import pytest
 import torch
@@ -33,10 +33,21 @@ def _pair(x, a, w1, b1, w2, b2, dil, write_raw=True, act="lrelu", act_param=0.01
     d.out_act = out_act.data_ptr() if want_act else None
     d.act, d.act_param = _lib.ACT[act], act_param
     d.precision = _lib.PREC[prec]
+    d.scratch, d.scratch_bytes = _scratch(lib)
     _lib.check(lib.vfx_resstack_pair(ctypes.byref(d), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
                "vfx_resstack_pair")
     torch.cuda.synchronize()
     return out_act
+
+
+_SCRATCH = {}
+
+
+def _scratch(lib):
+    n = int(lib.vfx_resstack_pair_scratch_bytes())
+    if "buf" not in _SCRATCH:
+        _SCRATCH["buf"] = torch.empty(n, dtype=torch.uint8, device=DEV)
+    return _SCRATCH["buf"].data_ptr(), n
 
 
 def _ref(x, a, w1, b1, w2, b2, dil):
@@ -63,7 +74,7 @@ def test_pair_matches_two_convolutions(L, dil, B):
 
 @pytest.mark.parametrize("L,dil,B", [(3000, 3, 2), (4000, 243, 1)])
 def test_pair_fp16_operands(L, dil, B):
-    """The same kernel with the other kind::f16 operand format: fp16 a / h / weights (tf32's mantissa in 2 bytes)."""
+    """The other 16-bit operand format: fp16 a / h / weights (tf32's mantissa in 2 bytes)."""
     torch.backends.cudnn.allow_tf32 = False
     C = 64
     x = _rnd(B, L, C, seed=1)
@@ -97,7 +108,7 @@ def test_pair_output_variants():
 
 
 def test_pair_rejects_other_widths():
-    """Widths whose weight sets fit neither one SM (64) nor a two-SM pipeline (128) are refused, not mis-computed."""
+    """Widths other than the vocoder's last two ResStacks (64, 128) are refused, not mis-computed."""
     from voicefixer_b200._lib import VfxError
     x = _rnd(1, 200, 256, seed=21)
     a = x.bfloat16()
@@ -107,7 +118,7 @@ def test_pair_rejects_other_widths():
         _pair(x, a, w, b, w, b, 1)
 
 
-# ---------------------------------------------------------------------------- two-CTA cluster pipeline (impl = 2)
+# ---------------------------------------------------------------------------- width 128 and the scratch
 def test_pair2_needs_scratch():
     from voicefixer_b200 import _lib
     from voicefixer_b200._lib import VfxError
@@ -124,18 +135,11 @@ def test_pair2_needs_scratch():
         _lib.check(lib.vfx_resstack_pair(ctypes.byref(d), None), "pair2")
 
 
-_SCRATCH = {}
-
-
 def _desc(lib_mod, **kw):
     d = lib_mod.PairDesc()
     for k, v in kw.items():
         setattr(d, k, v)
-    if kw.get("impl") == 2:                 # the two-CTA pipeline hands the intermediate tile over through this scratch ring
-        n = int(lib_mod.load().vfx_resstack_pair_scratch_bytes())
-        if "buf" not in _SCRATCH:
-            _SCRATCH["buf"] = torch.empty(n, dtype=torch.uint8, device=DEV)
-        d.scratch, d.scratch_bytes = _SCRATCH["buf"].data_ptr(), n
+    d.scratch, d.scratch_bytes = _scratch(lib_mod.load())
     return d
 
 
@@ -143,7 +147,7 @@ def _desc(lib_mod, **kw):
 @pytest.mark.parametrize("C,L,dil,B", [(128, 1000, 1, 2), (128, 5000, 27, 1), (128, 700, 243, 2), (128, 20000, 9, 3),
                                        (128, 9000, 2187, 1), (128, 125, 1, 1)])
 def test_pair2_16bit_matches_two_convolutions(C, L, dil, B, prec):
-    """conv1 on one SM, conv2 on its cluster neighbour, h through the L2-resident scratch ring: same arithmetic as impl 1."""
+    """Width 128: same arithmetic as width 64."""
     from voicefixer_b200 import _lib
     lib = _lib.load()
     torch.backends.cudnn.allow_tf32 = False
@@ -181,9 +185,9 @@ def _dec(s, slope=0.01):
                                              (40000, 243, 3, 1), (378, 9, 1, 1)])
 def test_pair_tf32_encoded_stream(L, dil, B, enc_out, impl):
     """tf32, C = 64: the encoded stream S is operand and residual carrier; the result goes to the other buffer as S' (or as
-    plain x' for the last pair of a stack).  impl 3 = one SM, residual stashed in tensor memory (resstack_pair3_tc.cu: halo
-    boxes for d <= 9, aligned boxes beyond); impl 2 = the two-CTA pipeline.  Reference: tf32-rounded operands and
-    intermediate, fp32 accumulation."""
+    plain x' for the last pair of a stack).  impl 3 and 2 are the values callers of the sm_100a build pass; both must be
+    accepted: 3 runs the fused kernel, 2 the two convolutions per row block through the scratch.  Reference: tf32-rounded
+    operands and intermediate, fp32 accumulation."""
     from voicefixer_b200 import _lib
     from voicefixer_b200.weights import round_tf32
     lib = _lib.load()

@@ -94,8 +94,8 @@ def test_api_dropin_restore_inmem_and_segmentation(tmp_path, monkeypatch, states
 # ---------------------------------------------------------------------------- BASELINE sizes, asserting
 # One 10 s utterance (T = 1001 frames, BASELINE configs[2] item size) and one 30 s segment (T = 3001, the segment
 # size of restore_inmem, voicefixer/base.py:116) against the CPU oracle on the same input and checkpoints, in every
-# precision.  Frozen after measurement on B200 (tools/measure_parity.py; CPU prediction of the operand-rounding
-# error alone, tools/sim_precision.py: tf32 1.7e-3, bf16 1.3e-2 relative RMS):
+# precision (CPU prediction of the operand-rounding error alone, tools/sim_precision.py: tf32 1.7e-3, bf16 1.3e-2
+# relative RMS):
 #   fp32   rel-RMS 2e-4
 #   tf32   rel-RMS 2e-3, mean-abs 1e-3      (SURVEY 8d's figure; measured 1.65e-3 / 3.5e-4 on the 10 s utterance)
 #   fp16   as tf32: the same 10-bit mantissa (CPU prediction 1.64e-3), 2-byte operands, fp16's exponent range
@@ -152,9 +152,8 @@ def test_full_size_properties(engine):
 
 
 # ---------------------------------------------------------------------------- bf16 tensor-core path
-# Stated tolerances for precision "bf16" (tcgen05 MMA: bf16 operands, fp32 accumulation in TMEM, fp32
-# bias / residual stream / activations).  Measured on B200 against the reference goldens
-# (tools/measure_parity.py): log-mel rel-RMS 5.4e-3, waveform rel-RMS 1.0-1.3e-2, mean-abs 2.5e-3.
+# Stated tolerances for precision "bf16" (wgmma: bf16 operands, fp32 accumulation, fp32 bias / residual stream /
+# activations), with margin over the error of bf16 rounding against the reference goldens.
 TOL_BF16_STAGE, TOL_BF16_WAV, TOL_BF16_MAE = 1.5e-2, 3e-2, 5e-3      # reference's own bar: mean-abs 1e-2
 
 
@@ -207,9 +206,9 @@ def test_bf16_mode2_vs_reference_golden(engine_bf16):
 
 
 # ---------------------------------------------------------------------------- tf32 tensor-core path
-# precision "tf32": tcgen05 kind::tf32 on fp32 storage, every operand rounded to tf32 by its producer, fp32
+# precision "tf32": wgmma tf32 on fp32 storage, every operand rounded to tf32 by its producer, fp32
 # accumulation -- the arithmetic class of the reference's own CUDA path (cuDNN TF32 convolutions, SURVEY D10).
-TOL_TF32_STAGE, TOL_TF32_WAV, TOL_TF32_MAE = 1e-3, 2e-3, 1e-3      # measured: log-mel <= 7e-4, wav 1.3-1.8e-3
+TOL_TF32_STAGE, TOL_TF32_WAV, TOL_TF32_MAE = 1e-3, 2e-3, 1e-3
 
 
 @pytest.fixture(scope="module")
@@ -240,8 +239,8 @@ def test_tf32_restore_vs_reference_golden(engine_tf32):
 
 
 def test_tf32_tensor_core_path_equals_simt_on_same_operands(engine_tf32):
-    """tf32 x tf32 products are exact in fp32: the SIMT kernel on the same rounded operands differs from the tcgen05
-    kernel only by accumulation order and the fast-math activations, far below the tf32 rounding noise."""
+    """tf32 x tf32 products are exact in fp32: the SIMT kernel on the same rounded operands differs from the wgmma
+    kernel only by accumulation order, far below the tf32 rounding noise."""
     from voicefixer_b200 import synthetic
     wav = synthetic.make_utterances(2, seconds=0.5, seed=13)
     y_tc = engine_tf32.restore(wav).cpu().numpy()
@@ -275,12 +274,12 @@ def test_tf32_encoded_stream_engine_path(states, oracle_10s):
 
 @pytest.mark.parametrize("prec", ["tf32", "fp16", "bf16"])
 def test_two_cta_pair_pipeline_engine_path(states, oracle_10s, prec):
-    """fuse_pair2: ResStack pairs as a two-CTA cluster pipeline (bf16 width 128, tf32 width 64): same tolerance as the
-    mode's plain path, and within rounding noise of it."""
+    """fuse_pair2: the width-128 ResStack pairs of the 16-bit modes (and, with 2, the tf32 width-64 pairs) as fused kernels:
+    same tolerance as the mode's plain path, and within rounding noise of it."""
     from voicefixer_b200.engine import Engine
     wav, ref = oracle_10s
     eng = Engine(states[0], states[1], precision=prec)
-    eng.set_option("fuse_pair3", 0)                       # tf32 width 64 would otherwise take the one-SM fused kernel
+    eng.set_option("fuse_pair3", 0)                       # tf32 width 64 would otherwise be fused already
     eng.set_option("fuse_pair2", 0)
     y0 = eng.restore(wav[None]).cpu().numpy()
     eng.set_option("fuse_pair2", 2)
@@ -290,8 +289,8 @@ def test_two_cta_pair_pipeline_engine_path(states, oracle_10s, prec):
 
 
 def test_tf32_fused_pair_engine_path(states, oracle_10s):
-    """fuse_pair3 (default on): the width-64 ResStack pairs of the tf32 mode as one fused kernel each (h on chip, residual
-    stashed in tensor memory): same arithmetic as the two-launch path -- the outputs agree to rounding noise of the
+    """fuse_pair3 (default on): the width-64 ResStack pairs of the tf32 mode as one fused kernel each (h kept in shared
+    memory): same arithmetic as the two-launch path -- the outputs agree to rounding noise of the
     accumulation order, far inside the mode's tolerance."""
     from voicefixer_b200.engine import Engine
     wav, ref = oracle_10s
@@ -305,7 +304,7 @@ def test_tf32_fused_pair_engine_path(states, oracle_10s):
 
 
 # ---------------------------------------------------------------------------- fp16 tensor-core path
-# precision "fp16": the bf16 mode's kernels (fused ResStack pair included) with the other kind::f16 operand format.  fp16
+# precision "fp16": the bf16 mode's kernels (fused ResStack pairs included) with the other 16-bit operand format.  fp16
 # carries tf32's 10-bit mantissa, so the tolerances are tf32's.
 @pytest.fixture(scope="module")
 def engine_fp16(states):

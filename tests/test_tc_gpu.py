@@ -1,5 +1,5 @@
-"""GPU tests of the tcgen05/TMA/TMEM conv-GEMM kernel (impl=1) through the C ABI, in both operand formats
-(bf16: kind::f16; tf32: kind::tf32 on fp32 storage pre-rounded to tf32).
+"""GPU tests of the wgmma conv-GEMM kernel (impl=1) through the C ABI, in every operand format
+(bf16 / fp16; tf32 on fp32 storage pre-rounded to tf32).
 
 bf16 x bf16 and tf32 x tf32 products are exact in fp32, so against an fp32 torch conv of the SAME rounded
 operands only the accumulation order differs: tolerance 2e-5 relative RMS on the fp32 output; the activated
@@ -167,7 +167,7 @@ def _dec(s, slope=0.01):
 @pytest.mark.parametrize("C,L,dil", [(64, 3000, 3), (128, 1000, 1), (256, 500, 243)])
 def test_tf32_encoded_stream(C, L, dil, impl):
     """One fp32 tensor S as tf32 operand AND lossless residual carrier.  The UN-rounded S goes to the tensor core: this
-    passes only if kind::tf32 ignores the low 13 mantissa bits (then the operand it sees is round-to-nearest(lrelu(x)))."""
+    passes only if the tf32 tensor core ignores the low 13 mantissa bits (then the operand it sees is round-to-nearest(lrelu(x)))."""
     from gpu_util import conv_gemm
     from voicefixer_b200.weights import round_tf32
     torch.backends.cudnn.allow_tf32 = False
@@ -189,13 +189,12 @@ def test_tf32_encoded_stream(C, L, dil, impl):
     assert rel_rms(got_op.cpu(), F.leaky_relu(ref, 0.01).cpu()) < 5e-4
 
 
-# ---------------------------------------------------------------------------- tf32, width 128: weights resident in TMEM
+# ---------------------------------------------------------------------------- tf32, width 128: the ResStack output forms
 @pytest.mark.parametrize("mode", ["act", "enc", "xsinx", "plain"])
 @pytest.mark.parametrize("L,dil,B", [(1000, 1, 2), (64, 3, 1), (63, 1, 1), (777, 9, 2), (5000, 27, 1), (3000, 81, 2),
                                      (9000, 2187, 1), (20000, 243, 3), (130, 729, 1)])
 def test_tf32_c128_weights_in_tmem(L, dil, B, mode):
-    """conv_ts_tc.cu (the C = 128 ResStack convolutions of the tf32 mode): transposed GEMM, weights as the A operand from
-    tensor memory, activations as B.  The four output forms the vocoder uses: activated operand only (conv1), encoded residual
+    """The C = 128 ResStack convolutions of the tf32 mode.  The four output forms the vocoder uses: activated operand only (conv1), encoded residual
     in / encoded stream out in place (conv2), encoded residual in / x + sin x operand out (last conv2 of a stack), plain
     residual / plain raw.  Against torch on the same tf32-rounded operands (fp32 accumulation: only the order differs)."""
     from gpu_util import conv_gemm

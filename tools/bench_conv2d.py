@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 conv kernel on the UNet 3x3 shapes (CUDA events).
+"""Micro-benchmark of the tensor-core conv kernel on the UNet 3x3 shapes (CUDA events).
 usage: python tools/bench_conv2d.py [--C 32 --H 1024 --W 127 --B 8 --kind f|r]"""
 import argparse, os, sys, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Capacity planning without a GPU: weight arena and activation workspace of restore() for a batch shape, and the
-largest batch that fits a given HBM budget (B200: 180 GB).  Uses the planning-only engine (vfx_engine_create with
+largest batch that fits a given HBM budget (H100: 80 GB).  Uses the planning-only engine (vfx_engine_create with
 device -1), i.e. the same dry-run allocator pass that sizes the workspace on the device.
 
-    python tools/plan_capacity.py --seconds 10 --batch 32 --precision bf16 [--hbm-gb 180]
+    python tools/plan_capacity.py --seconds 10 --batch 32 --precision bf16 [--hbm-gb 80]
 """
 import argparse
 import os
@@ -12,7 +12,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
-def plan(seconds, batch, precision, hbm_gb=180.0, reserve_gb=4.0):
+def plan(seconds, batch, precision, hbm_gb=80.0, reserve_gb=4.0):
     from voicefixer_b200 import synthetic
     from voicefixer_b200.engine import Planner
     from voicefixer_b200.weights import pack_analysis, pack_vocoder
@@ -38,7 +38,7 @@ if __name__ == "__main__":
     ap.add_argument("--seconds", type=float, default=10.0)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
-    ap.add_argument("--hbm-gb", type=float, default=180.0)
+    ap.add_argument("--hbm-gb", type=float, default=80.0)
     a = ap.parse_args()
     for k, v in plan(a.seconds, a.batch, a.precision, a.hbm_gb).items():
         print(f"{k:14s} {v:.3f}" if isinstance(v, float) else f"{k:14s} {v}")

@@ -1,4 +1,4 @@
-"""What does tcgen05 kind::tf32 do with fp32 operand bits below the tf32 mantissa?  Runs the tcgen05 conv kernel (1 tap,
+"""What does wgmma tf32 do with fp32 operand bits below the tf32 mantissa?  Runs the tensor-core conv kernel (1 tap,
 C = 64) on UN-rounded fp32 operands and compares with fp32 references computed from (a) truncated, (b) round-to-nearest
 tf32 operands.  The engine relies on the answer (operands are pre-rounded by their producers so that either way is exact)."""
 import os, sys, torch
@@ -23,4 +23,4 @@ got = raw[0, 0].double()
 for name, f in (("truncate", trunc), ("round-to-nearest", lambda t: round_tf32(t.cpu()).cuda())):
     ref = f(x)[0, 0].double() @ f(w)[0].double().t()
     err = float(((got - ref) ** 2).mean().sqrt() / (ref ** 2).mean().sqrt())
-    print(f"kind::tf32 on raw fp32 operands vs {name:17s} reference: rel-rms {err:.3e}")
+    print(f"wgmma tf32 on raw fp32 operands vs {name:17s} reference: rel-rms {err:.3e}")

@@ -6,7 +6,7 @@ a tensor-core input format (fp32 accumulate stays) and reports the waveform erro
 the stated tolerances of the tf32 / bf16 engine modes were derived before the kernels were measured on the GPU:
 
   tf32-rn    cvt.rna.tf32.f32 on both operands (what the engine's tf32 mode does when it writes operands)
-  tf32-trunc hardware truncation of raw fp32 operands (what kind::tf32 does to un-rounded inputs)
+  tf32-trunc hardware truncation of raw fp32 operands (what the tf32 tensor core does to un-rounded inputs)
   bf16       round-to-nearest bf16 operands (the engine's bf16 mode)
   fp16       round-to-nearest fp16 operands: the same 10-bit mantissa as tf32 in 2 bytes (5-bit exponent)
 

@@ -2,7 +2,7 @@
 
     from voicefixer import VoiceFixer, Vocoder
 
-resolves to the B200-native implementation in `voicefixer_b200` (same signatures, checkpoint
+resolves to the H100-native implementation in `voicefixer_b200` (same signatures, checkpoint
 paths and error behaviour; see INTEGRATION.md).  Nothing is imported from the reference package."""
 from voicefixer_b200 import __getattr__ as _lazy   # noqa: F401
 

@@ -1,4 +1,4 @@
-"""voicefixer_b200 — B200-native (sm_100a) implementation of VoiceFixer's restore() hot path.
+"""voicefixer_b200 — H100-native (sm_90a) implementation of VoiceFixer's restore() hot path.
 
 Public API mirrors the reference package:  `from voicefixer_b200 import VoiceFixer, Vocoder`.
 Importing this package does not touch CUDA; constructing VoiceFixer/Vocoder/Engine loads the

@@ -1,7 +1,7 @@
 """ctypes binding of libvfx_b200.so (the C ABI declared in include/vfx_b200.h).
 
 There is no CPU or PyTorch fallback: if the shared library is missing or fails to load, importing
-the product path raises.  Build it with `python -m voicefixer_b200.build` (nvcc, sm_100a)."""
+the product path raises.  Build it with `python -m voicefixer_b200.build` (nvcc, sm_90a)."""
 import ctypes
 import os
 

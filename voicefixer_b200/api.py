@@ -1,7 +1,7 @@
 """Drop-in mirror of the reference's public API (voicefixer/base.py, voicefixer/vocoder/base.py).
 
 Same class names, method signatures, checkpoint paths and error types; the bodies run the
-hand-written sm_100a kernels through the C-ABI engine.  The `cuda` argument is accepted for
+hand-written sm_90a kernels through the C-ABI engine.  The `cuda` argument is accepted for
 signature compatibility: the computation always runs on the GPU (there is no CPU path)."""
 import os
 import numpy as np
@@ -25,7 +25,7 @@ def _check_cuda(cuda):
     if not torch.cuda.is_available():
         if cuda:
             raise RuntimeError("Error: You set cuda=True but no cuda device found.")
-        raise RuntimeError("voicefixer_b200 has no CPU path: a B200 (sm_100a) device is required.")
+        raise RuntimeError("voicefixer_b200 has no CPU path: an H100 (sm_90a) device is required.")
 
 
 def _load_vocoder_state():

@@ -1,4 +1,4 @@
-"""Builds voicefixer_b200/libvfx_b200.so in-tree with nvcc for sm_100a (no JIT cache), and the
+"""Builds voicefixer_b200/libvfx_b200.so in-tree with nvcc for sm_90a (no JIT cache), and the
 host-only audio file codec voicefixer_b200/libvfx_hostio.so with gcc."""
 import os
 import subprocess
@@ -7,9 +7,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvfx_b200.so")
-SOURCES = ["engine.cu", "conv_gemm_simt.cu", "conv_gemm_tc.cu", "conv_ts_tc.cu", "resstack_pair_tc.cu", "resstack_pair2_tc.cu", "resstack_pair3_tc.cu", "elementwise.cu", "frontend.cu",
+SOURCES = ["engine.cu", "conv_gemm_simt.cu", "conv_gemm_tc.cu", "resstack_pair.cu", "elementwise.cu", "frontend.cu",
            "gru.cu", "hf_cut.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

@@ -11,7 +11,7 @@
 //   Conv1d k3/k7 dilated  voicefixer/vocoder/model/generator.py:33-54,75,96; modules.py:550-576
 //   ConvTranspose1d       voicefixer/vocoder/model/modules.py:451-459 (u output phases, 2 taps each)
 // With bf16 (or tf32-rounded) operands it reproduces the tensor-core path's arithmetic (the products are
-// exact in fp32) and is used by tests to cross-check the tcgen05 kernel.
+// exact in fp32) and is used by tests to cross-check the wgmma kernel.
 #include "vfx_common.cuh"
 
 namespace vfx {
@@ -28,8 +28,8 @@ template <> struct Vec8<float> {
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
   }
 };
-// tf32 operands: what kind::tf32 does with an fp32 word -- the low 13 mantissa bits are ignored (measured on B200,
-// tools/probe_tf32_rounding.py).  Pre-rounded operands pass through unchanged; an encoded stream (res_enc / raw_enc)
+// tf32 operands: what the tf32 tensor-core instructions do with an fp32 word -- the low 13 mantissa bits are ignored
+// (tools/probe_tf32_rounding.py).  Pre-rounded operands pass through unchanged; an encoded stream (res_enc / raw_enc)
 // comes out as round-to-nearest(lrelu(x)), exactly as on the tensor core.
 template <> struct Vec8<tf32_t> {
   float v[8];
@@ -190,7 +190,7 @@ int conv_gemm_simt(int precision, const vfx_conv_desc& d, cudaStream_t st) {
     conv_gemm_simt_kernel<__nv_bfloat16><<<grid, NT, 0, st>>>(d, vec_ok);
   else if (precision == VFX_PREC_FP16)
     conv_gemm_simt_kernel<__half><<<grid, NT, 0, st>>>(d, vec_ok);
-  else if (precision == VFX_PREC_TF32)     // fp32 FMA on tf32-rounded operands (products exact): same arithmetic as kind::tf32
+  else if (precision == VFX_PREC_TF32)     // fp32 FMA on tf32-rounded operands (products exact): same arithmetic as wgmma tf32
     conv_gemm_simt_kernel<tf32_t><<<grid, NT, 0, st>>>(d, vec_ok);
   else
     conv_gemm_simt_kernel<float><<<grid, NT, 0, st>>>(d, vec_ok);

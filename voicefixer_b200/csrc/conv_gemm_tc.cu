@@ -1,919 +1,200 @@
-// Channels-last shifted-window convolution GEMM on the 5th-gen tensor cores (sm_100a):
-// TMA-staged operand tiles -> tcgen05.mma (fp32 accumulators in TMEM) -> fused epilogue.
-// Two operand formats, same kernel (template parameter TF32):
-//   VFX_PREC_BF16  bf16 operands / weights, kind::f16, UMMA K = 16, K chunk = 64 channels (32 if Cin == 32)
-//   VFX_PREC_FP16  fp16 operands / weights: the same kernel as bf16 with the other kind::f16 operand format
-//   VFX_PREC_TF32  fp32 storage rounded to tf32 by the producers, kind::tf32, UMMA K = 8, K chunk = 32 channels
-// (a K chunk is one swizzled 128-byte row -- 64 bytes for the bf16 Cin == 32 case -- so every piece of address
-// arithmetic below is in bytes and shared by both formats; one MMA always advances 32 bytes along K).
+// Channels-last shifted-window convolution GEMM on the Hopper tensor cores (wgmma), the bf16 / fp16 / tf32 path of
+// every Conv1d / Conv2d / ConvTranspose / Linear (field semantics: include/vfx_b200.h, vfx_conv_desc).
 //
-// Same contract as conv_gemm_simt (vfx_conv_desc); this is the production path behind the
-// reference's Conv1d / Conv2d / ConvTranspose / Linear layers (file:line list in conv_gemm_simt.cu).
+//   out[b, oh, ow, n] = bias[n % bias_mod] + residual + sum_{tap} sum_{c} W[tap][n][c] * A[b, qh+dh, qw+dw, c]
 //
-//   D[128 positions][Ntile channels] += A_tap[128][KC] * W_tap[Ntile][KC]^T     (K-major, SW128/SW64)
-//
-// * One M-tile = a (th x tw) patch of the output grid of one item, th*tw = 128.  Operand staging:
-//     generic   every tap is a TMA box of the patch shifted by (dh, dw); rows/columns outside the
-//               tensor are zero-filled by TMA = the convolution's zero padding (no im2col).
-//     halo      (weights resident) ONE box per tile -- 1-D taps (-d,0,+d), d <= 64: (128+2d) rows;
-//               3x3: (th+2) x tw rows from (w0-1, h0-1) -- every tap is a row-shifted descriptor view
-//               of it (the MMA unit swizzles on absolute smem address bits, base_offset stays 0).
-//     multi-box (1-D, large dilation) one aligned 128-row box per tap, all on one stage / barrier.
-//   Weights are TMA boxes [Ntile][KC]; if all taps fit (<= 100 KB, one N tile) they stay resident.
-// * Persistent CTAs (one per SM), static round-robin tiles (division-free digit iterator), roles:
-//     warp 0   TMA producer  } warp-uniform loops, elect.sync around the issue instructions so that
-//     warp 1   MMA issuer    } descriptors live in uniform registers (no R2UR waterfalls)
-//     warp 2-9 epilogue (sub-partition = warp%4; column chunks split even/odd between the pair):
-//              TMA-staged for plain stride-1 outputs (residual tile in by TMA, fp32 result written back
-//              in place + activated bf16 operand tile, TMA stores), direct 16-byte stores otherwise;
-//              optional per-channel affine before the activation (fused eval-mode BatchNorm).
-//   smem ring of up to 24 stages (full/empty mbarriers), up to 8 TMEM accumulator stages (512 columns /
-//   Ntile; tmem_full/empty).
-// * Diagnostics: VFX_TC_DEBUG=1 prints per-role cycle counters (time in each wait / issue section) for
-//   three CTAs after every launch; VFX_NO_HALO / VFX_NO_TMA_EPI disable the respective paths.
-#include <cuda.h>
-#include <stdlib.h>
-#include <vector>
-#include "vfx_common.cuh"
+// A CTA computes a 128 x BN output tile with two warpgroups (64 rows each, one m64nBN wgmma accumulator in
+// registers).  The K loop runs over (tap, 128-byte channel slice): every thread stages 16-byte chunks of the
+// shifted input rows and of the tap's weight rows with cp.async into a 4-stage ring of 128-byte-swizzled K-major
+// tiles; chunks outside the input (convolution padding), beyond Cin or beyond N are zero-filled by the copy itself,
+// so any tap offset, stride and edge is handled without a separate padded tensor.  kind tf32 reads fp32 operands and
+// ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the encoded stream of
+// vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.  The epilogue (bias, fp32
+// residual, eval-BN affine, activation, operand for the next layer) works on the accumulator registers directly.
 #include "tc_ptx.cuh"
+#include "wgmma_ptx.cuh"
 
 namespace vfx {
 
 namespace {
 
-constexpr int TILE_M = 128;
-constexpr int MAX_EPI_WARPS = 8;          // launch-time choice (TcParams.epi_warps): 4 = one per TMEM sub-partition (default),
-                                          // 8 = two per sub-partition, interleaved over even / odd column chunks
-constexpr int NUM_THREADS = 64 + 32 * MAX_EPI_WARPS;     // upper bound (launch bounds); the launch uses 64 + 32 * epi_warps
-constexpr int SMEM_BUDGET = 216 * 1024;                   // weights + stages + epilogue staging (227 KB max incl. barriers/alignment)
-constexpr int MAX_STAGES = 24;
-constexpr int BIAS_SMEM_FLOATS = 2048;                   // TMA epilogue: max N whose bias / affine arrays are kept in smem
+constexpr int BM = 128, NT = 256, STAGES = 4;
+constexpr int A_BYTES = BM * 128;
 
-struct TcParams {
-  // tile schedule
-  int B, Hq, Wq, tw_log2, th, n_tw, n_th, n_nt, Ntile, KC, n_kc, ntaps, stages;
-  uint32_t total_tiles;
-  int dh[9], dw[9];
-  int w_row[9];             // first weight row of each tap (w_off / Cin)
-  // output mapping
-  int sh, rh, sw, rw, OH, OW, N;
-  float* out_raw; long long o_sB, o_sH, o_sW; int o_col;
-  __nv_bfloat16* out_act; long long oa_sB, oa_sH, oa_sW; int oa_col;
-  const float* bias; int bias_mod;
-  const float* residual; long long r_sB, r_sH, r_sW; int r_col;
-  int act; float act_param;
-  const float* act_scale; const float* act_shift;   // optional affine before the activation of out_act
-  uint32_t idesc;           // tcgen05 instruction descriptor
-  uint32_t a_stage_bytes, b_stage_bytes;
-  uint32_t row_bytes;       // bytes of one K-chunk row: KC * element size (128, or 64 for bf16 KC = 32)
-  uint32_t at_bytes;        // TMA epilogue: bytes of one activated-operand staging tile (32 rows x 32 columns)
-  uint32_t res_enc, raw_enc;           // encoded tf32 stream (vfx_conv_desc): decode the residual / encode the raw output
-  float enc_slope, enc_inv_slope;
-  uint32_t epi_warps;       // epilogue warps: 4 or 8 (the column chunks of a tile are dealt round-robin over epi_warps / 4 warps)
-  uint32_t stag_warps;      // ... of which own TMA-epilogue staging (8 warps at Ntile = 32: the odd-chunk warps idle)
-  uint32_t ro_slots;        // TMA epilogue: residual / raw staging ring per warp (2 or 4 tiles of 4 KB), prefetched ro_slots - 1 chunks ahead
-  uint32_t at_double;       // ... double-buffered (bf16) or single (tf32: see the wait before it is rewritten)
-  uint32_t sbo16;           // stride-byte-offset >> 4 of the K-major swizzled layout (8 rows)
-  uint32_t layout_type;     // 2 = SWIZZLE_128B, 4 = SWIZZLE_64B
-  uint32_t tmem_cols;
-  uint32_t w_resident;      // all taps' weights stay in smem for the CTA's lifetime (single N tile)
-  uint32_t w_bytes;         // bytes of the resident weight region (0 if streamed)
-  uint32_t tma_epi;         // plain (stride-1) conv: residual in / raw+operand out through TMA-staged tiles
-  uint32_t epi_arrivals;    // threads arriving on tmem_empty
-  uint32_t epi_warp_bytes, epi_at_off;   // TMA epilogue: per-warp staging bytes, offset of the bf16 tiles
-  uint32_t bias_floats;     // TMA epilogue: floats per smem array (bias, act_scale, act_shift), N rounded up
-  uint32_t nacc;            // TMEM accumulator stages (2..8): depth of the MMA <-> epilogue pipeline
-  int d_nt, d_iw, d_ih, d_b; // mixed-radix digits of gridDim.x in (n_nt, n_tw, n_th, B): per-iteration tile increment
-  uint32_t halo;            // ONE box per tile, taps = row-shifted views of it: 1-D taps (-d,0,+d) with d <= 64
-                            // [(128+2d) rows], or 3x3 [(th+2) x tw rows starting at (w0-1, h0-1)]
-  uint32_t halo_boxes;                 // 1 = one halo box per K chunk; ntaps = one 128-row box per tap (multi-box tile stage)
-  uint32_t halo_rows, halo_kc_bytes;   // rows of the TMA box, bytes of one K-chunk block (rows rounded up + zero pad rows)
-  uint32_t halo_nps;                   // K chunks per pipeline stage in halo mode: n_kc (a tile = one stage), or 1 when only
-                                       // single-chunk stages leave room for two of them (tf32 C = 64 with three tap boxes)
-  int halo_pw, halo_ph;                // the box starts at (w0 - pw, h0 - ph)
-  uint32_t halo_off[9];                // row offset of each tap's 128-row view inside the box
-  uint32_t jtiles;          // tiles whose k-steps are interleaved (independent accumulators hide MMA latency)
-  long long* dbg;           // optional per-CTA role counters (VFX_TC_DEBUG)
-  int bw_log2;              // TMA epilogue: a warp's 32 rows form a (32/bw) x bw sub-patch, bw = min(tw, 32)
-};
+template <int KIND> struct OpT;
+template <> struct OpT<0> { using T = tf32_t; static constexpr int ESZ = 4; };
+template <> struct OpT<1> { using T = __nv_bfloat16; static constexpr int ESZ = 2; };
+template <> struct OpT<2> { using T = __half; static constexpr int ESZ = 2; };
 
-struct TileCoord { int b, h0, w0, n0; };
-// Tile iterator of a persistent CTA: tile(i) = blockIdx.x + i * gridDim.x.  One real decode (integer
-// divisions are ~250-cycle dependent chains in a lone warp) and then carry-propagating digit adds.
-struct TileIter {
-  int b, ih, iw, nt;
-  __device__ __forceinline__ void init(const TcParams& p, uint32_t tile) {
-    nt = (int)(tile % (uint32_t)p.n_nt);
-    uint32_t m = tile / (uint32_t)p.n_nt;
-    iw = (int)(m % (uint32_t)p.n_tw); m /= (uint32_t)p.n_tw;
-    ih = (int)(m % (uint32_t)p.n_th);
-    b = (int)(m / (uint32_t)p.n_th);
-  }
-  __device__ __forceinline__ void next(const TcParams& p) {
-    nt += p.d_nt; int c = nt >= p.n_nt; nt -= c ? p.n_nt : 0;
-    iw += p.d_iw + c; c = iw >= p.n_tw; iw -= c ? p.n_tw : 0;
-    ih += p.d_ih + c; c = ih >= p.n_th; ih -= c ? p.n_th : 0;
-    b += p.d_b + c;
-  }
-  __device__ __forceinline__ TileCoord coord(const TcParams& p) const {
-    TileCoord t; t.b = b; t.h0 = ih * p.th; t.w0 = iw << p.tw_log2; t.n0 = nt * p.Ntile; return t;
-  }
-};
+template <int BN> constexpr int smem_bytes() { return STAGES * (A_BYTES + BN * 128) + 1024; }
 
-template <int ACT, bool TF32, bool FP16>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-                    const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO,
-                    const __grid_constant__ CUtensorMap tmT, const __grid_constant__ TcParams p) {
+template <int BN, int KIND>
+__global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d, const int nkc) {
+  using T = typename OpT<KIND>::T;
+  constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
+  constexpr int STAGE = A_BYTES + BN * 128;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  // [resident weights | S stages of (A [+ W]) | epilogue staging (TMA epilogue) | barriers]
-  uint8_t* wres = smem;
-  smem += p.w_bytes;
-  const uint32_t stage_bytes = p.halo ? p.halo_kc_bytes * p.halo_nps : p.a_stage_bytes + (p.w_resident ? 0u : p.b_stage_bytes);
-  uint8_t* staging = smem + (size_t)p.stages * stage_bytes;
-  float* bias_s = reinterpret_cast<float*>(staging + (p.tma_epi ? p.stag_warps * p.epi_warp_bytes : 0));
-  float* asc_s = bias_s + p.bias_floats;                // act_scale / act_shift copies (TMA epilogue)
-  float* ash_s = asc_s + p.bias_floats;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + (p.tma_epi ? 3 * p.bias_floats : 0));
-  uint64_t* full = bars;
-  uint64_t* empty = bars + p.stages;
-  uint64_t* tmem_full = bars + 2 * p.stages;
-  uint64_t* tmem_empty = tmem_full + 8;
-  uint64_t* wfull = tmem_empty + 8;
-  uint64_t* res_full = wfull + 1;                       // [epilogue warp][ring slot]: 8 x 2 or 4 x 4
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 16);
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x;
+  const long long M = (long long)d.B * d.Hq * d.Wq;
+  const long long m0 = (long long)blockIdx.x * BM;
+  const int n0 = blockIdx.y * BN;
+  const char* __restrict__ A = reinterpret_cast<const char*>(d.a);
+  const char* __restrict__ Wt = reinterpret_cast<const char*>(d.w);
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 8; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], p.epi_arrivals); }
-    mbar_init(wfull, 1);
-    for (int i = 0; i < 16; ++i) mbar_init(&res_full[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {   // TMEM allocation (whole warp), address published through smem
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (p.tma_epi)
-    for (int i = threadIdx.x; i < p.N; i += blockDim.x) {
-      bias_s[i] = p.bias ? p.bias[i % p.bias_mod] : 0.f;
-      asc_s[i] = p.act_scale ? p.act_scale[i] : 1.f;
-      ash_s[i] = p.act_scale ? p.act_shift[i] : 0.f;
-    }
-  if (p.halo) {   // rows behind the TMA box (read by the last taps' views, never written by TMA) must be zero
-    const uint32_t row_b = p.row_bytes, used = p.halo_rows * row_b, blk = p.halo_kc_bytes;
-    const uint32_t nblk = (uint32_t)p.stages * p.halo_nps, padw = (blk - used) / 4;
-    if (padw)
-      for (uint32_t i = threadIdx.x; i < nblk * padw; i += blockDim.x)
-        reinterpret_cast<uint32_t*>(smem + (size_t)(i / padw) * blk + used)[i % padw] = 0u;
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int k_steps = p.ntaps * p.n_kc;
-
-  if (warp == 0) {
-    // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
-    {
-      if (p.w_resident && elect_one()) {   // every tap's [N][Cin] matrix once, as [tap][kc] blocks of [Ntile][KC]
-        mbar_expect_tx(wfull, p.w_bytes);
-#pragma unroll 1
-        for (int tap = 0; tap < p.ntaps; ++tap)
-#pragma unroll 1
-          for (int kc = 0; kc < p.n_kc; ++kc)
-            tma_load_2d(&tmW, wfull, wres + (size_t)(tap * p.n_kc + kc) * p.b_stage_bytes, kc * p.KC, p.w_row[tap]);
-      }
-      __syncwarp();
-      uint32_t s = 0, ph = 0;
-      const bool dbg = p.dbg != nullptr;
-      long long w_empty = 0; const long long tstart = dbg ? clock64() : 0;
-      // tiles of this CTA: tile(i) = blockIdx.x + i * gridDim.x; groups of J tiles advance through their
-      // k-steps together: (tile 0, ks 0), (tile 1, ks 0), ..., (tile 0, ks 1), ...
-      const uint32_t n_my = blockIdx.x < p.total_tiles ? (p.total_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-      uint32_t n_done = 0;
-      TileIter pit; pit.init(p, blockIdx.x);
-      if (p.halo) {
-        for (uint32_t i = 0; i < n_my; ++i) {
-          const TileCoord t = pit.coord(p);
-          pit.next(p);
-#pragma unroll 1
-          for (int kc0 = 0; kc0 < p.n_kc; kc0 += (int)p.halo_nps) {
-            mbar_wait_t(&empty[s], ph ^ 1, w_empty, dbg);
-            uint8_t* sa = smem + (size_t)s * stage_bytes;
-            if (elect_one()) {
-              mbar_expect_tx(&full[s], p.halo_rows * p.row_bytes * p.halo_nps * p.halo_boxes);
-#pragma unroll 1
-              for (int kc = kc0; kc < kc0 + (int)p.halo_nps; ++kc) {
-                uint8_t* const blk = sa + (size_t)(kc - kc0) * p.halo_kc_bytes;
-                if (p.halo_boxes == 1) {
-                  tma_load_4d(&tmA, &full[s], blk, kc * p.KC, t.w0 - p.halo_pw, t.h0 - p.halo_ph, t.b);
-                } else {      // one aligned 128-row box per tap, all on this stage's barrier
-#pragma unroll 1
-                  for (int tap = 0; tap < p.ntaps; ++tap)
-                    tma_load_4d(&tmA, &full[s], blk + (size_t)p.halo_off[tap] * p.row_bytes, kc * p.KC,
-                                t.w0 + p.dw[tap], t.h0 + p.dh[tap], t.b);
-                }
-              }
-            }
-            __syncwarp();
-            if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
-          }
-        }
-        n_done = n_my;
-      }
-      for (uint32_t i0 = n_done; i0 < n_my; i0 += p.jtiles) {
-        const uint32_t jn = (n_my - i0) < p.jtiles ? (n_my - i0) : p.jtiles;
-        TileCoord tc[4];
+  // ---- this thread's staging work: chunk `chunk` of A rows lrow + 32 i and of B rows lrow + 32 i
+  const int chunk = tid & 7, lrow = tid >> 3;
+  int rb[4], rh[4], rw[4];
 #pragma unroll
-        for (uint32_t j = 0; j < 4; ++j) {
-          tc[j] = pit.coord(p);
-          if (j < jn) pit.next(p);
-        }
-#pragma unroll 1
-        for (int tap = 0; tap < p.ntaps; ++tap) {
-#pragma unroll 1
-          for (int kc = 0; kc < p.n_kc; ++kc) {
-#pragma unroll
-            for (uint32_t j = 0; j < 4; ++j) {
-              if (j < jn) {
-                mbar_wait_t(&empty[s], ph ^ 1, w_empty, dbg);
-                uint8_t* sa = smem + (size_t)s * stage_bytes;
-                if (elect_one()) {
-                  mbar_expect_tx(&full[s], stage_bytes);
-                  tma_load_4d(&tmA, &full[s], sa, kc * p.KC, tc[j].w0 + p.dw[tap], tc[j].h0 + p.dh[tap], tc[j].b);
-                  if (!p.w_resident) tma_load_2d(&tmW, &full[s], sa + p.a_stage_bytes, kc * p.KC, p.w_row[tap] + tc[j].n0);
-                }
-                __syncwarp();
-                if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
-              }
-            }
-          }
-        }
-      }
-      if (dbg && lane == 0) { long long* o = p.dbg + (long long)blockIdx.x * 64; o[0] = clock64() - tstart; o[1] = w_empty; }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      uint32_t s = 0, ph = 0;
-      const int kk = (int)(p.row_bytes / 32);         // MMAs per K chunk: UMMA_K = 16 bf16 / 8 tf32 elements = 32 bytes
-      if (p.w_resident) { mbar_wait(wfull, 0); tc_fence_after(); }
-      const bool dbg = p.dbg != nullptr;
-      long long w_full = 0, w_te = 0, w_mma = 0, w_cm = 0, w_cm2 = 0; const long long tstart = dbg ? clock64() : 0;
-      const uint32_t n_my = blockIdx.x < p.total_tiles ? (p.total_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-      const uint32_t nacc_mask = p.nacc - 1, nacc_log2 = 31 - __clz(p.nacc);
-      uint32_t n_done = 0;
-      if (p.halo) {
-        for (uint32_t i = 0; i < n_my; ++i) {
-          mbar_wait_t(&tmem_empty[i & nacc_mask], ((i >> nacc_log2) & 1) ^ 1, w_te, dbg);
-          const uint32_t d_tmem = tmem_base + (i & nacc_mask) * p.Ntile;
-          const uint32_t w_addr = smem_u32(wres);
-          const uint32_t dhi = desc_hi(p.sbo16, p.layout_type);
-#pragma unroll 1
-          for (int kc0 = 0; kc0 < p.n_kc; kc0 += (int)p.halo_nps) {
-            mbar_wait_t(&full[s], ph, w_full, dbg);
-            tc_fence_after();
-            const uint32_t s_addr = smem_u32(smem + (size_t)s * stage_bytes);
-            if (elect_one()) {
-              // ntaps is 3 (1-D) or 9 (3x3): bodies of 3 taps x kk MMAs are unrolled so that the descriptor
-              // arithmetic and the moves into uniform registers of several MMAs overlap (a fully rolled loop
-              // serialised ~200 cycles per MMA and made this warp the bottleneck of the N=32 UNet layers)
-#pragma unroll 1
-              for (int tap0 = 0; tap0 < p.ntaps; tap0 += 3) {
-#pragma unroll 1
-                for (int kc = kc0; kc < kc0 + (int)p.halo_nps; ++kc) {
-                  uint32_t a_lo[3], b_lo[3];
-#pragma unroll
-                  for (int dt = 0; dt < 3; ++dt) {
-                    a_lo[dt] = desc_lo(s_addr + (uint32_t)(kc - kc0) * p.halo_kc_bytes + p.halo_off[tap0 + dt] * p.row_bytes);
-                    b_lo[dt] = desc_lo(w_addr + (uint32_t)((tap0 + dt) * p.n_kc + kc) * p.b_stage_bytes);
-                  }
-                  if ((tap0 | kc) == 0) tc_mma_lo<false, TF32>(d_tmem, a_lo[0], b_lo[0], dhi, p.idesc);   // first MMA of the tile overwrites
-                  else tc_mma_lo<true, TF32>(d_tmem, a_lo[0], b_lo[0], dhi, p.idesc);
-                  if (kk == 4) {
-#pragma unroll
-                    for (int k = 1; k < 4; ++k) tc_mma_lo<true, TF32>(d_tmem, a_lo[0] + 2 * k, b_lo[0] + 2 * k, dhi, p.idesc);
-#pragma unroll
-                    for (int dt = 1; dt < 3; ++dt)
-#pragma unroll
-                      for (int k = 0; k < 4; ++k) tc_mma_lo<true, TF32>(d_tmem, a_lo[dt] + 2 * k, b_lo[dt] + 2 * k, dhi, p.idesc);
-                  } else {
-                    tc_mma_lo<true, TF32>(d_tmem, a_lo[0] + 2, b_lo[0] + 2, dhi, p.idesc);
-#pragma unroll
-                    for (int dt = 1; dt < 3; ++dt)
-#pragma unroll
-                      for (int k = 0; k < 2; ++k) tc_mma_lo<true, TF32>(d_tmem, a_lo[dt] + 2 * k, b_lo[dt] + 2 * k, dhi, p.idesc);
-                  }
-                }
-              }
-              tc_commit(&empty[s]);
-              if (kc0 + (int)p.halo_nps >= p.n_kc) tc_commit(&tmem_full[i & nacc_mask]);
-            }
-            __syncwarp();
-            if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
-          }
-        }
-        n_done = n_my;
-      }
-      for (uint32_t i0 = n_done; i0 < n_my; i0 += p.jtiles) {
-        const uint32_t jn = (n_my - i0) < p.jtiles ? (n_my - i0) : p.jtiles;
-        for (uint32_t j = 0; j < jn; ++j) {            // accumulators of the whole group must be drained
-          const uint32_t i = i0 + j;
-          mbar_wait_t(&tmem_empty[i & nacc_mask], ((i >> nacc_log2) & 1) ^ 1, w_te, dbg);
-        }
-        tc_fence_after();
-#pragma unroll 1
-        for (int ks = 0; ks < k_steps; ++ks) {
-          for (uint32_t j = 0; j < jn; ++j) {
-            const uint32_t d_tmem = tmem_base + ((i0 + j) & nacc_mask) * p.Ntile;
-            mbar_wait_t(&full[s], ph, w_full, dbg);
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(smem + (size_t)s * stage_bytes);
-            const uint32_t b_addr = p.w_resident ? smem_u32(wres + (size_t)ks * p.b_stage_bytes) : a_addr + p.a_stage_bytes;
-            const long long tm0 = dbg ? clock64() : 0;
-            if (elect_one()) {
-              const uint32_t ghi = desc_hi(p.sbo16, p.layout_type), ga = desc_lo(a_addr), gb = desc_lo(b_addr);
-              if (ks == 0) tc_mma_lo<false, TF32>(d_tmem, ga, gb, ghi, p.idesc);
-              else tc_mma_lo<true, TF32>(d_tmem, ga, gb, ghi, p.idesc);
-              tc_mma_lo<true, TF32>(d_tmem, ga + 2, gb + 2, ghi, p.idesc);
-              if (kk == 4) {
-                tc_mma_lo<true, TF32>(d_tmem, ga + 4, gb + 4, ghi, p.idesc);
-                tc_mma_lo<true, TF32>(d_tmem, ga + 6, gb + 6, ghi, p.idesc);
-              }
-              tc_commit(&empty[s]);                   // frees the smem stage when these MMAs retire
-              if (ks == k_steps - 1) tc_commit(&tmem_full[(i0 + j) & nacc_mask]);   // accumulator ready for the epilogue
-            }
-            __syncwarp();
-            if (dbg) w_mma += clock64() - tm0;
-            if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
-          }
-        }
-      }
-      if (dbg && lane == 0) { long long* o = p.dbg + (long long)blockIdx.x * 64 + 8; o[0] = clock64() - tstart; o[1] = w_full; o[2] = w_te; o[3] = w_mma; o[4] = w_cm; o[5] = w_cm2; }
-    }
-  } else if (p.tma_epi) {
-    // ===================== TMA-staged epilogue (plain stride-1 convs) =====================
-    // Warp (sub = warp%4, half = (warp-2)/4) owns accumulator rows [32 sub, 32 sub + 32) = a (32/bw) x bw sub-patch and
-    // the 32-column chunks c = half, half + cs, ... (cs = epi_warps / 4).  It walks its chunk stream n = 0, 1, ... across
-    // tiles.  Per chunk: the fp32 residual tile arrives by TMA in a SWIZZLE_128B staging tile of a ring of R slots,
-    // prefetched R - 1 chunks ahead (R = 4 with 4 warps: a DRAM round trip is longer than one chunk's work -- the fused
-    // pair kernel went from 4.4 to 6.4 TB/s with exactly this change; R = 2 is round 1's scheme); the thread owning a row
-    // reads its 128 B, adds accumulator + bias (smem copy), writes the fp32 result back IN PLACE and the activated operand
-    // into its own tile; one lane issues the TMA stores (full lines, asynchronous, clipped by the tensor map).  Slot
-    // (n + R - 1) % R = (n - 1) % R is free again once the store group of chunk n - 1 has been read out.
-    const int ew = warp - 2, sub = warp & 3, half = ew >> 2;
-    const int cs = (int)(p.epi_warps >> 2);
-    const uint32_t rmask = p.ro_slots - 1;
-    uint8_t* const stg = staging + ew * p.epi_warp_bytes;      // [RO ring (4 KB each, optional)] [AT (1 or 2 tiles)]
-    uint8_t* const at_base = stg + p.epi_at_off;
-    uint64_t* const rfull = res_full + ew * p.ro_slots;
-    const bool has_res = p.residual != nullptr;
-    const int r0 = sub * 32;
-    const int dh0 = r0 >> p.tw_log2, dw0 = r0 & ((1 << p.tw_log2) - 1);
-    const int nch = p.Ntile >> 5;
-    uint32_t n = 0, rph = 0, acc = 0, acc_ph = 0;               // n: chunk counter of this warp; rph bit b = phase of rfull[b]
-    TileIter eit; eit.init(p, blockIdx.x);
-    TileIter pit; pit.init(p, blockIdx.x);                      // prefetch stream: tile and chunk of the next residual to request
-    int pc = half;
-    uint32_t pn = 0;
-    const uint32_t n_my_e = blockIdx.x < p.total_tiles ? (p.total_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    const uint32_t n_chunks = half < nch ? n_my_e * (uint32_t)((nch - half + cs - 1) / cs) : 0u;
-#pragma unroll 1
-    for (; pn + 1 < p.ro_slots && pn < n_chunks; ++pn) {        // bookkeeping is warp-uniform, lane 0 issues
-      if (has_res && lane == 0) {
-        const TileCoord t = pit.coord(p);
-        mbar_expect_tx(&rfull[pn & rmask], 4096);
-        tma_load_4d(&tmR, &rfull[pn & rmask], stg + (pn & rmask) * 4096, p.r_col + t.n0 + pc * 32, t.w0 + dw0, t.h0 + dh0, t.b);
-      }
-      pc += cs;
-      if (pc >= nch) { pc = half; pit.next(p); }
-    }
-    const uint32_t sw128 = (uint32_t)(lane & 7) << 4, sw64 = (uint32_t)((lane >> 1) & 3) << 4;
-    const bool dbg = p.dbg != nullptr;
-    long long w_tf = 0, w_rf = 0, w_wg = 0, w_ld = 0, w_math = 0, w_fence = 0, w_issue = 0, w_dec = 0; const long long tstart = dbg ? clock64() : 0;
-    for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const long long td0 = dbg ? clock64() : 0;
-      const TileCoord t = eit.coord(p);
-      eit.next(p);
-      if (dbg) w_dec += clock64() - td0;
-      mbar_wait_t(&tmem_full[acc], acc_ph, w_tf, dbg);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(sub * 32) << 16) + acc * p.Ntile;
-#pragma unroll 1
-      for (int c = half; c < nch; c += cs, ++n) {
-        const int col = t.n0 + c * 32;
-        const uint32_t slot = n & rmask, k = n & 1u;
-        uint32_t bcol = (uint32_t)col;                    // bias_s is pre-tiled over the N columns
-        uint8_t* const ro = stg + slot * 4096 + lane * 128;
-        if (has_res) { mbar_wait_t(&rfull[slot], (rph >> slot) & 1, w_rf, dbg); rph ^= 1u << slot; }
-        uint32_t v[32];
-        { const long long t0 = dbg ? clock64() : 0; tc_ld32(t_row + c * 32, v); if (dbg) w_ld += clock64() - t0; }
-        const long long tq0 = dbg ? clock64() : 0;
-        float f[32];
-        {
-          const float4* bp = reinterpret_cast<const float4*>(bias_s + bcol);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b4 = bp[j];
-            f[4 * j] = __uint_as_float(v[4 * j]) + b4.x; f[4 * j + 1] = __uint_as_float(v[4 * j + 1]) + b4.y;
-            f[4 * j + 2] = __uint_as_float(v[4 * j + 2]) + b4.z; f[4 * j + 3] = __uint_as_float(v[4 * j + 3]) + b4.w;
-          }
-        }
-        if (has_res) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 r4 = *reinterpret_cast<const float4*>(ro + ((uint32_t)(j << 4) ^ sw128));
-            if (p.res_enc) {
-              r4.x = stream_dec(r4.x, p.enc_inv_slope); r4.y = stream_dec(r4.y, p.enc_inv_slope);
-              r4.z = stream_dec(r4.z, p.enc_inv_slope); r4.w = stream_dec(r4.w, p.enc_inv_slope);
-            }
-            f[4 * j] += r4.x; f[4 * j + 1] += r4.y; f[4 * j + 2] += r4.z; f[4 * j + 3] += r4.w;
-          }
-        }
-        if (p.out_raw) {
-          if (p.raw_enc) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(ro + ((uint32_t)(j << 4) ^ sw128)) =
-                  make_float4(stream_enc(f[4 * j], p.enc_slope), stream_enc(f[4 * j + 1], p.enc_slope),
-                              stream_enc(f[4 * j + 2], p.enc_slope), stream_enc(f[4 * j + 3], p.enc_slope));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(ro + ((uint32_t)(j << 4) ^ sw128)) = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-          }
-        }
-        if (p.out_act) {
-          uint8_t* const at_tile = at_base + (p.at_double ? k * p.at_bytes : 0u);
-          if (!p.at_double) {     // single staging tile: the store that read it (issued one chunk ago) must have drained
-            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            __syncwarp();
-          }
-          if (p.act_scale) {                          // fused eval-mode BatchNorm of the consumer
-            const float4* sp = reinterpret_cast<const float4*>(asc_s + bcol);
-            const float4* tp = reinterpret_cast<const float4*>(ash_s + bcol);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 s4 = sp[j], t4 = tp[j];
-              f[4 * j] = fmaf(f[4 * j], s4.x, t4.x); f[4 * j + 1] = fmaf(f[4 * j + 1], s4.y, t4.y);
-              f[4 * j + 2] = fmaf(f[4 * j + 2], s4.z, t4.z); f[4 * j + 3] = fmaf(f[4 * j + 3], s4.w, t4.w);
-            }
-          }
-          if (TF32) {             // fp32 storage, values rounded to tf32: a SWIZZLE_128B tile like the raw one
-            uint8_t* const at = at_tile + lane * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(at + ((uint32_t)(j << 4) ^ sw128)) =
-                  make_float4(round_tf32(act_fast<ACT>(f[4 * j], p.act_param)), round_tf32(act_fast<ACT>(f[4 * j + 1], p.act_param)),
-                              round_tf32(act_fast<ACT>(f[4 * j + 2], p.act_param)), round_tf32(act_fast<ACT>(f[4 * j + 3], p.act_param)));
-          } else {
-            uint8_t* const at = at_tile + lane * 64;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint32_t w[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q)
-                w[q] = pack16<FP16>(act_fast<ACT>(f[8 * j + 2 * q], p.act_param), act_fast<ACT>(f[8 * j + 2 * q + 1], p.act_param));
-              *reinterpret_cast<uint4*>(at + ((uint32_t)(j << 4) ^ sw64)) = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-          }
-        }
-        const long long tq1 = dbg ? clock64() : 0;
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        const long long tq2 = dbg ? clock64() : 0;
-        if (dbg) { w_math += tq1 - tq0; w_fence += tq2 - tq1; }
-        if (lane == 0) {
-          if (p.out_raw) tma_store_4d(&tmO, stg + slot * 4096, p.o_col + col, t.w0 + dw0, t.h0 + dh0, t.b);
-          if (p.out_act) tma_store_4d(&tmT, at_base + (p.at_double ? k * p.at_bytes : 0u), p.oa_col + col, t.w0 + dw0, t.h0 + dh0, t.b);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          { const long long t0 = dbg ? clock64() : 0;
-            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // the stores of chunk n-1 have left their buffers
-            if (dbg) w_wg += clock64() - t0; }
-          if (has_res && pn < n_chunks) {     // residual of chunk n + R - 1 -> the slot chunk n - 1 used
-            const TileCoord tp = pit.coord(p);
-            mbar_expect_tx(&rfull[pn & rmask], 4096);
-            tma_load_4d(&tmR, &rfull[pn & rmask], stg + (pn & rmask) * 4096, p.r_col + tp.n0 + pc * 32, tp.w0 + dw0, tp.h0 + dh0, tp.b);
-          }
-        }
-        if (pn < n_chunks) {                  // warp-uniform bookkeeping of the prefetch stream
-          ++pn; pc += cs;
-          if (pc >= nch) { pc = half; pit.next(p); }
-        }
-        __syncwarp();
-        if (dbg) w_issue += clock64() - tq2;
-      }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
-      if (++acc == p.nacc) { acc = 0; acc_ph ^= 1; }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (dbg && lane == 0) {
-      long long* o = p.dbg + (long long)blockIdx.x * 64 + 16 + ew * 6;
-      o[0] = clock64() - tstart; o[1] = w_tf; o[2] = w_rf; o[3] = w_wg; o[4] = w_ld;
-      if (ew == 0) { long long* q = p.dbg + (long long)blockIdx.x * 64 + 56; q[0] = w_math; q[1] = w_fence; q[2] = w_issue; q[3] = w_dec; }
-    }
-  } else {
-    // ===================== direct epilogue (4 or 8 warps over 128 TMEM lanes) =====================
-    const int sub = warp & 3;                         // TMEM sub-partition this warp may access
-    const int half = (warp - 2) >> 2;                 // 8 warps: 0/1 = even / odd column chunks; 4 warps: 0, every chunk
-    const int cstep = 32 * (int)(p.epi_warps >> 2);
-    const int row = sub * 32 + lane;                  // accumulator row = position inside the patch
-    uint32_t acc = 0, acc_ph = 0;
-    TileIter dit; dit.init(p, blockIdx.x);
-    for (uint32_t tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const TileCoord t = dit.coord(p);
-      dit.next(p);
-      const int qh = t.h0 + (row >> p.tw_log2), qw = t.w0 + (row & ((1 << p.tw_log2) - 1));
-      const int oh = qh * p.sh + p.rh, ow = qw * p.sw + p.rw;
-      const bool valid = qh < p.Hq && qw < p.Wq && oh < p.OH && ow < p.OW;
-      const long long off_r = (long long)t.b * p.r_sB + (long long)oh * p.r_sH + (long long)ow * p.r_sW + p.r_col + t.n0;
-      const long long off_o = (long long)t.b * p.o_sB + (long long)oh * p.o_sH + (long long)ow * p.o_sW + p.o_col + t.n0;
-      const long long off_a = (long long)t.b * p.oa_sB + (long long)oh * p.oa_sH + (long long)ow * p.oa_sW + p.oa_col + t.n0;
-      const bool has_res = p.residual != nullptr && valid;
-      // residual of this warp's first chunk: in flight while the MMAs of the tile finish
-      float4 rcur[8];
-      int c0 = half * 32;
-      if (has_res && c0 < p.Ntile) {
-        const float4* rp = reinterpret_cast<const float4*>(p.residual + off_r + c0);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) rcur[j] = __ldcs(rp + j);
-      }
-      mbar_wait(&tmem_full[acc], acc_ph);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(sub * 32) << 16) + acc * p.Ntile;
-#pragma unroll 1
-      for (; c0 < p.Ntile; c0 += cstep) {
-        uint32_t v[32];
-        tc_ld32(t_row + c0, v);
-        float4 rnext[8];
-        const bool more = has_res && (c0 + cstep < p.Ntile);
-        if (more) {                                   // next chunk's residual: in flight during this chunk
-          const float4* rp = reinterpret_cast<const float4*>(p.residual + off_r + c0 + cstep);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) rnext[j] = __ldcs(rp + j);
-        }
-        if (valid) {
-          const int n = t.n0 + c0;
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (p.bias) {
-            const float4* bp = reinterpret_cast<const float4*>(p.bias + (n % p.bias_mod));
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 b4 = __ldg(bp + j);
-              f[4 * j] += b4.x; f[4 * j + 1] += b4.y; f[4 * j + 2] += b4.z; f[4 * j + 3] += b4.w;
-            }
-          }
-          if (has_res) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 r4 = rcur[j];
-              if (p.res_enc) {
-                r4.x = stream_dec(r4.x, p.enc_inv_slope); r4.y = stream_dec(r4.y, p.enc_inv_slope);
-                r4.z = stream_dec(r4.z, p.enc_inv_slope); r4.w = stream_dec(r4.w, p.enc_inv_slope);
-              }
-              f[4 * j] += r4.x; f[4 * j + 1] += r4.y; f[4 * j + 2] += r4.z; f[4 * j + 3] += r4.w;
-            }
-          }
-          if (p.out_raw) {
-            float4* op = reinterpret_cast<float4*>(p.out_raw + off_o + c0);
-            if (p.raw_enc) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                op[j] = make_float4(stream_enc(f[4 * j], p.enc_slope), stream_enc(f[4 * j + 1], p.enc_slope),
-                                    stream_enc(f[4 * j + 2], p.enc_slope), stream_enc(f[4 * j + 3], p.enc_slope));
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) op[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-            }
-          }
-          if (p.out_act) {
-            if (p.act_scale) {
-              const float4* sp = reinterpret_cast<const float4*>(p.act_scale + n);
-              const float4* tp = reinterpret_cast<const float4*>(p.act_shift + n);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 s4 = __ldg(sp + j), t4 = __ldg(tp + j);
-                f[4 * j] = fmaf(f[4 * j], s4.x, t4.x); f[4 * j + 1] = fmaf(f[4 * j + 1], s4.y, t4.y);
-                f[4 * j + 2] = fmaf(f[4 * j + 2], s4.z, t4.z); f[4 * j + 3] = fmaf(f[4 * j + 3], s4.w, t4.w);
-              }
-            }
-            if (TF32) {
-              float4* ap = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out_act) + off_a + c0);
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                ap[j] = make_float4(round_tf32(act_fast<ACT>(f[4 * j], p.act_param)), round_tf32(act_fast<ACT>(f[4 * j + 1], p.act_param)),
-                                    round_tf32(act_fast<ACT>(f[4 * j + 2], p.act_param)), round_tf32(act_fast<ACT>(f[4 * j + 3], p.act_param)));
-            } else {
-              uint4* ap = reinterpret_cast<uint4*>(p.out_act + off_a + c0);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                uint32_t w[4];
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  w[q] = pack16<FP16>(act_fast<ACT>(f[8 * j + 2 * q], p.act_param), act_fast<ACT>(f[8 * j + 2 * q + 1], p.act_param));
-                ap[j] = make_uint4(w[0], w[1], w[2], w[3]);
-              }
-            }
-          }
-        }
-        if (more) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
-      if (++acc == p.nacc) { acc = 0; acc_ph ^= 1; }
+  for (int i = 0; i < 4; ++i) {
+    const long long m = m0 + lrow + 32 * i;
+    if (m < M) {
+      rw[i] = (int)(m % d.Wq);
+      const long long r = m / d.Wq;
+      rh[i] = (int)(r % d.Hq); rb[i] = (int)(r / d.Hq);
+    } else {
+      rb[i] = -1; rh[i] = 0; rw[i] = 0;
     }
   }
+  const int niter = d.ntaps * nkc;
+  auto load_stage = [&](int it, int s) {
+    const int tap = it / nkc;
+    const int c = (it - tap * nkc) * BK + chunk * AL;
+    const bool c_ok = c < d.Cin;
+    const uint32_t sa = sbase + s * STAGE, sb = sa + A_BYTES;
+    const int dh = d.dh[tap], dw = d.dw[tap];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = lrow + 32 * i;
+      const int ih = rh[i] + dh, iw = rw[i] + dw;
+      const bool ok = c_ok && rb[i] >= 0 && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W;
+      const char* src = ok ? A + ((long long)rb[i] * d.a_sB + (long long)ih * d.a_sH + (long long)iw * d.a_sW + c) * ESZ : A;
+      cp_async16(sa + sw128_offset(r, chunk), src, ok);
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 32; ++i) {
+      const int n = lrow + 32 * i;
+      const bool ok = c_ok && n0 + n < d.N;
+      const char* src = ok ? Wt + (d.w_off[tap] + (long long)(n0 + n) * d.Cin + c) * ESZ : Wt;
+      cp_async16(sb + sw128_offset(n, chunk), src, ok);
+    }
+  };
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  const int wg = tid >> 7;
+
+#pragma unroll
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < niter) load_stage(s, s);
+    cp_async_commit();
+  }
+  for (int it = 0; it < niter; ++it) {
+    cp_async_wait<STAGES - 2>();          // this thread's chunks of stage `it` have landed
+    fence_proxy_async();
+    __syncthreads();                      // ... everyone's, and stage it-1 is no longer read by either warpgroup
+    if (it + STAGES - 1 < niter) load_stage(it + STAGES - 1, (it + STAGES - 1) % STAGES);
+    cp_async_commit();
+    const uint32_t sa = sbase + (it % STAGES) * STAGE;
+    const uint64_t da = sw128_desc(sa + wg * 64 * 128), db = sw128_desc(sa + A_BYTES);
+    float part[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) Wgmma<BN, KIND>::mma(part, da + 2 * kk, db + 2 * kk);   // 32 bytes of K each
+    wgmma_commit();
+    wgmma_wait<0>();
+    // the tensor core's accumulator adds truncate; summing the K slices here rounds to nearest, so the error of
+    // long reductions (9 taps x 768 channels) does not build up as a bias
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+  }
+  cp_async_wait<0>();
+
+  // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of warpgroup wg is
+  //      row wg*64 + w*16 + l/4 + 8h, column 8j + 2(l%4) + e
+  const int w = (tid >> 5) & 3, l = tid & 31;
+  T* out_act = reinterpret_cast<T*>(d.out_act);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const long long m = m0 + wg * 64 + w * 16 + (l >> 2) + 8 * h;
+    if (m >= M) continue;
+    const int qw = (int)(m % d.Wq);
+    const long long r = m / d.Wq;
+    const int qh = (int)(r % d.Hq), b = (int)(r / d.Hq);
+    const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
+    if (oh >= d.OH || ow >= d.OW) continue;
+    const long long o_raw = (long long)b * d.o_sB + (long long)oh * d.o_sH + (long long)ow * d.o_sW + d.o_col;
+    const long long o_act = (long long)b * d.oa_sB + (long long)oh * d.oa_sH + (long long)ow * d.oa_sW + d.oa_col;
+    const long long o_res = (long long)b * d.r_sB + (long long)oh * d.r_sH + (long long)ow * d.r_sW + d.r_col;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = n0 + 8 * j + 2 * (l & 3) + e;
+        if (n >= d.N) continue;
+        float v = acc[4 * j + 2 * h + e];
+        if (d.bias) v += d.bias[n % d.bias_mod];
+        if (d.residual) {
+          const float rv = d.residual[o_res + n];
+          v += d.res_enc ? stream_dec(rv, 1.0f / d.enc_slope) : rv;
+        }
+        if (d.out_raw) d.out_raw[o_raw + n] = d.raw_enc ? stream_enc(v, d.enc_slope) : v;
+        if (out_act) {
+          const float va = d.act_scale ? fmaf(v, d.act_scale[n], d.act_shift[n]) : v;
+          out_act[o_act + n] = from_f<T>(apply_act(va, d.act, d.act_param));
+        }
+      }
   }
 }
 
-// ------------------------------------------------------------------ host side
-int ilog2(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
+template <int BN, int KIND>
+int launch(const vfx_conv_desc& d, cudaStream_t st) {
+  constexpr int smem = smem_bytes<BN>();
+  static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
+  int dev = 0;
+  VFX_CUDA_CHECK(cudaGetDevice(&dev));
+  if (dev >= 64 || !(attr_set >> dev & 1)) {
+    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    if (dev < 64) attr_set |= 1ull << dev;
+  }
+  const long long M = (long long)d.B * d.Hq * d.Wq;
+  const int nkc = ceil_div(d.Cin, 128 / OpT<KIND>::ESZ);
+  dim3 grid(ceil_div(M, BM), ceil_div(d.N, BN));
+  conv_gemm_wgmma_kernel<BN, KIND><<<grid, NT, smem, st>>>(d, nkc);
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+template <int KIND>
+int launch_kind(const vfx_conv_desc& d, cudaStream_t st) {
+  if (d.N <= 32) return launch<32, KIND>(d, st);
+  if (d.N <= 64) return launch<64, KIND>(d, st);
+  return launch<128, KIND>(d, st);
+}
 
 }  // namespace
 
-// conv_ts_tc.cu: tf32, k = 3, 128 -> 128 channels with the weights resident in tensor memory; VFX_ERR_UNSUPPORTED for anything else
-int conv_ts_tc(const vfx_conv_desc& d, cudaStream_t st);
-
 int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st) {
-  // ---- shapes this kernel covers; everything else returns UNSUPPORTED (caller uses the SIMT kernel)
+  // ---- shapes this kernel covers; everything else returns UNSUPPORTED (the engine then runs the SIMT kernel)
   if (precision != VFX_PREC_BF16 && precision != VFX_PREC_TF32 && precision != VFX_PREC_FP16) return VFX_ERR_UNSUPPORTED;
-  const bool tf32 = precision == VFX_PREC_TF32, fp16 = precision == VFX_PREC_FP16;
-  if (tf32) {                                    // width-128 k3 convolutions: weights resident in tensor memory (conv_ts_tc.cu)
-    const int r = conv_ts_tc(d, st);
-    if (r != VFX_ERR_UNSUPPORTED) return r;
-  }
-  const int esz = tf32 ? 4 : 2;
-  int KC = 0;
-  if (tf32) { if (d.Cin % 32 == 0) KC = 32; }
-  else if (d.Cin % 64 == 0) KC = 64; else if (d.Cin == 32) KC = 32;
-  if (!KC) return VFX_ERR_UNSUPPORTED;
-  const int al = 16 / esz;                 // elements per 16 bytes (TMA stride granularity)
-  int Ntile = 0;
-  for (int c : {256, 128, 64, 32}) if (d.N % c == 0) { Ntile = c; break; }
-  if (!Ntile) return VFX_ERR_UNSUPPORTED;
-  if (d.ntaps < 1 || d.ntaps > 9) return VFX_ERR_UNSUPPORTED;
-  if (d.a_sW % al || d.a_sH % al || d.a_sB % al || ((uintptr_t)d.a & 15) || ((uintptr_t)d.w & 15)) return VFX_ERR_UNSUPPORTED;
-  // epilogue vector alignment
-  if (d.out_raw && (d.o_sW % 4 || d.o_sH % 4 || d.o_sB % 4 || d.o_col % 4 || ((uintptr_t)d.out_raw & 15))) return VFX_ERR_UNSUPPORTED;
-  if (d.out_act && (d.oa_sW % al || d.oa_sH % al || d.oa_sB % al || d.oa_col % al || ((uintptr_t)d.out_act & 15))) return VFX_ERR_UNSUPPORTED;
-  if (d.residual && (d.r_sW % 4 || d.r_sH % 4 || d.r_sB % 4 || d.r_col % 4 || ((uintptr_t)d.residual & 15))) return VFX_ERR_UNSUPPORTED;
-  if (d.bias && (d.bias_mod % 32 || ((uintptr_t)d.bias & 15))) return VFX_ERR_UNSUPPORTED;
-  for (int t = 0; t < d.ntaps; ++t) if (d.w_off[t] % d.Cin) return VFX_ERR_UNSUPPORTED;
-  EncodeTiledFn encode = get_encode();
-  if (!encode) { set_error("conv_gemm_tc: cuTensorMapEncodeTiled not available"); return VFX_ERR_CUDA; }
-
-  TcParams p;
-  memset(&p, 0, sizeof(p));
-  int tw = 1;
-  while (tw < d.Wq && tw < TILE_M) tw <<= 1;
-  const int th = TILE_M / tw;
-  p.B = d.B; p.Hq = d.Hq; p.Wq = d.Wq; p.tw_log2 = ilog2(tw); p.th = th;
-  p.n_tw = ceil_div(d.Wq, tw); p.n_th = ceil_div(d.Hq, th); p.n_nt = d.N / Ntile; p.Ntile = Ntile;
-  p.KC = KC; p.n_kc = d.Cin / KC; p.ntaps = d.ntaps;
-  const long long total_tiles = (long long)d.B * p.n_th * p.n_tw * p.n_nt;
-  if (total_tiles >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;
-  p.total_tiles = (uint32_t)total_tiles;
-  long long max_row = 0;
-  for (int t = 0; t < d.ntaps; ++t) {
-    p.dh[t] = d.dh[t]; p.dw[t] = d.dw[t];
-    p.w_row[t] = (int)(d.w_off[t] / d.Cin);
-    if (p.w_row[t] + d.N > max_row) max_row = p.w_row[t] + d.N;
-  }
-  p.sh = d.sh; p.rh = d.rh; p.sw = d.sw; p.rw = d.rw; p.OH = d.OH; p.OW = d.OW; p.N = d.N;
-  p.out_raw = d.out_raw; p.o_sB = d.o_sB; p.o_sH = d.o_sH; p.o_sW = d.o_sW; p.o_col = d.o_col;
-  p.out_act = reinterpret_cast<__nv_bfloat16*>(d.out_act); p.oa_sB = d.oa_sB; p.oa_sH = d.oa_sH; p.oa_sW = d.oa_sW; p.oa_col = d.oa_col;
-  p.bias = d.bias; p.bias_mod = d.bias_mod > 0 ? d.bias_mod : d.N;
-  p.residual = d.residual; p.r_sB = d.r_sB; p.r_sH = d.r_sH; p.r_sW = d.r_sW; p.r_col = d.r_col;
-  p.act = d.act; p.act_param = d.act_param;
-  p.res_enc = (d.residual && d.res_enc) ? 1u : 0u; p.raw_enc = (d.out_raw && d.raw_enc) ? 1u : 0u;
-  if ((p.res_enc || p.raw_enc) && !(d.enc_slope > 0.f)) { set_error("conv_gemm_tc: enc_slope must be positive"); return VFX_ERR_INVALID; }
-  p.enc_slope = d.enc_slope; p.enc_inv_slope = d.enc_slope > 0.f ? 1.0f / d.enc_slope : 0.f;
-  p.act_scale = d.out_act ? d.act_scale : nullptr; p.act_shift = d.out_act ? d.act_shift : nullptr;
-  // instruction descriptor: c=F32 [4,6)=1, a/b format [7,10)/[10,13) = 0 (F16), 1 (BF16) or 2 (TF32), K-major both,
-  // N>>3 [17,23), M>>4 [24,29)
-  const uint32_t fmt = tf32 ? 2u : fp16 ? 0u : 1u;     // F16F32Format: 0 = F16, 1 = BF16, 2 = TF32
-  p.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(Ntile >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24);
-  const uint32_t row_bytes = KC * esz;
-  p.row_bytes = row_bytes;
-  p.a_stage_bytes = TILE_M * row_bytes;
-  p.b_stage_bytes = Ntile * row_bytes;
-  p.sbo16 = (8 * row_bytes) >> 4;
-  p.layout_type = row_bytes == 128 ? 2u : 4u;
-  p.nacc = 512 / Ntile > 8 ? 8 : 512 / Ntile;        // Ntile 256 -> 2, 128 -> 4, <= 64 -> 8
-  p.tmem_cols = 32;
-  while (p.tmem_cols < p.nacc * Ntile) p.tmem_cols <<= 1;
-  static const int jt_env = getenv("VFX_TC_JTILES") ? atoi(getenv("VFX_TC_JTILES")) : 0;
-  p.jtiles = 1u;    // interleaving tiles did not help once the issue path was made warp-uniform (kept as a knob)
-  if (jt_env >= 1 && jt_env <= 4 && (uint32_t)jt_env * 2 <= p.nacc) p.jtiles = (uint32_t)jt_env;
-  const size_t w_all = (size_t)p.ntaps * p.n_kc * p.b_stage_bytes;
-  p.w_resident = (p.n_nt == 1 && w_all <= 100 * 1024) ? 1u : 0u;
-  p.w_bytes = p.w_resident ? (uint32_t)w_all : 0u;
-  // plain stride-1 convolution whose output grid is the tensor itself -> TMA-staged epilogue
-  static const bool allow_tma_epi = getenv("VFX_NO_TMA_EPI") == nullptr;
-  p.tma_epi = (allow_tma_epi && d.sh == 1 && d.sw == 1 && d.rh == 0 && d.rw == 0 && d.OH == d.Hq && d.OW == d.Wq) ? 1u : 0u;
-  if (p.tma_epi && d.N > BIAS_SMEM_FLOATS) p.tma_epi = 0;
-  // Epilogue warps: 4 with a residual ring of 4 slots prefetched 3 chunks ahead, or 8 with round 1's two-slot ring (one chunk
-  // ahead, even / odd chunks in parallel).  Measured on one B200 box, B = 32 (A/B of the whole step, VFX_EPI_WARPS=4|8):
-  //   bf16 residual convolutions gain from the deep ring -- ResStack conv2 C = 128: 11.8 -> 10.2 ms per step, C = 256: 8.4 -> 8.1,
-  //   UNet 3x3: 15.6 -> 14.4;  operand-only convolutions lose (their chunks then run serially: C = 128 conv1 5.0 -> 5.8 ms) and
-  //   so does tf32 (already at 6.1 TB/s in conv2; its single operand staging tile serialises the chunks of a warp).
-  static const int epi_env = getenv("VFX_EPI_WARPS") ? atoi(getenv("VFX_EPI_WARPS")) : 0;
-  p.epi_warps = epi_env == 8 ? 8u : epi_env == 4 ? 4u : ((!tf32 && d.residual) ? 4u : 8u);
-  p.ro_slots = p.epi_warps == 8 ? 2u : 4u;
-  p.epi_arrivals = 32u * p.epi_warps;
-  const bool needs_ro = d.out_raw || d.residual;
-  p.epi_at_off = needs_ro ? p.ro_slots * 4096u : 0u;
-  // activated-operand staging: bf16 2 x 2 KB (double-buffered); tf32 one 4 KB tile (8 warps x 16 KB next to the
-  // raw/residual tiles would leave no room for the operand stages)
-  p.at_bytes = tf32 ? 4096u : 2048u;
-  p.at_double = tf32 ? 0u : 1u;      // tf32: one tile (the freed 4 KB per warp buys another operand stage: conv1 of a C = 64 pair
-                                     // had two halo stages and ran latency-bound at 70 % of HBM)
-  p.epi_warp_bytes = p.epi_at_off + (d.out_act ? p.at_bytes * (p.at_double ? 2u : 1u) : 0u);
-  p.bias_floats = ((uint32_t)d.N + 63u) & ~63u;
-  p.stag_warps = (p.epi_warps == 8 && Ntile < 64) ? 4u : p.epi_warps;   // 8 warps at Ntile = 32: only the even-chunk warps have work
-  const uint32_t epi_smem = p.tma_epi ? p.stag_warps * p.epi_warp_bytes + 3 * p.bias_floats * 4 : 0u;
-  if (p.w_resident && p.w_bytes + epi_smem + 3 * p.a_stage_bytes > SMEM_BUDGET) { p.w_resident = 0; p.w_bytes = 0; }
-  p.bw_log2 = p.tw_log2 < 5 ? p.tw_log2 : 5;
-  // halo mode (resident weights): 1-D conv with taps (-d, 0, +d), d <= 64; or a 3x3 conv (taps in kh,kw order)
-  static const bool allow_halo = getenv("VFX_NO_HALO") == nullptr;
-  p.halo = 0;
-  uint32_t halo_box_w = 0, halo_box_h = 0;
-  if (allow_halo && p.w_resident) {
-    const uint32_t row_b = row_bytes;
-    bool ok = false;
-    uint32_t box_w = 0, box_h = 0, extra = 0;
-    static const bool allow_halo_1d = getenv("VFX_NO_HALO_1D") == nullptr;
-    if (allow_halo_1d && d.H == 1 && d.Hq == 1 && d.ntaps == 3 && tw == TILE_M && row_bytes == 128 && d.dw[1] == 0 && d.dw[2] > 0 && d.dw[2] <= 64 &&
-        d.dw[0] == -d.dw[2] && d.dh[0] == 0 && d.dh[1] == 0 && d.dh[2] == 0) {
-      const int dd = d.dw[2];
-      box_w = TILE_M + 2 * dd; box_h = 1; p.halo_pw = dd; p.halo_ph = 0;
-      for (int t = 0; t < 3; ++t) p.halo_off[t] = (uint32_t)(t * dd);
-      ok = true;
-    } else if (d.ntaps == 9 && d.Hq == d.H && d.Wq == d.W) {
-      ok = true;
-      for (int t = 0; t < 9; ++t) {
-        if (d.dh[t] != t / 3 - 1 || d.dw[t] != t % 3 - 1) ok = false;
-        p.halo_off[t] = (uint32_t)((t / 3) * tw + (t % 3));
-      }
-      box_w = (uint32_t)tw; box_h = (uint32_t)th + 2; p.halo_pw = 1; p.halo_ph = 1; extra = 2;
-    }
-    p.halo_boxes = 1;
-    if (!ok && d.H == 1 && d.Hq == 1 && d.ntaps == 3 && tw == TILE_M && row_bytes == 128) {
-      // large dilation: the taps' boxes do not overlap -> one aligned 128-row box per tap, but still ONE pipeline
-      // stage / barrier round trip per tile
-      box_w = TILE_M; box_h = 1; p.halo_pw = 0; p.halo_ph = 0; p.halo_boxes = 3;
-      for (int t = 0; t < 3; ++t) p.halo_off[t] = (uint32_t)(t * TILE_M);
-      ok = true;
-    }
-    if (ok) {
-      p.halo_rows = box_w * box_h;
-      p.halo_kc_bytes = ((p.halo_rows * p.halo_boxes + extra + 7) / 8) * 8 * row_b;
-      p.halo_kc_bytes = (p.halo_kc_bytes + 1023) / 1024 * 1024;
-      // a stage normally holds all K chunks of a tile; worth it only if at least 2 stages fit.  If they do not, but two
-      // single-chunk stages do (tf32: C = 64 ResStack conv with three tap boxes, 48 KB per chunk; the 64 -> 32 3x3 conv of the
-      // UNet's last decoder level, 50 KB per chunk), a tile becomes n_kc stages.
-      const uint32_t room = (uint32_t)SMEM_BUDGET - p.w_bytes - epi_smem;
-      p.halo_nps = (uint32_t)p.n_kc;
-      p.halo = room / (p.halo_kc_bytes * (uint32_t)p.n_kc) >= 2 ? 1u : 0u;
-      if (!p.halo && p.n_kc > 1 && room / p.halo_kc_bytes >= 2) { p.halo = 1u; p.halo_nps = 1u; }
-      halo_box_w = box_w; halo_box_h = box_h;
-    }
-  }
-  if (!p.halo) p.halo_nps = (uint32_t)p.n_kc;
-  const uint32_t stage_bytes = p.halo ? p.halo_kc_bytes * p.halo_nps : p.a_stage_bytes + (p.w_resident ? 0u : p.b_stage_bytes);
-  int stages = (int)((SMEM_BUDGET - p.w_bytes - epi_smem) / stage_bytes);
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  const int k_steps = p.ntaps * p.n_kc;
-  if (stages < 2) return VFX_ERR_UNSUPPORTED;
-  p.stages = stages;
-  (void)k_steps;
-  const size_t smem_bytes = (size_t)p.w_bytes + (size_t)stages * stage_bytes + epi_smem + 1024 + (2 * stages + 17 + 16) * 8 + 16;
-
-  // ---- tensor maps
-  CUtensorMap tmA, tmW;
-  const CUtensorMapSwizzle swz = row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  const CUtensorMapDataType op_dt = tf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.B};
-    cuuint64_t strides[3] = {(cuuint64_t)d.a_sW * esz, (cuuint64_t)d.a_sH * esz, (cuuint64_t)d.a_sB * esz};
-    // a degenerate dimension of extent 1 may carry any stride; keep them valid multiples of 16
-    cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)(p.halo ? halo_box_w : (uint32_t)tw), (cuuint32_t)(p.halo ? halo_box_h : (uint32_t)th), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = encode(&tmA, op_dt, 4, const_cast<void*>(d.a), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("conv_gemm_tc: cuTensorMapEncodeTiled(A) failed with %d", (int)r); return VFX_ERR_CUDA; }
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)d.Cin, (cuuint64_t)max_row};
-    cuuint64_t strides[1] = {(cuuint64_t)d.Cin * esz};
-    cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)Ntile};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = encode(&tmW, op_dt, 2, const_cast<void*>(d.w), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("conv_gemm_tc: cuTensorMapEncodeTiled(W) failed with %d", (int)r); return VFX_ERR_CUDA; }
-  }
-
-  CUtensorMap tmR = tmA, tmO = tmA, tmT = tmA;     // placeholders when the direct epilogue is used
-  if (p.tma_epi) {
-    const cuuint32_t bw = 1u << p.bw_log2, bh = 32u >> p.bw_log2;
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    auto enc = [&](CUtensorMap* tm, CUtensorMapDataType dt, int esz, const void* base, long long cols, long long sW, long long sH,
-                   long long sB, CUtensorMapSwizzle swz) -> CUresult {
-      cuuint64_t dims[4] = {(cuuint64_t)cols, (cuuint64_t)d.OW, (cuuint64_t)d.OH, (cuuint64_t)d.B};
-      cuuint64_t strides[3] = {(cuuint64_t)sW * esz, (cuuint64_t)sH * esz, (cuuint64_t)sB * esz};
-      cuuint32_t box[4] = {32, bw, bh, 1};
-      return encode(tm, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    };
-    CUresult r = CUDA_SUCCESS;
-    if (d.residual) r = enc(&tmR, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.residual, d.r_col + d.N, d.r_sW, d.r_sH, d.r_sB, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r == CUDA_SUCCESS && d.out_raw) r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out_raw, d.o_col + d.N, d.o_sW, d.o_sH, d.o_sB, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (r == CUDA_SUCCESS && d.out_act)
-      r = tf32 ? enc(&tmT, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out_act, d.oa_col + d.N, d.oa_sW, d.oa_sH, d.oa_sB, CU_TENSOR_MAP_SWIZZLE_128B)
-               : enc(&tmT, op_dt, 2, d.out_act, d.oa_col + d.N, d.oa_sW, d.oa_sH, d.oa_sB, CU_TENSOR_MAP_SWIZZLE_64B);
-    if (r != CUDA_SUCCESS) { set_error("conv_gemm_tc: cuTensorMapEncodeTiled(epilogue) failed with %d", (int)r); return VFX_ERR_CUDA; }
-  }
-
-  static long long* dbg_buf = nullptr;
-  static const bool want_dbg = getenv("VFX_TC_DEBUG") != nullptr;
-  if (want_dbg && !dbg_buf) { VFX_CUDA_CHECK(cudaMalloc(&dbg_buf, 148 * 64 * sizeof(long long))); }
-  if (want_dbg) VFX_CUDA_CHECK(cudaMemsetAsync(dbg_buf, 0, 148 * 64 * sizeof(long long), st));
-  p.dbg = want_dbg ? dbg_buf : nullptr;
-
-  static int sms_of[64] = {0};                  // per device: SM count + the kernels' dynamic shared-memory attribute
-  int dev = 0, num_sms = 0;
-  VFX_CUDA_CHECK(cudaGetDevice(&dev));
-  if (dev < 64 && sms_of[dev]) num_sms = sms_of[dev];
-  else {
-    VFX_CUDA_CHECK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-#define VFX_TC_ATTR(A)                                                                                                                     \
-  VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tc_kernel<A, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-  VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tc_kernel<A, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));  \
-  VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tc_kernel<A, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
-    VFX_TC_ATTR(VFX_ACT_NONE); VFX_TC_ATTR(VFX_ACT_LRELU); VFX_TC_ATTR(VFX_ACT_ELU); VFX_TC_ATTR(VFX_ACT_LRELU_XSINX);
-    VFX_TC_ATTR(VFX_ACT_SIGMOID);
-#undef VFX_TC_ATTR
-    if (dev < 64) sms_of[dev] = num_sms;
-  }
-  const int grid = (int)(p.total_tiles < (uint32_t)num_sms ? p.total_tiles : (uint32_t)num_sms);
-  {
-    uint32_t g = (uint32_t)grid;
-    p.d_nt = (int)(g % (uint32_t)p.n_nt); g /= (uint32_t)p.n_nt;
-    p.d_iw = (int)(g % (uint32_t)p.n_tw); g /= (uint32_t)p.n_tw;
-    p.d_ih = (int)(g % (uint32_t)p.n_th); g /= (uint32_t)p.n_th;
-    p.d_b = (int)g;
-  }
-  const int act = d.out_act ? d.act : VFX_ACT_NONE;
-  switch (act) {
-#define VFX_TC_LAUNCH(A)                                                                                       \
-  case A:                                                                                                      \
-    if (tf32) conv_gemm_tc_kernel<A, true, false><<<grid, 64 + 32 * (int)p.epi_warps, smem_bytes, st>>>(tmA, tmW, tmR, tmO, tmT, p);       \
-    else if (fp16) conv_gemm_tc_kernel<A, false, true><<<grid, 64 + 32 * (int)p.epi_warps, smem_bytes, st>>>(tmA, tmW, tmR, tmO, tmT, p);  \
-    else conv_gemm_tc_kernel<A, false, false><<<grid, 64 + 32 * (int)p.epi_warps, smem_bytes, st>>>(tmA, tmW, tmR, tmO, tmT, p);           \
-    break
-    VFX_TC_LAUNCH(VFX_ACT_NONE); VFX_TC_LAUNCH(VFX_ACT_LRELU); VFX_TC_LAUNCH(VFX_ACT_ELU);
-    VFX_TC_LAUNCH(VFX_ACT_LRELU_XSINX); VFX_TC_LAUNCH(VFX_ACT_SIGMOID);
-#undef VFX_TC_LAUNCH
-    default: set_error("conv_gemm_tc: unknown activation %d", act); return VFX_ERR_INVALID;
-  }
-  VFX_LAUNCH_CHECK();
-  if (want_dbg) {
-    std::vector<long long> h(148 * 64);
-    VFX_CUDA_CHECK(cudaMemcpyAsync(h.data(), dbg_buf, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    VFX_CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int cta : {0, 73, 147}) {
-      const long long* o = h.data() + cta * 64;
-      fprintf(stderr, "[tc dbg] cta %3d tiles/cta %u | producer total %lld wait_empty %lld | mma total %lld wait_full %lld wait_tmem_empty %lld issue4mma %lld commit_stage %lld commit_acc %lld\n",
-              cta, (p.total_tiles + grid - 1) / grid, o[0], o[1], o[8], o[9], o[10], o[11], o[12], o[13]);
-      fprintf(stderr, "[tc dbg]   epi warp 0 breakdown: math+sts %lld fence+syncwarp %lld issue(store,commit,wait,prefetch) %lld decode %lld\n", o[56], o[57], o[58], o[59]);
-      for (int w = 0; w < 8; w += 4)
-        fprintf(stderr, "[tc dbg]   epi warp %d: total %lld wait_tmem_full %lld wait_res %lld wait_store_group %lld tmem_ld %lld\n", w,
-                o[16 + w * 6], o[17 + w * 6], o[18 + w * 6], o[19 + w * 6], o[20 + w * 6]);
-    }
-  }
-  return VFX_OK;
+  VFX_REQUIRE(d.ntaps >= 1 && d.ntaps <= 9, "conv_gemm: ntaps %d out of range", d.ntaps);
+  VFX_REQUIRE(d.B > 0 && d.Hq > 0 && d.Wq > 0 && d.N > 0 && d.Cin > 0, "conv_gemm: empty problem");
+  VFX_REQUIRE(d.a && d.w, "conv_gemm: null operand");
+  VFX_REQUIRE(!d.bias || d.bias_mod > 0, "conv_gemm: bias_mod must be > 0");
+  if ((d.res_enc && d.residual) || (d.raw_enc && d.out_raw))
+    VFX_REQUIRE(d.enc_slope > 0.f, "conv_gemm_tc: enc_slope must be positive");
+  const int al = 16 / (int)prec_esz(precision);     // 16-byte cp.async chunks of operand rows
+  if (d.Cin % al || d.a_sW % al || d.a_sH % al || d.a_sB % al || ((uintptr_t)d.a & 15) || ((uintptr_t)d.w & 15))
+    return VFX_ERR_UNSUPPORTED;
+  for (int t = 0; t < d.ntaps; ++t) if (d.w_off[t] % al) return VFX_ERR_UNSUPPORTED;
+  if (ceil_div((long long)d.B * d.Hq * d.Wq, BM) >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;
+  if (precision == VFX_PREC_TF32) return launch_kind<0>(d, st);
+  if (precision == VFX_PREC_BF16) return launch_kind<1>(d, st);
+  return launch_kind<2>(d, st);
 }
 
 }  // namespace vfx

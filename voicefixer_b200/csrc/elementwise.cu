@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(16 * POST_GROUPS) voc_post_kernel(const float*
 
 inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
-  if (g > 148LL * 32) g = 148LL * 32;
+  if (g > 132LL * 32) g = 132LL * 32;      // 32 blocks per SM of an H100 SXM
   if (g < 1) g = 1;
   return (int)g;
 }

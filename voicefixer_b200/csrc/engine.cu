@@ -36,16 +36,16 @@ struct vfx_engine {
   int device = 0;   // -1: planning-only engine (no CUDA calls; finalize and workspace queries only)
   int precision = VFX_PREC_FP32;
   bool finalized = false;
-  int use_tc = 1;   // BF16 / TF32: tcgen05 kernel where the shape allows (0 = SIMT cross-check on the same operands)
+  int use_tc = 1;   // BF16 / FP16 / TF32: wgmma tensor-core kernel where the shape allows (0 = SIMT cross-check on the same operands)
   std::unordered_map<std::string, vfx::Tensor> tensors;
   float* d_window = nullptr;    // periodic Hann, 2048
   float2* d_tw = nullptr;       // exp(-2 pi i k / 2048), k < 1024
   std::vector<std::string> missing;
   int parts = 0;    // VFX_PART_* bits of the weight sets found complete by vfx_engine_finalize
   int tf32_stream = 1;  // TF32: vocoder residual streams are kept as ONE encoded fp32 tensor (operand + residual carrier)
-  int fuse_pair = 1;  // BF16: ResStack pairs of width 64 run as ONE fused kernel (resstack_pair_tc.cu)
-  int fuse_pair3 = 1; // TF32 width 64: one-SM fused pair with the residual stashed in tensor memory (resstack_pair3_tc.cu)
-  int fuse_pair2 = 1; // two-CTA cluster pipeline (resstack_pair2_tc.cu): 1 = BF16 / FP16 width 128; 2 = also TF32 width 64 (no gain)
+  int fuse_pair = 1;  // BF16 / FP16: ResStack pairs of width 64 run as ONE fused kernel (resstack_pair.cu)
+  int fuse_pair3 = 1; // TF32 width 64: the same fused kernel on the encoded stream
+  int fuse_pair2 = 1; // fused pairs of width 128 (BF16 / FP16); 2 = also TF32 width 64 when fuse_pair3 is 0
   int profile = 0;
   std::vector<vfx::ProfRec> prof;
   std::string prof_report;
@@ -388,7 +388,7 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
 // ------------------------------------------------------------------ denoiser
 // nn.Sequential voicefixer/restorer/model.py:69-99 (always fp32 SIMT: 1 % of the path's FLOPs,
 // recurrent part is precision-sensitive).  mel [B][T][128] -> lin15 raw [B*T][128].
-// Denoiser GEMMs: fp32 SIMT in fp32 mode; in bf16 mode the same tcgen05 kernel as the convolutions
+// Denoiser GEMMs: fp32 SIMT in fp32 mode; in bf16 mode the same tensor-core kernel as the convolutions
 // (bf16 operands, fp32 accumulate / bias / outputs).  The GRU recurrence itself is always fp32.
 int linear(Ctx& c, const void* a, long long M, int K, const std::string& p, int N, float* out_raw,
            void* out_act, int act, const char* tag = "dn.linear") {
@@ -563,8 +563,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
       for (int grp = 0; grp < 2; ++grp) {
         const int nph = grp == 0 ? nA : u - nA;
         // Output described as the reshaped view [B][Lin][u*Co] (row q holds output samples q*u .. q*u+u-1):
-        // the phase group is then a plain stride-1 GEMM writing columns [r0*Co, (r0+nph)*Co) of row q, which
-        // lets the tensor-core kernel use its TMA-staged epilogue.
+        // the phase group is then a plain stride-1 GEMM writing columns [r0*Co, (r0+nph)*Co) of row q.
         vfx_conv_desc d = conv_base(U, B, 1, (int)Lin, Ci, w, nph * Co);
         d.ntaps = 2;
         int r0;
@@ -578,64 +577,45 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
       }
     }
     // ---- ResStack: 8 x (x + conv_k3_d1(lrelu(conv_k3_d3^i(lrelu(x))))), modules.py:550-576,592-595
-    // bf16, width 64: each pair is ONE fused kernel (h stays on chip); the activated operand copy ping-pongs between
-    // A0 and Hh because a pair reads it with a halo that neighbouring tiles would overwrite in place.
+    // 16-bit modes, width 64 / 128: each pair is ONE fused kernel (h stays on chip); the activated operand copy ping-pongs
+    // between A0 and Hh because a pair reads it with a halo that neighbouring tiles would overwrite in place.
     const bool is16 = prec == VFX_PREC_BF16 || prec == VFX_PREC_FP16;          // 2-byte operand modes share every kernel
     const bool fuse_pairs = is16 && c.e->use_tc &&
                             ((c.e->fuse_pair && Co == 64) || (c.e->fuse_pair2 && Co == 128));
     // tf32, width 64: the encoded stream ping-pongs between X and the (otherwise unused) operand buffer; 8 pairs end in X
     const bool fuse_tf32 = enc && (c.e->fuse_pair3 || c.e->fuse_pair2 >= 2) && Co == 64 && j == 3;
-    const int tf32_impl = c.e->fuse_pair3 ? 3 : 2;
     void* a_cur = A0; void* a_nxt = Hh;
     float* s_cur = X; float* s_nxt = (float*)A0;
-    void* pair_scratch = nullptr;                       // two-CTA pipeline: the h tiles cross SMs through this (L2-resident) ring
-    if ((fuse_tf32 && tf32_impl == 2) || (fuse_pairs && Co == 128)) pair_scratch = c.ws->raw(resstack_pair2_scratch_bytes());
     int dil = 1;
     for (int i = 0; i < 8; ++i, dil *= 3) {
       snprintf(name, sizeof(name), "voc.rs%d.l%d", j, i);
       const std::string p(name);
-      if (fuse_tf32) {
+      if (fuse_tf32 || fuse_pairs) {
         vfx_pair_desc pd;
         memset(&pd, 0, sizeof(pd));
-        pd.a = s_cur; pd.x = s_cur; pd.x_out = s_nxt; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co;
+        pd.precision = prec; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co;
         pd.w1 = getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec); pd.b1 = getf(c, p + ".c1.b", Co);
         pd.w2 = getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec); pd.b2 = getf(c, p + ".c2.b", Co);
-        pd.write_raw = 1; pd.precision = VFX_PREC_TF32; pd.impl = tf32_impl;
-        pd.scratch = pair_scratch; pd.scratch_bytes = resstack_pair2_scratch_bytes();
-        pd.stream_enc = 1; pd.stream_enc_out = i < 7 ? 1 : 0;     // the last pair hands plain x' to the final convolution
+        if (fuse_tf32) {
+          pd.a = s_cur; pd.x = s_cur; pd.x_out = s_nxt; pd.write_raw = 1;
+          pd.stream_enc = 1; pd.stream_enc_out = i < 7 ? 1 : 0;   // the last pair hands plain x' to the final convolution
+        } else {
+          pd.a = a_cur; pd.x = X;
+          pd.write_raw = (i < 7 || j == 3) ? 1 : 0;               // the next up-sampler consumes the operand only
+          if (i < 7) { pd.out_act = a_nxt; pd.act = VFX_ACT_LRELU; pd.act_param = 0.01f; }
+          else if (j < 3) { pd.out_act = U; pd.act = VFX_ACT_LRELU_XSINX; pd.act_param = 0.2f; }
+        }
         if (!c.dry && c.rc == VFX_OK) {
           char pt[48], ptd[64];
           snprintf(pt, sizeof(pt), "voc.rs%d.pair", j);
           snprintf(ptd, sizeof(ptd), "%s.d%d", pt, dil);
           const double els = (double)B * Lout * Co;
-          ProfScope ps(c, c.e->profile > 1 ? ptd : pt, 2.0 * 2.0 * 3.0 * Co * els, 8.0 * els);
-          VFX_TRY(tf32_impl == 3 ? resstack_pair3_tc(pd, c.st) : resstack_pair2_tc(pd, c.st));
-        }
-        float* t = s_cur; s_cur = s_nxt; s_nxt = t;
-        continue;
-      }
-      if (fuse_pairs) {
-        vfx_pair_desc pd;
-        memset(&pd, 0, sizeof(pd));
-        pd.precision = prec; pd.impl = Co == 64 ? 1 : 2;
-        pd.scratch = pair_scratch; pd.scratch_bytes = resstack_pair2_scratch_bytes();
-        pd.a = a_cur; pd.x = X; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co;
-        pd.w1 = getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec); pd.b1 = getf(c, p + ".c1.b", Co);
-        pd.w2 = getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec); pd.b2 = getf(c, p + ".c2.b", Co);
-        pd.write_raw = (i < 7 || j == 3) ? 1 : 0;           // the next up-sampler consumes the operand only
-        if (i < 7) { pd.out_act = a_nxt; pd.act = VFX_ACT_LRELU; pd.act_param = 0.01f; }
-        else if (j < 3) { pd.out_act = U; pd.act = VFX_ACT_LRELU_XSINX; pd.act_param = 0.2f; }
-        if (!c.dry && c.rc == VFX_OK) {
-          char pt[48];
-          snprintf(pt, sizeof(pt), "voc.rs%d.pair", j);
-          char ptd[64];
-          snprintf(ptd, sizeof(ptd), "%s.d%d", pt, dil);
-          const double els = (double)B * Lout * Co;
           // algorithmic bytes of a pair (SURVEY 8d): x in + x' out, fp32
           ProfScope ps(c, c.e->profile > 1 ? ptd : pt, 2.0 * 2.0 * 3.0 * Co * els, 8.0 * els);
-          VFX_TRY(pd.impl == 1 ? resstack_pair_tc(pd, c.st) : resstack_pair2_tc(pd, c.st));
+          VFX_TRY(resstack_pair(pd, c.st));
         }
-        void* t = a_cur; a_cur = a_nxt; a_nxt = t;
+        if (fuse_tf32) { float* t = s_cur; s_cur = s_nxt; s_nxt = t; }
+        else { void* t = a_cur; a_cur = a_nxt; a_nxt = t; }
         continue;
       }
       {
@@ -745,14 +725,12 @@ int vfx_engine_create(vfx_engine** out, int device, int precision) {
   VFX_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   VFX_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("vfx_b200 is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("vfx_b200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     return VFX_ERR_UNSUPPORTED;
   }
   vfx_engine* e = new vfx_engine();
   e->device = device; e->precision = precision;
-  if (getenv("VFX_FUSE_PAIR3")) e->fuse_pair3 = atoi(getenv("VFX_FUSE_PAIR3"));
-  if (getenv("VFX_FUSE_PAIR2")) e->fuse_pair2 = atoi(getenv("VFX_FUSE_PAIR2"));      // A/B knob for bench runs
   std::vector<float> win(2048);
   std::vector<float2> tw(1024);
   for (int n = 0; n < 2048; ++n) win[n] = (float)(0.5 - 0.5 * cos(2.0 * M_PI * n / 2048.0));
@@ -1005,28 +983,20 @@ int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream)
   VFX_REQUIRE(d, "conv_gemm: null descriptor");
   if (impl == 1) {
     VFX_REQUIRE(precision == VFX_PREC_BF16 || precision == VFX_PREC_TF32 || precision == VFX_PREC_FP16,
-                "conv_gemm: the tcgen05 implementation takes bf16, fp16 or tf32 operands");
+                "conv_gemm: the tensor-core implementation takes bf16, fp16 or tf32 operands");
     return conv_gemm_tc(precision, *d, (cudaStream_t)stream);
   }
   return conv_gemm_simt(precision, *d, (cudaStream_t)stream);
 }
 
-size_t vfx_resstack_pair_scratch_bytes(void) { return resstack_pair2_scratch_bytes(); }
+size_t vfx_resstack_pair_scratch_bytes(void) { return resstack_pair_scratch_bytes(); }
 
 int vfx_resstack_pair(const vfx_pair_desc* d, void* stream) {
   VFX_REQUIRE(d, "resstack_pair: null descriptor");
-  const bool tf32 = d->precision == VFX_PREC_TF32;
-  const bool one_cta = d->impl == 1 || (d->impl == 0 && !tf32 && d->C == 64 && !d->x_out);
-  int r;
-  if (tf32 && (d->impl == 3 || d->impl == 0)) {            // one SM, residual stashed in TMEM; the two-CTA form on request
-    r = resstack_pair3_tc(*d, (cudaStream_t)stream);
-    if (r == VFX_ERR_UNSUPPORTED && d->impl == 0) r = resstack_pair2_tc(*d, (cudaStream_t)stream);
-  } else if (d->impl == 3) r = VFX_ERR_UNSUPPORTED;
-  else
-    r = one_cta ? ((tf32 || d->x_out) ? VFX_ERR_UNSUPPORTED : resstack_pair_tc(*d, (cudaStream_t)stream))
-                : resstack_pair2_tc(*d, (cudaStream_t)stream);
+  const int r = resstack_pair(*d, (cudaStream_t)stream);
   if (r == VFX_ERR_UNSUPPORTED)
-    set_error("resstack_pair: unsupported shape (bf16: C = 64 or 128; tf32: C = 64 with stream_enc; 16-byte aligned tensors)");
+    set_error("resstack_pair: unsupported shape (impl 0..3; bf16 / fp16: C = 64 or 128; tf32: C = 64 with stream_enc and x_out; "
+              "16-byte aligned tensors)");
   return r;
 }
 

@@ -6,7 +6,7 @@
 // The input projections gi = x W_ih^T + b_ih are one batched GEMM (conv_gemm); this kernel is the
 // sequential part and is latency-bound (T = 1001 .. 3001 dependent steps).
 //
-// Design (sm_100a): one thread-block CLUSTER of 8 CTAs per (direction, group of G sequences).
+// Design (sm_90a): one thread-block CLUSTER of 8 CTAs per (direction, group of G sequences).
 //   * W_hh (768 x 256 fp32 = 786 KB) never fits one SM: CTA c owns hidden units [32c, 32c+32), i.e.
 //     96 gate rows, and keeps its 96 x 256 slice in REGISTERS (96 per thread) for all T steps, so a
 //     step reads no weights from shared memory, L2 or HBM.
@@ -14,10 +14,7 @@
 //     values a CTA pushes them into all 8 replicas with st.async (distributed shared memory stores
 //     that complete_tx on the DESTINATION CTA's mbarrier); each CTA starts its next step when its
 //     own mbarrier has received all 256 x G values.  No cluster barrier and no memory fence per
-//     step (an ncu capture of the cluster.sync() version showed 25 % membar + 12 % barrier stalls).
-//   * (tried: splitting the G sequences into two halves that ping-pong within a step to hide the exchange
-//     latency -- measured slower, 2.66 vs 2.23 us/step: the extra CTA barrier and mbarrier wait per
-//     half-step cost more than the latency they hide.)
+//     step.
 //   * fp32 FMA throughout (the recurrence is precision-sensitive); gi for step t+1 is prefetched
 //     into registers during step t.
 #include <cooperative_groups.h>
@@ -207,9 +204,7 @@ int launch(const float* gi, const float* whh_t, const float* bhh, int B, int T, 
 int gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out,
               cudaStream_t st) {
   VFX_REQUIRE(B > 0 && T > 0, "gru_layer: empty problem");
-  // one wave: 8 GPCs x 2 clusters of 8 CTAs = 16 co-resident clusters on the 148 SMs
-  // measured on B200 (B = 32, T = 1001, four layers per step): KQ = 8: 8.8 / 11.0 ms, KQ = 16: 9.9 / 9.7 ms in two runs each --
-  // within run-to-run noise, step time unchanged (88.9 vs 89.1 ms): the step is bound by the serial chain, not by warp count
+  // one wave: at most 16 clusters of 8 CTAs (128 of the 132 SMs, two clusters per GPC)
   static const int kq = getenv("VFX_GRU_KQ") ? atoi(getenv("VFX_GRU_KQ")) : 8;
   if (kq == 8) {
     if (2 * ((B + 1) / 2) <= 16) return launch<2, 8>(gi, whh_t, bhh, B, T, out, st);

@@ -1,136 +1,34 @@
-// PTX wrappers shared by the tcgen05 / TMA kernels of this library (conv_gemm_tc.cu, resstack_pair_tc.cu):
-// mbarriers, TMA tensor loads / stores, tcgen05 MMA issue / commit / TMEM loads, shared-memory matrix
-// descriptors, the fast activations of the operand-producing epilogues and the host-side tensor-map encoder.
+// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu): cp.async operand staging with zero fill,
+// the generic -> async proxy fence, wgmma fences / groups and the shared-memory matrix descriptor.
 #pragma once
-#include <cuda.h>
 #include "vfx_common.cuh"
 
 namespace vfx {
 namespace {
 
-// ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+// 16-byte global -> shared copy; ok == false writes 16 zero bytes (convolution padding, K / N tails)
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_LOOP:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra WAIT_DONE;\n\t"
-      "bra WAIT_LOOP;\n\t"
-      "WAIT_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_t(uint64_t* bar, uint32_t parity, long long& acc, bool on) {
-  if (on) { const long long t0 = clock64(); mbar_wait(bar, parity); acc += clock64() - t0; } else mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-// one elected lane of a fully converged warp (keeps the surrounding control flow and all operands
-// warp-uniform, so descriptors/coordinates stay in uniform registers instead of R2UR waterfalls)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Lean issue form: the descriptor high word (SBO, version, layout) is constant for the kernel; per MMA only
-// the 32-bit low words (start address >> 4, LBO field = 1) change.  lo = desc_lo(addr) is one shift/or and
-// advancing K by 16 elements is lo + 2.
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
-__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo16, uint32_t layout_type) {
-  return (sbo16 & 0x3FFFu) | (1u << 14) | ((layout_type & 7u) << 29);
-}
-#define VFX_TC_MMA_ASM(SETP, KIND)                                                                                              \
-  asm volatile("{\n\t.reg .b64 da, db;\n\t.reg .pred p;\n\t" SETP " p, 0, 0;\n\tmov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t" \
-               "tcgen05.mma.cta_group::1.kind::" KIND " [%0], da, db, %4, p;\n\t}"                                               \
-               ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc) : "memory")
-template <bool ACCUM, bool TF32>
-__device__ __forceinline__ void tc_mma_lo(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-  if (TF32) { if (ACCUM) VFX_TC_MMA_ASM("setp.eq.b32", "tf32"); else VFX_TC_MMA_ASM("setp.ne.b32", "tf32"); }
-  else      { if (ACCUM) VFX_TC_MMA_ASM("setp.eq.b32", "f16");  else VFX_TC_MMA_ASM("setp.ne.b32", "f16"); }
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// wgmma reads shared memory through the async proxy: make this thread's (generic-proxy) cp.async data visible to it
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// K-major swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// [0,14) start>>4, [16,30) LBO>>4 (unused for swizzled K-major: 1), [32,46) SBO>>4, [46,48) version=1,
-// [61,64) layout type -- built as desc_lo()/desc_hi() below.
-// Row-shifted views of a SWIZZLE_128B tile (halo mode) use the same descriptor with the shifted start
-// address and base_offset 0: verified on B200 that the MMA unit, like TMA, derives the swizzle phase
-// from the absolute shared-memory address bits [7,10) (base_offset = (addr>>7)&7 gives wrong results).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Compile-time activation for the bf16 operand output (compact code: the generic runtime switch
-// with sinf/expm1f slow paths made the epilogue instruction-fetch bound).  Results are rounded to
-// bf16 (rel. 4e-3), so the fast intrinsics (abs. error ~1e-6 after range reduction) are ample.
-template <int ACT>
-__device__ __forceinline__ float act_fast(float v, float p) {
-  if (ACT == VFX_ACT_LRELU) return v > 0.f ? v : v * p;
-  if (ACT == VFX_ACT_ELU) return v > 0.f ? v : __expf(v) - 1.f;
-  if (ACT == VFX_ACT_LRELU_XSINX) {
-    const float u = v > 0.f ? v : v * p;
-    const float k = rintf(u * 0.15915494309189535f);            // u / 2pi
-    const float r = fmaf(k, -6.2831854820251465f, u);            // Cody-Waite, 2 terms
-    return u + __sinf(fmaf(k, 1.7484555e-7f, r));
-  }
-  if (ACT == VFX_ACT_SIGMOID) return 1.f / (1.f + __expf(-v));
-  return v;
+// K-major operand tile with 128-byte rows in the 128-byte swizzle (16-byte chunk c of row r stored at chunk c ^ (r & 7)),
+// 1024-byte aligned.  Descriptor: [0,14) start >> 4, [16,30) leading offset >> 4 (unused for this layout: 1),
+// [32,46) stride between 8-row groups >> 4 (1024 B), [62,64) layout = 1 (128-byte swizzle).  Adding k >> 4 to the
+// descriptor selects the K slice starting k bytes into each row (the swizzle is applied on absolute address bits).
+__device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-
-
-// ------------------------------------------------------------------ host side: cuTensorMapEncodeTiled through the runtime
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
+__device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
 
 }  // namespace
 }  // namespace vfx

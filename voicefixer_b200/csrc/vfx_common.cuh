@@ -1,4 +1,4 @@
-// Shared declarations of the vfx_b200 CUDA library (sm_100a only).
+// Shared declarations of the vfx_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -48,7 +48,7 @@ template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 // VFX_PREC_TF32 operand element: fp32 storage holding a value already rounded to tf32 (10-bit mantissa,
 // round-to-nearest) by its producer, so that the tensor core's truncation of the low 13 bits is exact.
-// (Un-rounded operands make kind::tf32 truncate: a CPU simulation of the whole path gave 1.4e-2 waveform
+// (Un-rounded operands make the tf32 tensor core truncate: a CPU simulation of the whole path gave 1.4e-2 waveform
 // rel-RMS with truncation against 1.7e-3 with round-to-nearest, tools/sim_precision.py.)
 struct tf32_t { float v; };
 __device__ __forceinline__ float round_tf32(float v) {
@@ -94,11 +94,9 @@ __device__ __forceinline__ float apply_act(float v, int act, float p) {
 
 // ------------------------------------------------------------------ kernels (host launchers)
 int conv_gemm_simt(int precision, const vfx_conv_desc& d, cudaStream_t st);
-int resstack_pair_tc(const vfx_pair_desc& d, cudaStream_t st);     // fused ResStack pair (bf16, C = 64), one CTA per tile
-int resstack_pair2_tc(const vfx_pair_desc& d, cudaStream_t st);    // ... two-CTA cluster pipeline (bf16 C = 128, tf32 C = 64)
-size_t resstack_pair2_scratch_bytes();
-int resstack_pair3_tc(const vfx_pair_desc& d, cudaStream_t st);    // ... tf32 C = 64 on one SM, residual stashed in TMEM
-int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st);   // tcgen05: bf16 (kind::f16) or tf32 (kind::tf32)
+int resstack_pair(const vfx_pair_desc& d, cudaStream_t st);        // ResStack pair as two conv_gemm_tc launches per row block
+size_t resstack_pair_scratch_bytes();
+int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st);   // wgmma: bf16 / fp16 (f16 kinds) or tf32
 
 // y = act(scale[b][c]*x + shift[b][c]); x fp32 [B][P][C] (row pitch ldx), y operand type.
 // bn_C == 1: single-channel BN (scale[b][0]).  stat_sB: element stride between items (0 = shared).

@@ -22,11 +22,11 @@ def _stream():
 
 
 def default_precision():
-    """"tf32": tcgen05 kind::tf32 on tf32-rounded fp32 operands -- the arithmetic class of the reference's own CUDA path
+    """"tf32": wgmma tf32 on tf32-rounded fp32 operands -- the arithmetic class of the reference's own CUDA path
     (cuDNN TF32 convolutions; waveform within 2e-3 relative RMS of the fp32 CPU path).  VFX_PRECISION selects another mode:
-    "bf16" (tcgen05 kind::f16, 1.6x faster, 1.3e-2 relative RMS / 2.7e-3 mean-abs: inside the reference's own 1e-2 mean-abs
-    acceptance bar), "fp16" (tcgen05 kind::f16 on fp16 operands: tf32's 10-bit mantissa, hence tf32's parity, at the bf16 mode's
-    speed -- within fp16's exponent range) or "fp32" (SIMT fp32 validation path, reference-exact to ~4e-6)."""
+    "bf16" (wgmma on bf16 operands, half the operand traffic; within 3e-2 relative RMS / 5e-3 mean-abs, inside the reference's
+    own 1e-2 mean-abs acceptance bar), "fp16" (wgmma on fp16 operands: tf32's 10-bit mantissa, hence tf32's tolerance, with the
+    bf16 mode's traffic -- within fp16's exponent range) or "fp32" (SIMT fp32 validation path, within 2e-4 of the reference)."""
     return os.environ.get("VFX_PRECISION", "tf32")
 
 
@@ -66,7 +66,7 @@ class Engine:
 
     def __init__(self, ana=None, voc=None, device=None, precision=None, packed=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("voicefixer_b200 needs a CUDA device (B200, sm_100a); there is no CPU path")
+            raise RuntimeError("voicefixer_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.lib = _lib.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.precision = precision or default_precision()

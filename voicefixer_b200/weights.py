@@ -13,7 +13,7 @@ BN_EPS = 1e-5
 
 def round_tf32(t):
     """fp32 -> nearest tf32 value (10-bit mantissa, ties away from zero = PTX cvt.rna.tf32.f32), kept in fp32 storage.
-    The tensor core truncates the low 13 mantissa bits of a kind::tf32 operand; pre-rounded weights make that exact."""
+    The tensor core truncates the low 13 mantissa bits of a tf32 operand; pre-rounded weights make that exact."""
     i = t.float().contiguous().view(torch.int32)
     return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
 
