@@ -7,8 +7,11 @@ from voicefixer_b200 import _lib
 def conv_gemm(a, w, taps, Hq=None, Wq=None, N=None, w_off=None, bias=None, bias_mod=None, residual=None,
               act="none", act_param=0.0, want_raw=True, want_act=False, sh=1, rh=0, sw=1, rw=0, OH=None, OW=None,
               out_ld=None, out_col=0, precision="fp32", impl=0, out_raw=None, out_act=None, res_enc=0, raw_enc=0,
-              enc_slope=0.0):
-    """a: (B,H,W,Cin) cuda (fp32 or bf16); w: flat weight tensor; taps: [(dh,dw)]."""
+              enc_slope=0.0, act_scale=None, act_shift=None, act_ld=None, act_col=None, act_sB=None):
+    """a: (B,H,W,Cin) cuda (fp32 or bf16); w: flat weight tensor; taps: [(dh,dw)].
+    act_scale / act_shift: per-channel affine applied before the activation of out_act (both or neither);
+    act_ld / act_col: row pitch and first column of out_act when they differ from the raw output's (out_ld / out_col);
+    act_sB: item stride of out_act in elements, in place of the dense OH * OW * pitch (e.g. a padded buffer)."""
     lib = _lib.load()
     B, H, W, Cin = a.shape
     d = _lib.ConvDesc()
@@ -30,10 +33,18 @@ def conv_gemm(a, w, taps, Hq=None, Wq=None, N=None, w_off=None, bias=None, bias_
         d.out_raw = out_raw.data_ptr()
         d.o_sW, d.o_sH, d.o_sB, d.o_col = ld, d.OW * ld, d.OH * d.OW * ld, out_col
     if want_act:
+        ald = act_ld or ld
         if out_act is None:
-            out_act = torch.zeros(B, d.OH, d.OW, ld, device=a.device, dtype=dt)
+            out_act = torch.zeros(B, d.OH, d.OW, ald, device=a.device, dtype=dt)
         d.out_act = out_act.data_ptr()
-        d.oa_sW, d.oa_sH, d.oa_sB, d.oa_col = ld, d.OW * ld, d.OH * d.OW * ld, out_col
+        d.oa_sW, d.oa_sH, d.oa_sB = ald, d.OW * ald, d.OH * d.OW * ald
+        d.oa_col = out_col if act_col is None else act_col
+        if act_sB is not None:
+            d.oa_sB = act_sB
+    if (act_scale is None) != (act_shift is None):
+        raise ValueError("act_scale and act_shift go together")
+    if act_scale is not None:
+        d.act_scale, d.act_shift = act_scale.data_ptr(), act_shift.data_ptr()
     if bias is not None:
         d.bias = bias.data_ptr(); d.bias_mod = bias_mod or bias.numel()
     if residual is not None:
