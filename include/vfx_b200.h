@@ -119,10 +119,20 @@ int vfx_vocoder(vfx_engine* e, const float* mel, int B, int T, int input_is_log,
 int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav_out, int trim_len,
                      float scale, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Whole restore_inmem loop body (voicefixer/base.py:120-135) for B equal-length segments:
+/* Whole restore_inmem loop body (voicefixer/base.py:120-135) for B equal-length segments (vfx_restore_ragged below for
+ * segments of different lengths):
  * wav[B][L] -> wav_out[B][L].  Equivalent to frontend -> analysis -> vocoder(trim_len = L). */
 int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
                 float* wav_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* vfx_restore (mode 0) for B segments of DIFFERENT lengths: wav[B][L_cap] holds item b in its first lens[b] samples
+ * (the rest is never read), lens[B] is a device int32 array.  wav_out[B][L_cap] receives item b's restoration in its
+ * first lens[b] samples -- bit-identical to vfx_restore on that item alone -- and zeros after them.  A small kernel turns
+ * lens into per-item extents at every stage (frames, UNet levels, vocoder rates) that the kernels read on the device, so
+ * one launch sequence (or one captured CUDA graph) of shape (B, L_cap) serves any lengths; lengths are clamped into
+ * [1025, L_cap].  Workspace: vfx_workspace_bytes(e, B, L_cap). */
+int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* wav_out,
+                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* mode 1 pre-filter, VoiceFixer.remove_higher_frequency (voicefixer/base.py:87-104) with the
  * librosa 0.10.1 stft/istft defaults (n_fft 2048, hop 512, Hann, center, zero pad):
@@ -164,6 +174,14 @@ typedef struct vfx_conv_desc {
    * res_enc: `residual` holds S, it is decoded before the add.  raw_enc: `out_raw` receives S of the result. */
   int res_enc, raw_enc;
   float enc_slope;
+  /* Per-item extents along one sequence axis (ragged batches, vfx_restore_ragged); NULL = the whole tensor.
+   * seq_axis 0 = H (the UNet's [B][T][F][C]), 1 = W (the 1-D [B][1][L][C] layouts).  An input coordinate on that axis
+   * >= seq_in[b] reads as zero (like one outside [0, H) x [0, W)); an output whose coordinate on that axis, in the
+   * output space (q*s + r, the space of OH / OW), is >= seq_out[b] is not stored.  A 128-row tile whose rows all lie
+   * beyond seq_out exits before its K loop. */
+  const int* seq_in;
+  const int* seq_out;
+  int seq_axis;
 } vfx_conv_desc;
 
 enum vfx_act { VFX_ACT_NONE = 0, VFX_ACT_LRELU = 1, VFX_ACT_ELU = 2,
@@ -196,6 +214,8 @@ typedef struct vfx_pair_desc {
   int stream_enc, stream_enc_out;
   void* scratch;            /* impl 2: device scratch of vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned: holds h */
   size_t scratch_bytes;
+  const int* lens;          /* optional per-item length (<= L; L stays the item stride): rows >= lens[b] read as zero and are not
+                             * written, as if item b had length lens[b].  NULL = every item has length L.  impl 2 refuses it. */
 } vfx_pair_desc;
 size_t vfx_resstack_pair_scratch_bytes(void);
 int vfx_resstack_pair(const vfx_pair_desc* d, void* stream);
@@ -205,6 +225,10 @@ int vfx_resstack_pair(const vfx_pair_desc* d, void* stream);
  * torch.nn.GRU gate order r,z,n (voicefixer/restorer/model.py:35-42,61). */
 int vfx_gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out,
                   void* stream);
+/* The same with a per-item sequence length lens[B] (device int32, 1 <= lens[b] <= T): item b's backward direction starts
+ * at lens[b] - 1, as if the item were run alone with T = lens[b].  out[b][t] for t >= lens[b] is undefined. */
+int vfx_gru_layer_ragged(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens,
+                         float* out, void* stream);
 
 #ifdef __cplusplus
 }

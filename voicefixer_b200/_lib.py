@@ -30,6 +30,7 @@ class ConvDesc(ctypes.Structure):
         ("residual", _vp), ("r_sB", _ll), ("r_sH", _ll), ("r_sW", _ll), ("r_col", _i),
         ("act", _i), ("act_param", _f), ("act_scale", _vp), ("act_shift", _vp),
         ("res_enc", _i), ("raw_enc", _i), ("enc_slope", _f),
+        ("seq_in", _vp), ("seq_out", _vp), ("seq_axis", _i),
     ]
 
 
@@ -38,7 +39,7 @@ class PairDesc(ctypes.Structure):
     _fields_ = [("a", _vp), ("x", _vp), ("w1", _vp), ("b1", _vp), ("dilation", _i), ("w2", _vp), ("b2", _vp),
                 ("B", _i), ("L", _i), ("C", _i), ("write_raw", _i), ("out_act", _vp), ("act", _i), ("act_param", _f),
                 ("precision", _i), ("impl", _i), ("x_out", _vp), ("stream_enc", _i), ("stream_enc_out", _i),
-                ("scratch", _vp), ("scratch_bytes", _sz)]
+                ("scratch", _vp), ("scratch_bytes", _sz), ("lens", _vp)]
 
 
 # name -> (restype, argtypes); must list every symbol include/vfx_b200.h declares
@@ -64,6 +65,8 @@ SIGNATURES = {
     "vfx_resstack_pair": (_i, [_c.POINTER(PairDesc), _vp]),
     "vfx_resstack_pair_scratch_bytes": (_sz, []),
     "vfx_gru_layer": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
+    "vfx_gru_layer_ragged": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "vfx_restore_ragged": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

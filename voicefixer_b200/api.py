@@ -35,6 +35,29 @@ def _load_vocoder_state():
     return torch.load(path, map_location="cpu")["generator"]
 
 
+def ragged_plan(wavs):
+    """Validates the list form of VoiceFixer.restore_batch: a non-empty list of 1-D arrays of 1025 .. 30 s samples each.
+    Returns (items as contiguous float32 arrays, their lengths, L_cap): L_cap is the longest length rounded up to a
+    whole second, so batches of other lengths under the same cap share one captured graph."""
+    if len(wavs) == 0:
+        raise ValueError("restore_batch takes a non-empty list of 1-D arrays")
+    items, lens = [], []
+    for i, w in enumerate(wavs):
+        a = np.ascontiguousarray(w, dtype=np.float32)
+        if a.ndim != 1:
+            raise ValueError(f"restore_batch: item {i} has shape {a.shape}; the list form takes 1-D arrays, one utterance each")
+        if a.shape[0] <= 1024:
+            raise ValueError(f"restore_batch: item {i} has {a.shape[0]} samples; the front end reflect-pads 1024, "
+                             "so every item needs at least 1025")
+        if a.shape[0] > SEG_LENGTH:
+            raise ValueError(f"restore_batch: item {i} has {a.shape[0]} samples, more than 30 s "
+                             "(longer inputs: restore_inmem segments them)")
+        items.append(a)
+        lens.append(a.shape[0])
+    L_cap = -(-max(lens) // 44100) * 44100
+    return items, lens, L_cap
+
+
 class _ModelShim:
     """Stands in for `VoiceFixer._model` (the reference nn.Module): callers poke
     `.parameters()`, `.to()`, `.eval()`, `.train()` and `.vocoder` (test/streamlit.py:40-42)."""
@@ -237,15 +260,22 @@ class VoiceFixer:
 
     @torch.no_grad()
     def restore_batch(self, wavs, cuda=True, mode=0, out=None):
-        """Extension of the reference API for many utterances of one length (the reference restores one array per call,
+        """Extension of the reference API for many utterances (the reference restores one array per call,
         voicefixer/base.py:106): wavs np (B, L) float32, L <= 30 s -> np (B, L) float32, every row exactly what
         restore_inmem(row, mode) returns (mode 0 here; modes 1 / 2 go through restore_inmem).  The launch sequence of a
         shape is captured into a CUDA graph on first use and replayed afterwards; host buffers move through pinned
         staging (directly, when `wavs` / `out` are pinned: see pinned_empty).  Without `out`, the result is a view of an
-        internal pinned buffer that the next call with the same shape overwrites."""
+        internal pinned buffer that the next call with the same shape overwrites.
+
+        wavs may also be a list of 1-D arrays of different lengths (1025 samples .. 30 s each): they run as ONE ragged
+        batch (vfx_restore_ragged) and the result is a list of new arrays, item i exactly what
+        restore_batch(wavs[i][None])[0] returns.  The graph is keyed by (B, L_cap), L_cap = the longest item rounded up
+        to a whole second, so later lists of as many items under the same cap replay it.  `out` is not used then."""
         _check_cuda(cuda)
         if mode != 0:
             raise ValueError("restore_batch runs mode 0; use restore_inmem for modes 1 and 2")
+        if isinstance(wavs, (list, tuple)):
+            return self._restore_ragged(wavs)
         x = np.ascontiguousarray(wavs, dtype=np.float32)
         if x.ndim != 2 or x.shape[1] > SEG_LENGTH:
             raise ValueError("restore_batch takes (B, L) with L <= 30 s (longer inputs: restore_inmem segments them)")
@@ -279,6 +309,37 @@ class VoiceFixer:
             out[...] = dst.numpy()
             return out
         return out if out is not None else dst.numpy()
+
+    def _restore_ragged(self, wavs):
+        items, lens, L_cap = ragged_plan(wavs)
+        B = len(items)
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+        plans = self.__dict__.setdefault("_batch_plans", {})
+        key = ("ragged", B, L_cap)
+        p = plans.get(key)
+        fresh = p is None
+        if fresh:
+            if len(plans) >= 4:                                            # a few shapes at most: graphs own workspaces
+                plans.pop(next(iter(plans)))
+            p = {"dev_in": torch.zeros((B, L_cap), device=dev), "dev_out": torch.empty((B, L_cap), device=dev),
+                 "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
+                 "host_in": torch.zeros((B, L_cap)).pin_memory(), "host_out": torch.empty((B, L_cap)).pin_memory(),
+                 "host_lens": torch.empty(B, dtype=torch.int32).pin_memory()}
+        hin = p["host_in"].numpy()
+        for i, a in enumerate(items):            # samples past an item's length are never read: no need to clear them
+            hin[i, :lens[i]] = a
+        p["host_lens"].copy_(torch.tensor(lens, dtype=torch.int32))
+        p["dev_in"].copy_(p["host_in"], non_blocking=True)
+        p["dev_lens"].copy_(p["host_lens"], non_blocking=True)
+        if fresh:
+            p["graph"] = eng.make_graph(p["dev_in"], p["dev_out"], mode=0, lens=p["dev_lens"])
+            plans[key] = p
+        p["graph"].replay()
+        p["host_out"].copy_(p["dev_out"], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        hout = p["host_out"].numpy()
+        return [hout[i, :lens[i]].copy() for i in range(B)]
 
     # ------------------------------------------------------------------ streaming entry point (extension, SURVEY 8f-3)
     @torch.no_grad()

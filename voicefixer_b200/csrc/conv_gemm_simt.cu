@@ -63,7 +63,7 @@ template <typename T>
 __global__ void __launch_bounds__(NT) conv_gemm_simt_kernel(const vfx_conv_desc d, const bool vec_ok) {
   __shared__ __align__(16) float As[BK][BM];
   __shared__ __align__(16) float Bs[BK][BN];
-  __shared__ int row_b[BM], row_h[BM], row_w[BM];
+  __shared__ int row_b[BM], row_h[BM], row_w[BM], row_lim[BM];
 
   const int tid = threadIdx.x;
   const long long M = (long long)d.B * d.Hq * d.Wq;
@@ -78,9 +78,18 @@ __global__ void __launch_bounds__(NT) conv_gemm_simt_kernel(const vfx_conv_desc 
       int qw = (int)(m % d.Wq);
       long long r = m / d.Wq;
       row_w[tid] = qw; row_h[tid] = (int)(r % d.Hq); row_b[tid] = (int)(r / d.Hq);
+      row_lim[tid] = d.seq_in ? d.seq_in[row_b[tid]] : 0x7fffffff;     // the item's extent (vfx_conv_desc.seq_in)
     } else {
-      row_b[tid] = -1; row_h[tid] = 0; row_w[tid] = 0;
+      row_b[tid] = -1; row_h[tid] = 0; row_w[tid] = 0; row_lim[tid] = 0;
     }
+  }
+  if (d.seq_out) {     // ragged batch: a tile whose rows all lie beyond their items' extents has nothing to store
+    bool live = false;
+    if (tid < BM && row_b[tid] >= 0) {
+      const int oh = row_h[tid] * d.sh + d.rh, ow = row_w[tid] * d.sw + d.rw;
+      live = oh < d.OH && ow < d.OW && (d.seq_axis ? ow : oh) < d.seq_out[row_b[tid]];
+    }
+    if (!__syncthreads_or(live)) return;
   }
   __syncthreads();
 
@@ -93,12 +102,12 @@ __global__ void __launch_bounds__(NT) conv_gemm_simt_kernel(const vfx_conv_desc 
 
   const int a_row = tid >> 1, a_k = (tid & 1) * 8;     // A loader: 128 rows x 2 halves of 8
   const int b_row = tid >> 2, b_k = (tid & 3) * 4;     // B loader: 64 rows x 4 quarters of 4
-  const int ab = row_b[a_row], ah = row_h[a_row], aw = row_w[a_row];
+  const int ab = row_b[a_row], ah = row_h[a_row], aw = row_w[a_row], alim = row_lim[a_row];
   const int bn = n0 + b_row;
 
   for (int tap = 0; tap < d.ntaps; ++tap) {
     const int ih = ah + d.dh[tap], iw = aw + d.dw[tap];
-    const bool inb = (ab >= 0) && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W;
+    const bool inb = (ab >= 0) && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W && (d.seq_axis ? iw : ih) < alim;
     const T* ap = A + (long long)(ab < 0 ? 0 : ab) * d.a_sB + (long long)ih * d.a_sH + (long long)iw * d.a_sW;
     const T* wp = Wt + d.w_off[tap] + (long long)bn * d.Cin;
     for (int c0 = 0; c0 < d.Cin; c0 += BK) {
@@ -151,6 +160,7 @@ __global__ void __launch_bounds__(NT) conv_gemm_simt_kernel(const vfx_conv_desc 
     if (b < 0) continue;
     const int oh = row_h[r] * d.sh + d.rh, ow = row_w[r] * d.sw + d.rw;
     if (oh >= d.OH || ow >= d.OW) continue;
+    if (d.seq_out && (d.seq_axis ? ow : oh) >= d.seq_out[b]) continue;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;

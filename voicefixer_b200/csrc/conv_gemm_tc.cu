@@ -11,6 +11,8 @@
 // ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the encoded stream of
 // vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.  The epilogue (bias, fp32
 // residual, eval-BN affine, activation, operand for the next layer) works on the accumulator registers directly.
+// Ragged batches (seq_in / seq_out): each item's extent on the sequence axis acts as that item's own edge, so every row
+// inside it is computed from the same operands as with the item alone.
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -28,7 +30,8 @@ template <> struct OpT<2> { using T = __half; static constexpr int ESZ = 2; };
 
 template <int BN> constexpr int smem_bytes() { return STAGES * (A_BYTES + BN * 128) + 1024; }
 
-template <int BN, int KIND>
+// SEQ: the descriptor carries per-item extents (seq_in / seq_out); without them the kernel is compiled without the checks
+template <int BN, int KIND, bool SEQ>
 __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d, const int nkc) {
   using T = typename OpT<KIND>::T;
   constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
@@ -45,7 +48,8 @@ __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_consta
 
   // ---- this thread's staging work: chunk `chunk` of A rows lrow + 32 i and of B rows lrow + 32 i
   const int chunk = tid & 7, lrow = tid >> 3;
-  int rb[4], rh[4], rw[4];
+  int rb[4], rh[4], rw[4], rlim[4];     // rlim: the item's extent on the sequence axis (vfx_conv_desc.seq_in)
+  bool live = false;                    // some row of this thread is stored (checked only with seq_out)
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const long long m = m0 + lrow + 32 * i;
@@ -53,10 +57,17 @@ __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_consta
       rw[i] = (int)(m % d.Wq);
       const long long r = m / d.Wq;
       rh[i] = (int)(r % d.Hq); rb[i] = (int)(r / d.Hq);
+      rlim[i] = SEQ && d.seq_in ? d.seq_in[rb[i]] : 0x7fffffff;
+      if (SEQ && d.seq_out) {
+        const int oh = rh[i] * d.sh + d.rh, ow = rw[i] * d.sw + d.rw;
+        live |= oh < d.OH && ow < d.OW && (d.seq_axis ? ow : oh) < d.seq_out[rb[i]];
+      }
     } else {
-      rb[i] = -1; rh[i] = 0; rw[i] = 0;
+      rb[i] = -1; rh[i] = 0; rw[i] = 0; rlim[i] = 0;
     }
   }
+  // ragged batch: a tile whose 128 rows all lie beyond their items' extents has nothing to store
+  if (SEQ && d.seq_out && !__syncthreads_or(live)) return;
   const int niter = d.ntaps * nkc;
   auto load_stage = [&](int it, int s) {
     const int tap = it / nkc;
@@ -68,7 +79,7 @@ __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_consta
     for (int i = 0; i < 4; ++i) {
       const int r = lrow + 32 * i;
       const int ih = rh[i] + dh, iw = rw[i] + dw;
-      const bool ok = c_ok && rb[i] >= 0 && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W;
+      const bool ok = c_ok && rb[i] >= 0 && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W && (!SEQ || (d.seq_axis ? iw : ih) < rlim[i]);
       const char* src = ok ? A + ((long long)rb[i] * d.a_sB + (long long)ih * d.a_sH + (long long)iw * d.a_sW + c) * ESZ : A;
       cp_async16(sa + sw128_offset(r, chunk), src, ok);
     }
@@ -127,6 +138,7 @@ __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_consta
     const int qh = (int)(r % d.Hq), b = (int)(r / d.Hq);
     const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
     if (oh >= d.OH || ow >= d.OW) continue;
+    if (SEQ && d.seq_out && (d.seq_axis ? ow : oh) >= d.seq_out[b]) continue;
     const long long o_raw = (long long)b * d.o_sB + (long long)oh * d.o_sH + (long long)ow * d.o_sW + d.o_col;
     const long long o_act = (long long)b * d.oa_sB + (long long)oh * d.oa_sH + (long long)ow * d.oa_sW + d.oa_col;
     const long long o_res = (long long)b * d.r_sB + (long long)oh * d.r_sH + (long long)ow * d.r_sW + d.r_col;
@@ -151,29 +163,34 @@ __global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_consta
   }
 }
 
-template <int BN, int KIND>
+template <int BN, int KIND, bool SEQ>
 int launch(const vfx_conv_desc& d, cudaStream_t st) {
   constexpr int smem = smem_bytes<BN>();
   static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
   int dev = 0;
   VFX_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, SEQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     if (dev < 64) attr_set |= 1ull << dev;
   }
   const long long M = (long long)d.B * d.Hq * d.Wq;
   const int nkc = ceil_div(d.Cin, 128 / OpT<KIND>::ESZ);
   dim3 grid(ceil_div(M, BM), ceil_div(d.N, BN));
-  conv_gemm_wgmma_kernel<BN, KIND><<<grid, NT, smem, st>>>(d, nkc);
+  conv_gemm_wgmma_kernel<BN, KIND, SEQ><<<grid, NT, smem, st>>>(d, nkc);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
 
+template <int KIND, bool SEQ>
+int launch_n(const vfx_conv_desc& d, cudaStream_t st) {
+  if (d.N <= 32) return launch<32, KIND, SEQ>(d, st);
+  if (d.N <= 64) return launch<64, KIND, SEQ>(d, st);
+  return launch<128, KIND, SEQ>(d, st);
+}
+
 template <int KIND>
 int launch_kind(const vfx_conv_desc& d, cudaStream_t st) {
-  if (d.N <= 32) return launch<32, KIND>(d, st);
-  if (d.N <= 64) return launch<64, KIND>(d, st);
-  return launch<128, KIND>(d, st);
+  return (d.seq_in || d.seq_out) ? launch_n<KIND, true>(d, st) : launch_n<KIND, false>(d, st);
 }
 
 }  // namespace

@@ -137,8 +137,8 @@ __global__ void avgpool_kernel(const float* __restrict__ x, long long x_sB, long
 // restorer/model_kqq_bn.py:144-151: clean = sigmoid(lin)*mel; x = to_log(clean);
 // unet_in[b][t][f][0..1] = (to_log(mel), x) for f < 127, zero rows for T <= t < Tp.
 __global__ void mask_log_pack_kernel(const float* __restrict__ lin, const float* __restrict__ mel,
-                                     int B, int T, int Tp, float* __restrict__ xlog,
-                                     float* __restrict__ unet_in) {
+                                     int B, int T, int Tp, const int* __restrict__ ext_frames,
+                                     float* __restrict__ xlog, float* __restrict__ unet_in) {
   const long long total = (long long)B * Tp * 128;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -147,7 +147,7 @@ __global__ void mask_log_pack_kernel(const float* __restrict__ lin, const float*
     const int t = (int)(r % Tp);
     const int b = (int)(r / Tp);
     float lm = 0.f, lx = 0.f;
-    if (t < T) {
+    if (t < (ext_frames ? ext_frames[b] : T)) {
       const long long src = ((long long)b * T + t) * 128 + f;
       const float m = mel[src];
       const float s = 1.f / (1.f + expf(-lin[src]));
@@ -193,7 +193,7 @@ __global__ void unet_head_kernel(const float* __restrict__ x, int B, int T, int 
 // tr_normalize, tr_pre vocoder/model/util.py:8-36,69-80.  tab = mel_weight[128] ++ [min_level].
 template <typename T>
 __global__ void voc_normalize_kernel(const float* __restrict__ mel, int B, int Tn, int Tc,
-                                     int input_is_log, const float* __restrict__ tab,
+                                     const int* __restrict__ ext_frames, int input_is_log, const float* __restrict__ tab,
                                      T* __restrict__ cond) {
   const long long total = (long long)B * Tc * 128;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -203,7 +203,7 @@ __global__ void voc_normalize_kernel(const float* __restrict__ mel, int B, int T
     const int t = (int)(r % Tc);
     const int b = (int)(r / Tc);
     float c = -4.0f;
-    if (t < Tn) {
+    if (t < (ext_frames ? ext_frames[b] : Tn)) {
       float v = mel[((long long)b * Tn + t) * 128 + k];
       if (input_is_log) v = exp10f(fminf(v, 5.0f));
       v = v / tab[k];
@@ -223,14 +223,15 @@ __global__ void cast_kernel(const float* __restrict__ x, long long n, T* __restr
 
 // nn.ReflectionPad1d(3) voicefixer/vocoder/model/generator.py:74,94 on a [B][L+6][C] buffer
 template <typename T>
-__global__ void reflect_pad3_kernel(T* __restrict__ buf, int B, int L, int C) {
+__global__ void reflect_pad3_kernel(T* __restrict__ buf, int B, int Lmax, int C, const int* __restrict__ ext_len) {
   const long long total = (long long)B * 6 * C;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % C);
     const int j = (int)((i / C) % 6);
     const int b = (int)(i / (6LL * C));
-    T* base = buf + (long long)b * (L + 6) * C;
+    T* base = buf + (long long)b * (Lmax + 6) * C;
+    const int L = ext_len ? ext_len[b] : Lmax;    // ragged batch: the item's own length, padded at its own end
     const int dst = j < 3 ? j : L + j;            // rows 0,1,2 and L+3,L+4,L+5
     const int src = j < 3 ? 6 - j : L + 4 - j;    // x[3-j] at row 6-j ; x[L-2-(j-3)] at row L+4-j
     base[(long long)dst * C + c] = base[(long long)src * C + c];
@@ -259,14 +260,20 @@ __device__ __forceinline__ float4 post_load_row(const float* __restrict__ xb, in
   return v;
 }
 
-__global__ void __launch_bounds__(16 * POST_GROUPS) voc_post_kernel(const float* __restrict__ x, int L,
+__global__ void __launch_bounds__(16 * POST_GROUPS) voc_post_kernel(const float* __restrict__ x, int Lmax,
                                                                      const float* __restrict__ w,
                                                                      const float* __restrict__ bias, int lo,
-                                                                     int out_len, float scale, float* __restrict__ out) {
+                                                                     int out_len, const int* __restrict__ ext_gen,
+                                                                     const int* __restrict__ ext_len, float scale,
+                                                                     float* __restrict__ out) {
   const int q = threadIdx.x & 15, g = threadIdx.x >> 4;
   const int b = blockIdx.y;
   const int o0 = (blockIdx.x * POST_GROUPS + g) * POST_RUN;       // first output of this group's run (may be >= out_len)
-  const float* xb = x + (long long)b * L * 64;
+  const float* xb = x + (long long)b * Lmax * 64;
+  // ragged batch: the item's generated length L and its own centred trim; outputs from `valid` to out_len are zeros
+  const int L = ext_gen ? ext_gen[b] : Lmax;
+  const int valid = ext_gen ? ext_len[b] : out_len;
+  if (ext_gen) lo = (L - valid) / 2;
   float4 wk[7];
 #pragma unroll
   for (int k = 0; k < 7; ++k) wk[k] = *reinterpret_cast<const float4*>(w + k * 64 + 4 * q);
@@ -305,12 +312,32 @@ __global__ void __launch_bounds__(16 * POST_GROUPS) voc_post_kernel(const float*
       if ((o & 15) == q) res = sum;                               // lane q keeps outputs o = q (mod 16)
       if (o >= 0 && (o & 15) == 15) {                             // 16 outputs gathered: one coalesced 64-byte store
         const int oo = o0 + o - 15 + q;
-        if (oo < out_len) out[(long long)b * out_len + oo] = tanhf(res + bv) * scale;
+        if (oo < out_len) out[(long long)b * out_len + oo] = oo < valid ? tanhf(res + bv) * scale : 0.f;
       }
     }
 #pragma unroll
     for (int j = 0; j < 7; ++j) cur[j] = nxt[j];
   }
+}
+
+// Per-item extents of a ragged batch at every stage of restore() (vfx_common.cuh, EXT_*): the shapes each item would
+// have if it were restored alone.  Lengths are clamped into [1025, L_cap] so that no kernel can leave the tensors.
+__global__ void ragged_extents_kernel(const int* __restrict__ lens, int B, int L_cap, int* __restrict__ ext) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int L = min(max(lens[b], 1025), L_cap);
+  const int T = 1 + L / 441;
+  const int Tp = (T + 63) / 64 * 64;
+  const int Tc = T + T % 2 + 4;
+  ext[EXT_SAMPLES * B + b] = L;
+  ext[EXT_FRAMES * B + b] = T;
+  for (int k = 0; k < 7; ++k) ext[(EXT_UNET0 + k) * B + b] = Tp >> k;
+  ext[EXT_COND * B + b] = Tc;
+  ext[EXT_COND_PAD * B + b] = Tc + 6;
+  ext[(EXT_UP0 + 0) * B + b] = Tc * 7;
+  ext[(EXT_UP0 + 1) * B + b] = Tc * 49;
+  ext[(EXT_UP0 + 2) * B + b] = Tc * 147;
+  ext[(EXT_UP0 + 3) * B + b] = Tc * 441;
 }
 
 inline int grid_for(long long total, int block = 256) {
@@ -374,9 +401,9 @@ int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, i
   return VFX_OK;
 }
 
-int mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, float* xlog,
+int mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, const int* ext_frames, float* xlog,
                   float* unet_in, cudaStream_t st) {
-  mask_log_pack_kernel<<<grid_for((long long)B * Tp * 128), 256, 0, st>>>(lin, mel, B, T, Tp, xlog, unet_in);
+  mask_log_pack_kernel<<<grid_for((long long)B * Tp * 128), 256, 0, st>>>(lin, mel, B, T, Tp, ext_frames, xlog, unet_in);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
@@ -388,19 +415,26 @@ int unet_head(const float* x, int B, int T, int Tp, const float* w, const float*
   return VFX_OK;
 }
 
-int voc_normalize(const float* mel, int B, int T, int Tc, int input_is_log, const float* tab,
-                      void* cond, int precision, cudaStream_t st) {
+int voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames, int input_is_log, const float* tab,
+                  void* cond, int precision, cudaStream_t st) {
   const int g = grid_for((long long)B * Tc * 128);
   if (precision == VFX_PREC_BF16)
-    voc_normalize_kernel<__nv_bfloat16><<<g, 256, 0, st>>>(mel, B, T, Tc, input_is_log, tab,
+    voc_normalize_kernel<__nv_bfloat16><<<g, 256, 0, st>>>(mel, B, T, Tc, ext_frames, input_is_log, tab,
                                                            reinterpret_cast<__nv_bfloat16*>(cond));
   else if (precision == VFX_PREC_FP16)
-    voc_normalize_kernel<__half><<<g, 256, 0, st>>>(mel, B, T, Tc, input_is_log, tab, reinterpret_cast<__half*>(cond));
+    voc_normalize_kernel<__half><<<g, 256, 0, st>>>(mel, B, T, Tc, ext_frames, input_is_log, tab, reinterpret_cast<__half*>(cond));
   else if (precision == VFX_PREC_TF32)
-    voc_normalize_kernel<tf32_t><<<g, 256, 0, st>>>(mel, B, T, Tc, input_is_log, tab, reinterpret_cast<tf32_t*>(cond));
+    voc_normalize_kernel<tf32_t><<<g, 256, 0, st>>>(mel, B, T, Tc, ext_frames, input_is_log, tab, reinterpret_cast<tf32_t*>(cond));
   else
-    voc_normalize_kernel<float><<<g, 256, 0, st>>>(mel, B, T, Tc, input_is_log, tab,
+    voc_normalize_kernel<float><<<g, 256, 0, st>>>(mel, B, T, Tc, ext_frames, input_is_log, tab,
                                                    reinterpret_cast<float*>(cond));
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+int ragged_extents(const int* lens, int B, int L_cap, int* ext, cudaStream_t st) {
+  VFX_REQUIRE(lens && ext && B > 0 && L_cap > 1024, "ragged_extents: bad arguments");
+  ragged_extents_kernel<<<ceil_div(B, 128), 128, 0, st>>>(lens, B, L_cap, ext);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
@@ -418,22 +452,22 @@ int cast_rows(const float* x, long long n, void* y, int precision, cudaStream_t 
   return VFX_OK;
 }
 
-int reflect_pad3(void* buf, int B, int L, int C, int precision, cudaStream_t st) {
+int reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precision, cudaStream_t st) {
   VFX_REQUIRE(L >= 4, "reflect_pad3: length %d too short for reflection pad 3", L);
   const int g = grid_for((long long)B * 6 * C);
   if (precision == VFX_PREC_BF16 || precision == VFX_PREC_FP16)      // a 2-byte copy either way
-    reflect_pad3_kernel<__nv_bfloat16><<<g, 256, 0, st>>>(reinterpret_cast<__nv_bfloat16*>(buf), B, L, C);
+    reflect_pad3_kernel<__nv_bfloat16><<<g, 256, 0, st>>>(reinterpret_cast<__nv_bfloat16*>(buf), B, L, C, ext_len);
   else
-    reflect_pad3_kernel<float><<<g, 256, 0, st>>>(reinterpret_cast<float*>(buf), B, L, C);
+    reflect_pad3_kernel<float><<<g, 256, 0, st>>>(reinterpret_cast<float*>(buf), B, L, C, ext_len);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
 
 int voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len,
-             float scale, float* out, cudaStream_t st) {
+             const int* ext_gen, const int* ext_len, float scale, float* out, cudaStream_t st) {
   VFX_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0, "voc_post: x and w must be 16-byte aligned");
   dim3 grid(ceil_div(out_len, POST_RUN * POST_GROUPS), B);
-  voc_post_kernel<<<grid, 16 * POST_GROUPS, 0, st>>>(x, L, w, bias, lo, out_len, scale, out);
+  voc_post_kernel<<<grid, 16 * POST_GROUPS, 0, st>>>(x, L, w, bias, lo, out_len, ext_gen, ext_len, scale, out);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

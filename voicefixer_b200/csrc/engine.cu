@@ -6,6 +6,7 @@
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <mutex>
 #include <unordered_map>
 #include <vector>
@@ -82,9 +83,20 @@ struct Bump {
 
 struct Ctx {
   vfx_engine* e; cudaStream_t st; Bump* ws; bool dry; int mode; int rc = VFX_OK;
+  const int* ext = nullptr;   // ragged batch: per-item extents ext[EXT_LEVELS][B] on the device (NULL = equal lengths)
+  int ext_B = 0;
   bool train() const { return mode == VFX_MODE_TRAIN_BN; }
   int prec() const { return e->precision; }
+  const int* ext_at(int level) const { return ext ? ext + (size_t)level * ext_B : nullptr; }
 };
+
+// workspace of the ragged path's extent table (taken from the planner's slack, see dry_run)
+size_t ext_table_bytes(int B) { return ((size_t)EXT_LEVELS * B * sizeof(int) + 255) & ~(size_t)255; }
+
+// Sets a convolution's per-item extents (vfx_conv_desc.seq_in / seq_out; NULL on an equal-length batch)
+void set_seq(vfx_conv_desc& d, const int* seq_in, const int* seq_out, int axis) {
+  d.seq_in = seq_in; d.seq_out = seq_out; d.seq_axis = axis;
+}
 
 struct ProfScope {
   Ctx& c; bool on;
@@ -217,8 +229,11 @@ struct BlockScratch { void* opA; float* rawH; void* opH; float* rawS; void* opX;
 //               DecoderBlockRes.bn1)
 struct BlockFuse { bool opA_ready = false; const char* next_bn = nullptr; float next_slope = 0.01f; };
 
+// seq: the items' extents along H at this level (ragged batch; NULL = all H rows).  The eval BatchNorms (bn_act) are
+// pointwise, so rows beyond an item's extent only carry values that the convolutions never read.
 int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, int B, int H, int W,
-               int Cin, int Cout, float* out, long long ld_out, const BlockScratch& s, const BlockFuse& fz = BlockFuse()) {
+               int Cin, int Cout, float* out, long long ld_out, const BlockScratch& s, const int* seq,
+               const BlockFuse& fz = BlockFuse()) {
   const int prec = c.prec();
   const long long P = (long long)H * W;
   const bool fuse = !c.train();
@@ -242,6 +257,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
   if (fuse) {     // conv1 with bn2 folded in: h = lrelu(conv1f(a) + b) straight into the operand buffer
     vfx_conv_desc d = conv_base(s.opA, B, H, W, Cop, getw(c, p + ".conv1f.w", (size_t)9 * Cout * Cop, prec), Cout);
     taps3x3(d, (long long)Cout * Cop);
+    set_seq(d, seq, seq, 0);
     d.bias = getf(c, p + ".conv1f.b", Cout);
     set_act(d, s.opH, Cout, 0, VFX_ACT_LRELU, 0.01f);
     snprintf(tg, sizeof(tg), "unet.conv3x3.W%d.%dto%d", W, Cin, Cout);
@@ -249,6 +265,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
   } else {
     vfx_conv_desc d = conv_base(s.opA, B, H, W, Cop, getw(c, p + ".conv1.w", (size_t)9 * Cout * Cop, prec), Cout);
     taps3x3(d, (long long)Cout * Cop);
+    set_seq(d, seq, seq, 0);
     set_raw(d, s.rawH, Cout, 0);
     snprintf(tg, sizeof(tg), "unet.conv3x3.W%d.%dto%d", W, Cin, Cout);
     VFX_TRY(run_conv(c, prec, d, c.e->profile > 1 ? tg : "unet.conv3x3"));
@@ -264,6 +281,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
     }
     vfx_conv_desc d = conv_base(xin, B, H, W, Cop, getw(c, p + ".sc.w", (size_t)Cout * Cop, prec), Cout);
     d.ntaps = 1;
+    set_seq(d, seq, seq, 0);
     d.bias = getf(c, p + ".sc.b", Cout);
     set_raw(d, s.rawS, Cout, 0);
     VFX_TRY(run_conv(c, prec, d, "unet.shortcut"));
@@ -272,6 +290,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
   {
     vfx_conv_desc d = conv_base(s.opH, B, H, W, Cout, getw(c, p + ".conv2.w", (size_t)9 * Cout * Cout, prec), Cout);
     taps3x3(d, (long long)Cout * Cout);
+    set_seq(d, seq, seq, 0);
     set_res(d, res, ld_res, 0);
     set_raw(d, out, ld_out, 0);
     if (fuse && fz.next_bn) {   // the consumer's eval BatchNorm + activation, fused: s.opA = act(bn(out))
@@ -319,9 +338,10 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
       BlockFuse fz;
       fz.opA_ready = j > 1;                               // produced by block j-1's conv2 epilogue
       if (j < 4) { snprintf(nbn[j], sizeof(nbn[j]), "unet.enc%d.b%d.bn1", l, j + 1); fz.next_bn = nbn[j]; }
-      if (j == 1) VFX_TRY(conv_block(c, name, x, Cx, B, H, W, Cx, C, skip, 2 * C, s, fz));
-      else VFX_TRY(conv_block(c, name, skip, 2 * C, B, H, W, C, C, skip, 2 * C, s, fz));
+      if (j == 1) VFX_TRY(conv_block(c, name, x, Cx, B, H, W, Cx, C, skip, 2 * C, s, c.ext_at(EXT_UNET0 + l - 1), fz));
+      else VFX_TRY(conv_block(c, name, skip, 2 * C, B, H, W, C, C, skip, 2 * C, s, c.ext_at(EXT_UNET0 + l - 1), fz));
     }
+    // (every extent is a multiple of 64 >> (l - 1): the 2 x 2 windows of an item's rows never straddle its end)
     ProfScope ps(c, "unet.pool", 0.0, (double)B * H * W * C * 5.0);
     if (!c.dry) VFX_TRY(avgpool2x2(skip, (long long)H * W * 2 * C, (long long)W * 2 * C, 2 * C, B, H, W, C, pool[l], c.st));
     x = pool[l]; Cx = C;
@@ -329,7 +349,7 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
   // ---- centre block (in place on pool[6]): conv_block7
   {
     BlockFuse fz; fz.next_bn = "unet.dec1.bn1"; fz.next_slope = 0.0f;      // relu(bn1(x)) before the first ConvTranspose
-    VFX_TRY(conv_block(c, "unet.center", pool[6], 384, B, Hl[6], Wl[6], 384, 384, pool[6], 384, s, fz));
+    VFX_TRY(conv_block(c, "unet.center", pool[6], 384, B, Hl[6], Wl[6], 384, 384, pool[6], 384, s, c.ext_at(EXT_UNET0 + 6), fz));
   }
   float* xd = pool[6];
   int Cd = 384;
@@ -358,6 +378,7 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
             ++n;
           }
         d.ntaps = n;
+        set_seq(d, c.ext_at(EXT_UNET0 + l), c.ext_at(EXT_UNET0 + l - 1), 0);
         set_raw(d, cat[l], 2 * Cout, 0);
         VFX_TRY(run_conv(c, prec, d, "unet.convT"));
       }
@@ -372,14 +393,14 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
       if (j < 5) { snprintf(nbn, sizeof(nbn), "unet.dec%d.b%d.bn1", i, j + 1); fz.next_bn = nbn; }
       else if (i < 6) { snprintf(nbn, sizeof(nbn), "unet.dec%d.bn1", i + 1); fz.next_bn = nbn; fz.next_slope = 0.0f; }
       else { snprintf(nbn, sizeof(nbn), "unet.after.bn1"); fz.next_bn = nbn; }
-      if (j == 2) VFX_TRY(conv_block(c, name, cat[l], 2 * Cout, B, OH, OW, 2 * Cout, Cout, dl, Cout, s, fz));
-      else VFX_TRY(conv_block(c, name, dl, Cout, B, OH, OW, Cout, Cout, dl, Cout, s, fz));
+      if (j == 2) VFX_TRY(conv_block(c, name, cat[l], 2 * Cout, B, OH, OW, 2 * Cout, Cout, dl, Cout, s, c.ext_at(EXT_UNET0 + l - 1), fz));
+      else VFX_TRY(conv_block(c, name, dl, Cout, B, OH, OW, Cout, Cout, dl, Cout, s, c.ext_at(EXT_UNET0 + l - 1), fz));
     }
     xd = dl; Cd = Cout;
   }
   {
     BlockFuse fz; fz.opA_ready = true;                   // dec6.b5 produced lrelu(after.bn1(x))
-    VFX_TRY(conv_block(c, "unet.after", xd, 32, B, Tp, 127, 32, 32, xd, 32, s, fz));
+    VFX_TRY(conv_block(c, "unet.after", xd, 32, B, Tp, 127, 32, 32, xd, 32, s, c.ext_at(EXT_UNET0), fz));
   }
   *feat_out = xd;
   return c.rc;
@@ -430,7 +451,7 @@ int bn_gru(Ctx& c, const std::string& p, const float* x, int B, int T, void* op,
     VFX_TRY(run_conv(c, prec, d, "dn.gru_in"));
     if (!c.dry && c.rc == VFX_OK) {
       ProfScope ps(c, "dn.gru", 2.0 * M * 2 * 768 * 256, 0.0);
-      VFX_TRY(gru_layer(gi, whh, bhh, B, T, outs[layer], c.st));
+      VFX_TRY(gru_layer(gi, whh, bhh, B, T, c.ext_at(EXT_FRAMES), outs[layer], c.st));
     }
     if (layer == 0) { int rc; in = dn_operand(c, y0, M, 512, op, &rc); VFX_TRY(rc); }
   }
@@ -443,6 +464,8 @@ int relu_inplace(Ctx& c, float* x, int B, int T, int C) {
                 (long long)T * C, C, c.st);
 }
 
+// Ragged batch: every op but the GRU recurrence is per frame (Linear GEMMs over B*T rows, eval BatchNorm and ReLU via
+// bn_act), so frames beyond an item's end only produce values that no later kernel reads.
 int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop, float* lin_out) {
   const long long M = (long long)B * T;
   const int prec = c.prec();
@@ -482,7 +505,7 @@ int analysis_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop
     VFX_TRY(denoiser_forward(c, mel, B, T, drop, lin));
     c.ws->reset(m1);
   }
-  if (!c.dry) VFX_TRY(mask_log_pack(lin, mel, B, T, Tp, xlog, unet_in, c.st));
+  if (!c.dry) VFX_TRY(mask_log_pack(lin, mel, B, T, Tp, c.ext_at(EXT_FRAMES), xlog, unet_in, c.st));
   float* feat = nullptr;
   VFX_TRY(unet_forward(c, unet_in, B, Tp, &feat));
   const float* hw = getf(c, "unet.head.w", 32);
@@ -519,6 +542,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
     vfx_conv_desc d = conv_base(in, B, 1, Tc, Cin, getw(c, p + ".w", (size_t)3 * 512 * Cin, prec), 512);
     d.ntaps = 3;
     for (int k = 0; k < 3; ++k) { d.dw[k] = k - 1; d.w_off[k] = (long long)k * 512 * Cin; }
+    set_seq(d, c.ext_at(EXT_COND), c.ext_at(EXT_COND), 1);
     d.bias = getf(c, p + ".b", 512);
     void* out = pp[i & 1];
     if (i == 4) {   // last ELU output goes to rows 3..Tc+2 of the reflect-padded buffer
@@ -530,13 +554,14 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
     VFX_TRY(run_conv(c, prec, d, "voc.condnet"));
     in = out; Cin = 512;
   }
-  if (!c.dry) VFX_TRY(reflect_pad3((void*)in, B, Tc, 512, prec, c.st));
+  if (!c.dry) VFX_TRY(reflect_pad3((void*)in, B, Tc, 512, c.ext_at(EXT_COND), prec, c.st));
   // ---- ReflectionPad1d(3) + Conv1d(512,1024,k7) + LeakyReLU(0.2); the x + sin x of the first
   //      UpsampleNet (modules.py:504) is applied in the same epilogue.
   {
     vfx_conv_desc d = conv_base(in, B, 1, Tc + 6, 512, getw(c, "voc.pre.w", (size_t)7 * 1024 * 512, prec), 1024);
     d.ntaps = 7; d.Wq = Tc; d.OW = Tc;
     for (int k = 0; k < 7; ++k) { d.dw[k] = k; d.w_off[k] = (long long)k * 1024 * 512; }
+    set_seq(d, c.ext_at(EXT_COND_PAD), c.ext_at(EXT_COND), 1);
     d.bias = getf(c, "voc.pre.b", 1024);
     set_act(d, U, 1024, 0, VFX_ACT_LRELU_XSINX, 0.2f);
     VFX_TRY(run_conv(c, prec, d, "voc.pre"));
@@ -548,6 +573,9 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
   for (int j = 0; j < 4; ++j) {
     const int Ci = VOC_CIN[j], Co = VOC_COUT[j], u = VOC_U[j];
     const long long Lout = Lin * u;
+    // ragged batch: items' lengths at this up-sampler's input (= rows of its reshaped output view) and output rate
+    const int* ext_in = c.ext_at(j == 0 ? EXT_COND : EXT_UP0 + j - 1);
+    const int* ext_out = c.ext_at(EXT_UP0 + j);
     char up_tag[32], c1_tag[32], c2_tag[32];
     snprintf(up_tag, sizeof(up_tag), "voc.up%d", j);
     snprintf(c1_tag, sizeof(c1_tag), "voc.rs%d.c1", j);
@@ -570,6 +598,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
         if (grp == 0) { d.dw[0] = 0; d.w_off[0] = pad * mat; d.dw[1] = -1; d.w_off[1] = (pad + u) * mat; r0 = 0; }
         else          { d.dw[0] = 1; d.w_off[0] = 0;         d.dw[1] = 0;  d.w_off[1] = u * mat;         r0 = nA; }
         d.bias = bias; d.bias_mod = Co;
+        set_seq(d, ext_in, ext_in, 1);
         set_raw(d, X, (long long)u * Co, r0 * Co);
         if (enc) { d.raw_enc = 1; d.enc_slope = 0.01f; }
         else set_act(d, A0, (long long)u * Co, r0 * Co, VFX_ACT_LRELU, 0.01f);
@@ -593,7 +622,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
       if (fuse_tf32 || fuse_pairs) {
         vfx_pair_desc pd;
         memset(&pd, 0, sizeof(pd));
-        pd.precision = prec; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co;
+        pd.precision = prec; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co; pd.lens = ext_out;
         pd.w1 = getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec); pd.b1 = getf(c, p + ".c1.b", Co);
         pd.w2 = getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec); pd.b2 = getf(c, p + ".c2.b", Co);
         if (fuse_tf32) {
@@ -623,6 +652,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
                                     getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec), Co);
         d.ntaps = 3;
         for (int k = 0; k < 3; ++k) { d.dw[k] = (k - 1) * dil; d.w_off[k] = (long long)k * Co * Co; }
+        set_seq(d, ext_out, ext_out, 1);
         d.bias = getf(c, p + ".c1.b", Co);
         set_act(d, Hh, Co, 0, VFX_ACT_LRELU, 0.01f);
         char c1d[48];
@@ -633,6 +663,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
         vfx_conv_desc d = conv_base(Hh, B, 1, (int)Lout, Co, getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec), Co);
         d.ntaps = 3;
         for (int k = 0; k < 3; ++k) { d.dw[k] = k - 1; d.w_off[k] = (long long)k * Co * Co; }
+        set_seq(d, ext_out, ext_out, 1);
         d.bias = getf(c, p + ".c2.b", Co);
         set_res(d, X, Co, 0);
         if (enc) {
@@ -661,7 +692,8 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
   const float* pw = getf(c, "voc.post.w", 7 * 64);
   const float* pb = getf(c, "voc.post.b", 1);
   ProfScope ps(c, "voc.post", 2.0 * B * out_len * 7 * 64, (double)B * S * 64 * 4);
-  if (!c.dry && c.rc == VFX_OK) VFX_TRY(voc_post(X, B, (int)S, pw, pb, lo, (int)out_len, scale, wav_out, c.st));
+  if (!c.dry && c.rc == VFX_OK) VFX_TRY(voc_post(X, B, (int)S, pw, pb, lo, (int)out_len, c.ext_at(EXT_UP0 + 3),
+                                                         c.ext_at(EXT_SAMPLES), scale, wav_out, c.st));
   c.ws->reset(m0);
   return c.rc;
 }
@@ -672,7 +704,7 @@ int vocoder_forward(Ctx& c, const float* mel, int B, int T, int input_is_log, fl
   const size_t m0 = c.ws->mark();
   void* cond = c.ws->raw((size_t)B * Tc * 128 * c.e->esz());
   const float* tab = getf(c, "voc.mel_tab", 129);
-  if (!c.dry && c.rc == VFX_OK) VFX_TRY(voc_normalize(mel, B, T, Tc, input_is_log, tab, cond, c.prec(), c.st));
+  if (!c.dry && c.rc == VFX_OK) VFX_TRY(voc_normalize(mel, B, T, Tc, c.ext_at(EXT_FRAMES), input_is_log, tab, cond, c.prec(), c.st));
   VFX_TRY(vocoder_generator(c, cond, B, Tc, wav_out, trim_len, scale));
   c.ws->reset(m0);
   return c.rc;
@@ -685,11 +717,18 @@ int frontend_forward(Ctx& c, const float* wav, int B, int L, float* mel, float* 
   const int* fl = (const int*)get(c, "fe.fb_len", 128 * 4);
   if (c.dry || c.rc != VFX_OK) return c.rc;
   ProfScope ps(c, "fe.stft_mel", (double)B * T * (5.0 * 1024 * 10 + 2.0 * 2050), (double)B * L * 4);
-  return stft_mel(wav, B, L, T, c.e->d_window, c.e->d_tw, fbT, fs, fl, mel, sp, c.st);
+  return stft_mel(wav, B, L, T, c.ext_at(EXT_SAMPLES), c.ext_at(EXT_FRAMES), c.e->d_window, c.e->d_tw, fbT, fs, fl, mel,
+                  sp, c.st);
 }
 
-int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop, float* wav_out) {
+// lens (ragged batch, mode 0): per-item lengths on the device; L is then the capacity (row stride of wav / wav_out)
+int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop, const int* lens, float* wav_out) {
   const int T = 1 + L / 441;
+  if (lens) {
+    int* ext = c.ws->alloc<int>((size_t)EXT_LEVELS * B);
+    if (!c.dry) VFX_TRY(ragged_extents(lens, B, L, ext, c.st));
+    c.ext = ext; c.ext_B = B;
+  }
   float* mel = c.ws->alloc<float>((size_t)B * T * 128);
   float* mel_log = c.ws->alloc<float>((size_t)B * T * 128);
   VFX_TRY(frontend_forward(c, wav, B, L, mel, nullptr));
@@ -809,14 +848,15 @@ static int dry_run(vfx_engine* e, int B, int T, int L, size_t* bytes) {
   Bump ws(nullptr, 0);
   Ctx c{e, nullptr, &ws, true, VFX_MODE_TRAIN_BN};
   int r;
-  if (L > 0) r = restore_forward(c, nullptr, B, L, nullptr, nullptr);
+  if (L > 0) r = restore_forward(c, nullptr, B, L, nullptr, nullptr, nullptr);
   else {
     float* mel = ws.alloc<float>((size_t)B * T * 128);
     const bool voc_only = e->finalized && !(e->parts & VFX_PART_ANALYSIS);
     r = voc_only ? VFX_OK : analysis_forward(c, mel, B, T, nullptr, mel);
     if (r == VFX_OK) r = vocoder_forward(c, mel, B, T, 1, nullptr, -1, 1.f);
   }
-  *bytes = ws.peak + 4096;
+  // the slack also holds vfx_restore_ragged's extent table, so one workspace size serves both entry points
+  *bytes = ws.peak + std::max<size_t>(4096, ext_table_bytes(B));
   return r;
 }
 
@@ -957,19 +997,30 @@ int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav
   VFX_FINISH(c, ws);
 }
 
-int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
-                float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
+static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
+                         const int* lens, float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
   VFX_NEED_ANALYSIS(e);
   VFX_REQUIRE(wav && wav_out && B > 0 && workspace, "restore: bad arguments");
   VFX_REQUIRE(mode == VFX_MODE_EVAL || mode == VFX_MODE_TRAIN_BN, "restore: bad mode %d", mode);
   VFX_REQUIRE(L > 1024, "restore: L=%d must exceed 1024 samples", L);
-  VFX_PREFLIGHT(mode, restore_forward(c, wav, B, L, nullptr, wav_out));
+  VFX_PREFLIGHT(mode, restore_forward(c, wav, B, L, nullptr, lens, wav_out));
   Bump ws(workspace, workspace_bytes);
   Ctx c{e, (cudaStream_t)stream, &ws, false, mode};
-  int r = restore_forward(c, wav, B, L, drop_masks, wav_out);
+  int r = restore_forward(c, wav, B, L, drop_masks, lens, wav_out);
   if (r != VFX_OK) return r;
   VFX_FINISH(c, ws);
+}
+
+int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
+                float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return restore_entry(e, wav, B, L, mode, drop_masks, nullptr, wav_out, workspace, workspace_bytes, stream);
+}
+
+int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* wav_out,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_REQUIRE(lens, "restore_ragged: lens is null");
+  return restore_entry(e, wav, B, L_cap, VFX_MODE_EVAL, nullptr, lens, wav_out, workspace, workspace_bytes, stream);
 }
 
 int vfx_hf_cut(vfx_engine* e, const float* wav, int B, int L, float ratio, float* wav_out, int* cut_bins,
@@ -1001,7 +1052,13 @@ int vfx_resstack_pair(const vfx_pair_desc* d, void* stream) {
 }
 
 int vfx_gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out, void* stream) {
-  return gru_layer(gi, whh_t, bhh, B, T, out, (cudaStream_t)stream);
+  return gru_layer(gi, whh_t, bhh, B, T, nullptr, out, (cudaStream_t)stream);
+}
+
+int vfx_gru_layer_ragged(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens,
+                         float* out, void* stream) {
+  VFX_REQUIRE(lens, "gru_layer_ragged: lens is null");
+  return gru_layer(gi, whh_t, bhh, B, T, lens, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

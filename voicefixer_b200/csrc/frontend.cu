@@ -12,6 +12,7 @@ namespace vfx {
 namespace {
 
 __global__ void __launch_bounds__(256) stft_mel_kernel(const float* __restrict__ wav, int L, int T,
+                                                       const int* __restrict__ ext_len, const int* __restrict__ ext_frames,
                                                        const float* __restrict__ window,
                                                        const float2* __restrict__ tw,
                                                        const float* __restrict__ fbT,
@@ -22,6 +23,9 @@ __global__ void __launch_bounds__(256) stft_mel_kernel(const float* __restrict__
   __shared__ float mag[1025];
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const float* x = wav + (long long)b * L;
+  // ragged batch: item b has its own length Lb <= L (the row stride) and frames t < 1 + Lb / 441; it is reflected at Lb
+  const int Lb = ext_len ? ext_len[b] : L;
+  if (ext_frames && t >= ext_frames[b]) return;
   const int base = t * 441 - 1024;
   // z[n] = xw[2n] + i*xw[2n+1], reflect padding at both ends (F.pad(..., mode='reflect'))
   for (int n = tid; n < 1024; n += 256) {
@@ -30,7 +34,7 @@ __global__ void __launch_bounds__(256) stft_mel_kernel(const float* __restrict__
     for (int h = 0; h < 2; ++h) {
       int i = base + 2 * n + h;
       if (i < 0) i = -i;
-      if (i >= L) i = 2 * (L - 1) - i;
+      if (i >= Lb) i = 2 * (Lb - 1) - i;
       v[h] = x[i] * window[2 * n + h];
     }
     bufA[n] = make_float2(v[0], v[1]);
@@ -56,13 +60,13 @@ __global__ void __launch_bounds__(256) stft_mel_kernel(const float* __restrict__
 
 }  // namespace
 
-int stft_mel(const float* wav, int B, int L, int T, const float* window, const float2* tw,
-             const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
+int stft_mel(const float* wav, int B, int L, int T, const int* ext_len, const int* ext_frames, const float* window,
+             const float2* tw, const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
              cudaStream_t st) {
   VFX_REQUIRE(L > 1024, "frontend: L=%d must exceed 1024 (reflect padding of n_fft/2)", L);
   VFX_REQUIRE(T == 1 + L / 441, "frontend: T=%d inconsistent with L=%d", T, L);
   dim3 grid(T, B);
-  stft_mel_kernel<<<grid, 256, 0, st>>>(wav, L, T, window, tw, fbT, fb_start, fb_len, mel, sp);
+  stft_mel_kernel<<<grid, 256, 0, st>>>(wav, L, T, ext_len, ext_frames, window, tw, fbT, fb_start, fb_len, mel, sp);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

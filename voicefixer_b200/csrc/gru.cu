@@ -39,7 +39,7 @@ constexpr int RPC = 3 * UPC;     // gate rows per CTA = 96
 template <int G, int KQ>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(32 * KQ, 1)
 gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t,
-                   const float* __restrict__ bhh, int B, int T, float* __restrict__ out) {
+                   const float* __restrict__ bhh, int B, int T, const int* __restrict__ lens, float* __restrict__ out) {
   constexpr int KW = H / KQ, NT = 32 * KQ;
   extern __shared__ __align__(16) uint8_t gru_smem[];
   float (*h_s)[G][H] = reinterpret_cast<float (*)[G][H]>(gru_smem);                       // [2][G][H]
@@ -68,6 +68,8 @@ gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t
   const bool fin = tid < UPC * G;
   const int fu = tid % UPC, fg = tid / UPC;
   const bool fvalid = fin && (b0 + fg) < B;
+  // ragged batch: this item's own length; its backward direction starts at Tb - 1 and steps >= Tb store nothing
+  const int Tb = fvalid && lens ? lens[b0 + fg] : T;
   const int hu = rank * UPC + fu;
   float b_r = 0.f, b_z = 0.f, b_n = 0.f;
   if (fin) {
@@ -101,14 +103,14 @@ gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t
   float pr[2] = {0.f, 0.f}, pz[2] = {0.f, 0.f}, pn[2] = {0.f, 0.f};
 #pragma unroll
   for (int s = 0; s < 2; ++s)
-    if (fvalid && s < T) {
-      const int ts = dir == 0 ? s : T - 1 - s;
+    if (fvalid && s < Tb) {
+      const int ts = dir == 0 ? s : Tb - 1 - s;
       const float* p = gbase + (long long)ts * gstride;
       pr[s] = p[0]; pz[s] = p[H]; pn[s] = p[2 * H];
     }
 
   for (int step = 0; step < T; ++step) {
-    const int t = dir == 0 ? step : T - 1 - step;
+    const int t = dir == 0 ? step : Tb - 1 - step;      // < 0 (backward) or >= Tb (forward) past this item's end
     const int cur = step & 1, nxt = cur ^ 1;
     const bool last = step + 1 == T;
     if (tid == 0 && !last) {      // arm the mbarrier of the buffer this step's exchange fills
@@ -117,7 +119,7 @@ gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t
     }
     const float gir = pr[0], giz = pz[0], gin = pn[0];
     pr[0] = pr[1]; pz[0] = pz[1]; pn[0] = pn[1];
-    if (fvalid && step + 2 < T) {
+    if (fvalid && step + 2 < Tb) {
       const int tn = dir == 0 ? t + 2 : t - 2;
       const float* p = gbase + (long long)tn * gstride;
       pr[1] = p[0]; pz[1] = p[H]; pn[1] = p[2 * H];
@@ -165,7 +167,7 @@ gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t
           asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
                        ::"r"(rem_h[c] + off), "r"(__float_as_uint(hn)), "r"(rem_bar[c] + 8u * nxt) : "memory");
       }
-      if (fvalid) out[((long long)(b0 + fg) * T + t) * (2 * H) + dir * H + hu] = hn;
+      if (fvalid && step < Tb) out[((long long)(b0 + fg) * T + t) * (2 * H) + dir * H + hu] = hn;
     }
     if (!last) {                  // wait until all 8 CTAs' contributions to h[nxt] have landed here
       const uint32_t lb = (uint32_t)__cvta_generic_to_shared(&hbar[nxt]);
@@ -183,7 +185,8 @@ gru_cluster_kernel(const float* __restrict__ gi, const float* __restrict__ whh_t
 }
 
 template <int G, int KQ>
-int launch(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out, cudaStream_t st) {
+int launch(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens, float* out,
+           cudaStream_t st) {
   constexpr int NT = 32 * KQ;
   const int groups = (B + G - 1) / G;
   const size_t smem = sizeof(float) * (2 * G * H + 2 * KQ * G * RPC) + 16;
@@ -194,26 +197,26 @@ int launch(const float* gi, const float* whh_t, const float* bhh, int B, int T, 
     VFX_CUDA_CHECK(cudaFuncSetAttribute(gru_cluster_kernel<G, KQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (dev < 64) attr_set[dev] = true;
   }
-  gru_cluster_kernel<G, KQ><<<2 * groups * CL, NT, smem, st>>>(gi, whh_t, bhh, B, T, out);
+  gru_cluster_kernel<G, KQ><<<2 * groups * CL, NT, smem, st>>>(gi, whh_t, bhh, B, T, lens, out);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
 
 }  // namespace
 
-int gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out,
+int gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens, float* out,
               cudaStream_t st) {
   VFX_REQUIRE(B > 0 && T > 0, "gru_layer: empty problem");
   // one wave: at most 16 clusters of 8 CTAs (128 of the 132 SMs, two clusters per GPC)
   static const int kq = getenv("VFX_GRU_KQ") ? atoi(getenv("VFX_GRU_KQ")) : 8;
   if (kq == 8) {
-    if (2 * ((B + 1) / 2) <= 16) return launch<2, 8>(gi, whh_t, bhh, B, T, out, st);
-    if (2 * ((B + 3) / 4) <= 16) return launch<4, 8>(gi, whh_t, bhh, B, T, out, st);
-    return launch<8, 8>(gi, whh_t, bhh, B, T, out, st);
+    if (2 * ((B + 1) / 2) <= 16) return launch<2, 8>(gi, whh_t, bhh, B, T, lens, out, st);
+    if (2 * ((B + 3) / 4) <= 16) return launch<4, 8>(gi, whh_t, bhh, B, T, lens, out, st);
+    return launch<8, 8>(gi, whh_t, bhh, B, T, lens, out, st);
   }
-  if (2 * ((B + 1) / 2) <= 16) return launch<2, 16>(gi, whh_t, bhh, B, T, out, st);
-  if (2 * ((B + 3) / 4) <= 16) return launch<4, 16>(gi, whh_t, bhh, B, T, out, st);
-  return launch<8, 16>(gi, whh_t, bhh, B, T, out, st);
+  if (2 * ((B + 1) / 2) <= 16) return launch<2, 16>(gi, whh_t, bhh, B, T, lens, out, st);
+  if (2 * ((B + 3) / 4) <= 16) return launch<4, 16>(gi, whh_t, bhh, B, T, lens, out, st);
+  return launch<8, 16>(gi, whh_t, bhh, B, T, lens, out, st);
 }
 
 }  // namespace vfx

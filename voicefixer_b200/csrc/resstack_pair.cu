@@ -10,6 +10,8 @@
 // the residual and the outputs.  Shared memory: 3 copies of h (48 KB bf16 C = 64, 96 KB tf32 C = 64 or 16-bit C = 128)
 // + 3 stages of (16 KB of a + C x 128 B of weights).
 //
+// Ragged batches (vfx_pair_desc.lens): item b is computed as if its length were lens[b]; tiles starting beyond it exit.
+//
 // Blocked form (impl 2): the two convolutions of conv_gemm_tc.cu per block of rows, h in the caller's scratch.
 #include <string.h>
 #include "tc_ptx.cuh"
@@ -49,8 +51,10 @@ __global__ void __launch_bounds__(256) pair_fused_kernel(const __grid_constant__
   uint8_t* const hgen = smem_raw + (hbase - smem_u32(smem_raw));
 
   const int tid = threadIdx.x, chunk = tid & 7, lrow = tid >> 3, wg = tid >> 7, w = (tid >> 5) & 3, l = tid & 31;
-  const int L = d.L, b = blockIdx.y, r0 = blockIdx.x * P_ROWS;
-  const long long item = (long long)b * L * C;
+  const int b = blockIdx.y, r0 = blockIdx.x * P_ROWS;
+  const long long item = (long long)b * d.L * C;
+  const int L = d.lens ? d.lens[b] : d.L;         // this item's length (ragged batch): its rows beyond are padding
+  if (r0 >= L) return;
   const char* __restrict__ A = reinterpret_cast<const char*>(d.a) + item * ESZ;
   const char* __restrict__ W1 = reinterpret_cast<const char*>(d.w1);
   const char* __restrict__ W2 = reinterpret_cast<const char*>(d.w2);
@@ -237,7 +241,7 @@ int resstack_pair(const vfx_pair_desc& d, cudaStream_t st) {
                              : ((prec == VFX_PREC_BF16 || prec == VFX_PREC_FP16) && (d.C == 64 || d.C == 128) && !d.stream_enc);
   if (!shape_ok || d.impl < 0 || d.impl > 3) return VFX_ERR_UNSUPPORTED;
   VFX_REQUIRE(d.a && d.x && d.w1 && d.w2 && d.b1 && d.b2 && d.B > 0 && d.L > 0 && d.dilation > 0, "resstack_pair: bad arguments");
-  if (d.impl == 2) return pair_blocked(d, prec, st);
+  if (d.impl == 2) return d.lens ? VFX_ERR_UNSUPPORTED : pair_blocked(d, prec, st);
   if (((uintptr_t)d.a & 15) || ((uintptr_t)d.w1 & 15) || ((uintptr_t)d.w2 & 15)) return VFX_ERR_UNSUPPORTED;
   if (tf32) return launch_fused<64, 0>(d, st);
   if (prec == VFX_PREC_BF16) return d.C == 64 ? launch_fused<64, 1>(d, st) : launch_fused<128, 1>(d, st);

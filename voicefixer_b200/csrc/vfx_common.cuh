@@ -111,27 +111,44 @@ int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, 
 int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st);
 int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W,
                int C, float* y, cudaStream_t st);
-int stft_mel(const float* wav, int B, int L, int T, const float* window, const float2* tw,
-             const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
+// Ragged batches: the kernels below that take `ext_*` / `lens` pointers (device int32 [B], NULL = every item spans the
+// whole tensor) read each item's own extent at that stage from the table ragged_extents() fills.
+enum {
+  EXT_SAMPLES = 0,          // L_b
+  EXT_FRAMES = 1,           // T_b = 1 + L_b / 441
+  EXT_UNET0 = 2,            // EXT_UNET0 + k, k = 0..6: Tp_b >> k, Tp_b = 64 * ceil(T_b / 64)
+  EXT_COND = 9,             // Tc_b = T_b + T_b % 2 + 4
+  EXT_COND_PAD = 10,        // Tc_b + 6 (reflect-padded condnet output)
+  EXT_UP0 = 11,             // EXT_UP0 + j, j = 0..3: up-sampler j's output length Tc_b * (7, 49, 147, 441)
+  EXT_LEVELS = 15
+};
+// lens[B] -> ext[EXT_LEVELS][B]; every length is clamped into [1025, L_cap] first
+int ragged_extents(const int* lens, int B, int L_cap, int* ext, cudaStream_t st);
+int stft_mel(const float* wav, int B, int L, int T, const int* ext_len, const int* ext_frames, const float* window,
+             const float2* tw, const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
              cudaStream_t st);
-int gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, float* out,
+int gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens, float* out,
               cudaStream_t st);
 // denoiser tail: clean = sigmoid(lin)*mel ; x = log10(clip(clean)); unet_in[b][t][f<127][2]
-int mask_log_pack(const float* lin_sig, const float* mel, int B, int T, int Tp, float* xlog,
+// (zero rows for ext_frames[b] <= t < Tp)
+int mask_log_pack(const float* lin_sig, const float* mel, int B, int T, int Tp, const int* ext_frames, float* xlog,
                   float* unet_in, cudaStream_t st);
 // unet head: out[b][t][f] = (f<127 ? bias + sum_c w[c]*x[b][t][f][c] : 0) + xlog[b][t][f]
 int unet_head(const float* x, int B, int T, int Tp, const float* w, const float* bias,
               const float* xlog, float* out, cudaStream_t st);
 // vocoder conditions: (from_log) / weight, dB, normalise, tail pad of -4 -> cond [B][Tc][128]
 // tab = mel_weight[128] ++ [min_level] (fp32, computed by the host exactly as the reference does)
-int voc_normalize(const float* mel, int B, int T, int Tc, int input_is_log, const float* tab,
+// (ragged: frames t < ext_frames[b] are converted, the rest of the rows is the -4 tail)
+int voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames, int input_is_log, const float* tab,
                   void* cond, int precision, cudaStream_t st);
 int cast_rows(const float* x, long long n, void* y, int precision, cudaStream_t st);
-// rows [0,3) and [3+L, L+6) of a [B][L+6][C] operand buffer <- reflection of the interior
-int reflect_pad3(void* buf, int B, int L, int C, int precision, cudaStream_t st);
+// rows [0,3) and [3+L, L+6) of a [B][L+6][C] operand buffer <- reflection of the interior (ragged: L_b = ext_len[b])
+int reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precision, cudaStream_t st);
 // final conv: lrelu0.2 -> reflect pad 3 -> conv k7 (64->1) -> tanh -> trim -> *scale
+// ragged (ext_gen, ext_len non-NULL): item b reflects at S_b = ext_gen[b], trims to L_b = ext_len[b] centred
+// (lo_b = (S_b - L_b) / 2) and writes zeros from L_b to out_len
 int voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len,
-             float scale, float* out, cudaStream_t st);
+             const int* ext_gen, const int* ext_len, float scale, float* out, cudaStream_t st);
 int hf_cut(const float* wav, int B, int L, float ratio, const float* window, const float2* tw,
            float* out, int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t hf_cut_workspace(int B, int L);

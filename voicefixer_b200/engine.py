@@ -220,14 +220,26 @@ class Engine:
                                              ws.numel(), _stream()), "vfx_vocoder_cond")
         return out
 
-    def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None):
-        """wav (B, L) on device -> restored wav (B, L) on device (one launch sequence)."""
+    def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None, lens=None):
+        """wav (B, L) on device -> restored wav (B, L) on device (one launch sequence).
+
+        lens (ragged batch, mode 0): int32 device tensor (B,) of per-item lengths <= L.  Row b of `wav` then holds
+        item b in its first lens[b] samples; row b of the result is bit-identical to restoring that item alone, followed
+        by zeros.  Lengths are read on the device (vfx_restore_ragged), so a captured graph serves any lengths."""
         wav = self._dev(wav)
         B, L = wav.shape
         if out is None:
             out = torch.empty_like(wav)
         if ws is None:
             ws = self._workspace(self.workspace_bytes(B, L))
+        if lens is not None:
+            if mode != 0 or drop_masks is not None:
+                raise ValueError("a ragged batch (lens) runs mode 0 only")
+            if not (lens.is_cuda and lens.dtype == torch.int32 and tuple(lens.shape) == (B,) and lens.is_contiguous()):
+                raise ValueError(f"lens must be a contiguous int32 CUDA tensor of shape ({B},)")
+            _lib.check(self.lib.vfx_restore_ragged(self.h, _ptr(wav), B, L, _ptr(lens), _ptr(out), _ptr(ws), ws.numel(),
+                                                   _stream()), "vfx_restore_ragged")
+            return out
         dm = None
         if drop_masks is not None:
             dm = drop_masks.to(device=wav.device, dtype=torch.uint8).contiguous()
@@ -235,10 +247,11 @@ class Engine:
                                         _stream()), "vfx_restore")
         return out
 
-    def make_graph(self, wav, out, mode=0):
+    def make_graph(self, wav, out, mode=0, lens=None):
         """Captures the whole restore() launch sequence (~360 kernels) for the given device buffers into a
         CUDA graph; returns an object whose .replay() re-runs it (inputs are read from `wav`, results land in
-        `out`).  Shapes, buffers and the workspace are frozen into the graph."""
+        `out`).  Shapes, buffers and the workspace are frozen into the graph.  With `lens` (ragged batch) the graph
+        reads the lengths from that buffer at every replay: refill it, like `wav`, before replay()."""
         assert wav.is_cuda and out.is_cuda and wav.shape == out.shape
         # the graph bakes raw device pointers in: it gets its OWN workspace, and the returned object keeps every
         # buffer it touches alive (a later, larger call may replace the engine's shared workspace)
@@ -247,13 +260,13 @@ class Engine:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                                # warm-up: one-time attribute / table setup
             for _ in range(2):
-                self.restore(wav, mode=mode, out=out, ws=ws)
+                self.restore(wav, mode=mode, out=out, ws=ws, lens=lens)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            self.restore(wav, mode=mode, out=out, ws=ws)
-        g._keep = (ws, wav, out, self.arena)
+            self.restore(wav, mode=mode, out=out, ws=ws, lens=lens)
+        g._keep = (ws, wav, out, lens, self.arena)
         return g
 
     def hf_cut(self, wav, ratio=0.95):
