@@ -125,7 +125,7 @@ int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav
 int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
                 float* wav_out, void* workspace, size_t workspace_bytes, void* stream);
 
-/* vfx_restore (mode 0) for B segments of DIFFERENT lengths: wav[B][L_cap] holds item b in its first lens[b] samples
+/* vfx_restore (mode 0; vfx_restore_ragged_mode below for mode 2) for B segments of DIFFERENT lengths: wav[B][L_cap] holds item b in its first lens[b] samples
  * (the rest is never read), lens[B] is a device int32 array.  wav_out[B][L_cap] receives item b's restoration in its
  * first lens[b] samples -- bit-identical to vfx_restore on that item alone -- and zeros after them.  A small kernel turns
  * lens into per-item extents at every stage (frames, UNet levels, vocoder rates) that the kernels read on the device, so
@@ -134,11 +134,30 @@ int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const u
 int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* wav_out,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* vfx_restore_ragged in either mode: vfx_restore_ragged is the mode-0 call (mode = VFX_MODE_EVAL, drop_masks = NULL).
+ * mode VFX_MODE_TRAIN_BN: every train-mode BatchNorm takes item b's statistics over its own rows only (its T_b frames in
+ * the denoiser, its Tp_b >> k rows of UNet level k), so row b is bit-identical to vfx_restore(mode 2) on item b alone
+ * with the masks drop_masks[:, b, :T_b].  drop_masks (optional): keep-masks uint8 [2][B][T_cap][512], T_cap =
+ * 1 + L_cap/441; rows t >= T_b are never read.  Precondition of mode 2 (the caller enforces it): every item has
+ * 1 + lens[b]/441 > 64 frames, because the reference refuses a 1 x 1 UNet centre in train mode; an item that breaks it
+ * gets finite, unspecified samples.  Workspace: vfx_workspace_bytes(e, B, L_cap). */
+int vfx_restore_ragged_mode(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, int mode,
+                            const uint8_t* drop_masks, float* wav_out, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* mode 1 pre-filter, VoiceFixer.remove_higher_frequency (voicefixer/base.py:87-104) with the
  * librosa 0.10.1 stft/istft defaults (n_fft 2048, hop 512, Hann, center, zero pad):
  * wav[B][L] -> wav_out[B][512*(L/512)].  Returns the per-item cut bin in cut_bins[B] (optional). */
 int vfx_hf_cut(vfx_engine* e, const float* wav, int B, int L, float ratio, float* wav_out,
                int* cut_bins, void* workspace, size_t workspace_bytes, void* stream);
+
+/* vfx_hf_cut for B items of DIFFERENT lengths: wav[B][L_cap] holds item b in its first lens[b] samples (device int32;
+ * clamped into [512, L_cap]; the rest of the row is never read).  Item b is filtered as if it were alone: its own
+ * 1 + L_b/512 frames set its cut bin, and wav_out[B][L_cap] receives its 512*(L_b/512) filtered samples followed by
+ * zeros.  lens_out[B] (device int32, optional) receives those lengths, so the result can feed vfx_restore_ragged(_mode)
+ * without a host round trip (mode 1 of a ragged batch).  Workspace: that of vfx_hf_cut for (B, L_cap). */
+int vfx_hf_cut_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float ratio, float* wav_out,
+                      int* lens_out, int* cut_bins, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- per-kernel test entry points (tests/ call the kernels through these) --------------- */
 

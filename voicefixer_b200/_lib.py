@@ -67,6 +67,8 @@ SIGNATURES = {
     "vfx_gru_layer": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
     "vfx_gru_layer_ragged": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "vfx_restore_ragged": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_restore_ragged_mode": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_hf_cut_ragged": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

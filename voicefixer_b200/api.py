@@ -58,6 +58,59 @@ def ragged_plan(wavs):
     return items, lens, L_cap
 
 
+_MODE2_MSG = ("Expected more than 1 value per channel when training, got input size "
+              "torch.Size([1, 384, 1, 1])")
+
+
+def segment_bounds(n):
+    """[(start, stop)] of the 30 s segments restore_inmem cuts a recording of n samples into (voicefixer/base.py:117-119):
+    full segments, then the rest; a recording of a whole number of segments has no empty tail."""
+    out = []
+    bp = SEG_LENGTH
+    while bp < n + SEG_LENGTH:
+        out.append((bp - SEG_LENGTH, min(bp, n)))
+        bp += SEG_LENGTH
+    return out
+
+
+def plan_many(lengths, mode, max_items):
+    """Segments the recordings of the given lengths exactly as restore_inmem does and packs all their segments into ragged
+    batches (VoiceFixer.restore_many).  Segments are ordered by length, longest first, and each batch takes the longest
+    segment left plus up to max_items(L_cap) - 1 of the next ones, L_cap being that first segment's length (the batch's
+    capacity).  Returns [(L_cap, [(recording, start, stop), ...]), ...].
+
+    Raises ValueError, naming the recording, before anything runs: for an empty list, a segment of 1024 samples or fewer
+    (after the mode-1 pre-filter's 512 * (L // 512) in mode 1: the front end reflect-pads 1024), or in mode 2 a segment of
+    64 frames or fewer (the reference's train-mode BatchNorm refuses its 1 x 1 UNet centre)."""
+    if mode not in (0, 1, 2):
+        raise ValueError("mode must be 0, 1 or 2")
+    if len(lengths) == 0:
+        raise ValueError("restore_many takes a non-empty list of 1-D arrays")
+    segs = []
+    for i, n in enumerate(lengths):
+        bounds = segment_bounds(int(n))
+        if not bounds:
+            raise ValueError(f"restore_many: recording {i} is empty")
+        for a, b in bounds:
+            L = b - a
+            Lnet = 512 * (L // 512) if mode == 1 else L
+            if mode == 2 and 1 + Lnet // 441 <= 64:
+                raise ValueError(f"restore_many: recording {i}, samples {a}..{b}: {_MODE2_MSG}")
+            if Lnet <= 1024:
+                what = f"{L} samples, {Lnet} after the mode-1 pre-filter" if mode == 1 else f"{L} samples"
+                raise ValueError(f"restore_many: recording {i} has a segment (samples {a}..{b}) of {what}; the front end "
+                                 "reflect-pads 1024, so every segment needs at least 1025")
+            segs.append((i, a, b))
+    segs.sort(key=lambda s: s[1] - s[2])             # longest first; stable, so equal lengths keep their order
+    batches, k = [], 0
+    while k < len(segs):
+        L_cap = segs[k][2] - segs[k][1]
+        n = max(1, int(max_items(L_cap)))
+        batches.append((L_cap, segs[k:k + n]))
+        k += n
+    return batches
+
+
 class _ModelShim:
     """Stands in for `VoiceFixer._model` (the reference nn.Module): callers poke
     `.parameters()`, `.to()`, `.eval()`, `.train()` and `.vocoder` (test/streamlit.py:40-42)."""
@@ -247,6 +300,63 @@ class VoiceFixer:
                     outs[i] = y[k]
         out = torch.cat(outs, -1)[None]
         return out.cpu().numpy()
+
+    @torch.no_grad()
+    def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None):
+        """Extension of the reference API: restores a list of 1-D recordings of any lengths, in any mode, and returns a
+        list of (1, L_i') arrays, element i what restore_inmem(wavs[i], cuda=True, mode=mode) returns -- bit-identical in
+        modes 0 and 1 and in mode 2 with drop_masks_fn=False; in mode 2 with dropout, the same distribution.
+
+        The recordings are cut into 30 s segments as restore_inmem cuts them, and all segments of all recordings run as
+        ragged batches ordered by length (plan_many), each batch sized to the device memory that is free.  Mode 1 runs the
+        ragged pre-filter and then a ragged restore per batch; mode 2 a ragged restore with train-mode statistics per item.
+        drop_masks_fn (mode 2): None = Bernoulli(0.5) keep-masks from torch's CPU generator, as restore_inmem draws them;
+        a callable (B, T_cap) -> uint8 (2, B, T_cap, 512) supplies them for each launch (item b of a batch reads
+        [:, b, :T_b]); False = no dropout.  Bad input raises ValueError before anything is launched.  The vocoder hook of
+        restore_inmem (your_vocoder_func) runs per segment on the host and is not offered here."""
+        _check_cuda(cuda)
+        items = []
+        for i, w in enumerate(wavs):
+            a = np.ascontiguousarray(w, dtype=np.float32)
+            if a.ndim != 1:
+                raise ValueError(f"restore_many: recording {i} has shape {a.shape}; the list takes 1-D arrays")
+            items.append(a)
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+
+        def max_items(L_cap):
+            extra = 0
+            if mode == 1:     # the pre-filter's workspace and its (B, L_cap) output live alongside the restore
+                extra = eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
+            return eng.max_batch(L_cap, extra_per_item=extra)
+
+        plan = plan_many([a.shape[0] for a in items], mode, max_items)
+        pieces = {}                                                      # (recording, start) -> restored segment
+        for L_cap, segs in plan:
+            B = len(segs)
+            x = torch.zeros((B, L_cap))
+            for k, (i, a, b) in enumerate(segs):
+                x[k, :b - a] = torch.from_numpy(items[i][a:b])
+            x = x.to(dev)
+            lens = torch.tensor([b - a for _, a, b in segs], dtype=torch.int32).to(dev)
+            if mode == 1:
+                x, _, lens = eng.hf_cut(x, lens=lens)
+                out_lens = [512 * ((b - a) // 512) for _, a, b in segs]
+            else:
+                out_lens = [b - a for _, a, b in segs]
+            masks = None
+            if mode == 2 and drop_masks_fn is not False:
+                T = 1 + L_cap // 441
+                # the reference's train-mode Dropout(0.5) draws from torch's global RNG; see restore_inmem
+                masks = drop_masks_fn(B, T) if drop_masks_fn else (torch.rand(2, B, T, 512) >= 0.5)
+                masks = torch.as_tensor(masks).to(torch.uint8)
+                if tuple(masks.shape) != (2, B, T, 512):
+                    raise ValueError(f"dropout masks must have shape (2, {B}, {T}, 512), got {tuple(masks.shape)}")
+            y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens).cpu().numpy()
+            for k, (i, a, _) in enumerate(segs):
+                pieces[(i, a)] = y[k, :out_lens[k]]
+        return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(it.shape[0])])[None]
+                for i, it in enumerate(items)]
 
     # ------------------------------------------------------------------ batch entry point (extension)
     def pinned_empty(self, shape):

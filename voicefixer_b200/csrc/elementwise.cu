@@ -55,13 +55,22 @@ __global__ void bn_act_scalar_kernel(const float* __restrict__ x, long long x_sB
 
 // ------------------------------------------------------------------ bn_stats (mode 2)
 // Biased batch statistics per item (reference batch is 1: SURVEY D5), F.batch_norm training=True.
+// Ragged batch (seq non-NULL): item b's positions are its first seq[b] * per_row; the blocks past them exit, and the
+// blocks inside see exactly the rows (and row partition) they would see on the item alone.
+__device__ __forceinline__ long long stat_positions(const int* seq, int per_row, int b, long long P) {
+  return seq ? min(P, (long long)seq[b] * per_row) : P;
+}
+
 __global__ void bn_stats_accum_kernel(const float* __restrict__ x, long long x_sB, long long ldx,
                                       long long P, int C, int bn_C, long long rows_per_block,
+                                      const int* __restrict__ seq, int per_row,
                                       double* __restrict__ acc /*[B][bn_C][2]*/) {
   const int b = blockIdx.z;
   const int c = blockIdx.y * 32 + threadIdx.x;
+  const long long Pb = stat_positions(seq, per_row, b, P);
   const long long p0 = (long long)blockIdx.x * rows_per_block;
-  const long long p1 = min(P, p0 + rows_per_block);
+  if (p0 >= Pb) return;                          // uniform over the block
+  const long long p1 = min(Pb, p0 + rows_per_block);
   double s = 0.0, s2 = 0.0;
   if (c < C) {
     const float* xp = x + b * x_sB + c;
@@ -89,12 +98,16 @@ __global__ void bn_stats_accum_kernel(const float* __restrict__ x, long long x_s
   }
 }
 
-__global__ void bn_stats_final_kernel(const double* __restrict__ acc, int B, int bn_C, double count,
+// count: values per statistic, positions x C for the single-channel (bn_C == 1) norms, positions otherwise
+__global__ void bn_stats_final_kernel(const double* __restrict__ acc, int B, int bn_C, long long P, int C,
+                                      const int* __restrict__ seq, int per_row,
                                       const float* __restrict__ gamma, const float* __restrict__ beta,
                                       float* __restrict__ scale, float* __restrict__ shift) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * bn_C) return;
   const int c = i % bn_C;
+  const long long Pb = stat_positions(seq, per_row, i / bn_C, P);
+  const double count = bn_C == 1 ? (double)Pb * C : (double)Pb;
   const double mean = acc[2 * i] / count;
   double var = acc[2 * i + 1] / count - mean * mean;
   if (var < 0) var = 0;
@@ -374,14 +387,14 @@ int bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, 
 
 int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, int C, int bn_C,
              const float* gamma, const float* beta, float* scale, float* shift, double* acc,
-             cudaStream_t st) {
+             const int* seq, int per_row, cudaStream_t st) {
   VFX_CUDA_CHECK(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * B * bn_C, st));
   const long long rows_per_block = 256;
   dim3 grid(ceil_div(P, rows_per_block), ceil_div(C, 32), B), block(32, 8);
-  bn_stats_accum_kernel<<<grid, block, 0, st>>>(x, x_sB, ldx, P, C, bn_C, rows_per_block, acc);
+  bn_stats_accum_kernel<<<grid, block, 0, st>>>(x, x_sB, ldx, P, C, bn_C, rows_per_block, seq, per_row, acc);
   VFX_LAUNCH_CHECK();
-  const double count = bn_C == 1 ? (double)P * C : (double)P;
-  bn_stats_final_kernel<<<ceil_div(B * bn_C, 128), 128, 0, st>>>(acc, B, bn_C, count, gamma, beta, scale, shift);
+  bn_stats_final_kernel<<<ceil_div(B * bn_C, 128), 128, 0, st>>>(acc, B, bn_C, P, C, seq, per_row, gamma, beta, scale,
+                                                                  shift);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

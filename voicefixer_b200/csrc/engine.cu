@@ -187,9 +187,10 @@ void taps3x3(vfx_conv_desc& d, long long mat) {
 struct BnRef { const float* scale; const float* shift; int stat_sB; };
 
 // Eval: the folded running-stat affine registered by the host ("<name>.scale/.shift").
-// Train (mode 2): per-item biased batch statistics of `x` (SURVEY D5/a19).
+// Train (mode 2): per-item biased batch statistics of `x` (SURVEY D5/a19).  seq / per_row: the items' extents at this
+// level (ragged batch; NULL = all P positions): item b's statistics cover its first seq[b] * per_row positions.
 int bn_resolve(Ctx& c, const std::string& name, int bn_C, const float* x, long long x_sB, long long ldx,
-               int B, long long P, int C, BnRef* out) {
+               int B, long long P, int C, const int* seq, int per_row, BnRef* out) {
   if (!c.train()) {
     out->scale = getf(c, name + ".scale", bn_C);
     out->shift = getf(c, name + ".shift", bn_C);
@@ -203,14 +204,14 @@ int bn_resolve(Ctx& c, const std::string& name, int bn_C, const float* x, long l
   double* acc = c.ws->alloc<double>((size_t)2 * B * bn_C);
   out->scale = sc; out->shift = sh; out->stat_sB = bn_C;
   if (c.dry || c.rc != VFX_OK) return c.rc;
-  return bn_stats(x, x_sB, ldx, B, P, C, bn_C, gamma, beta, sc, sh, acc, c.st);
+  return bn_stats(x, x_sB, ldx, B, P, C, bn_C, gamma, beta, sc, sh, acc, seq, per_row, c.st);
 }
 
 // operand = act(bn(x)); x raw fp32 [B][P][C] (pitch ldx) -> dense operand [B][P][C]
 int bn_act_op(Ctx& c, int prec, const std::string& bn, int bn_C, const float* x, long long x_sB,
-              long long ldx, int B, long long P, int C, int act, float slope, void* y) {
+              long long ldx, int B, long long P, int C, const int* seq, int per_row, int act, float slope, void* y) {
   BnRef r;
-  VFX_TRY(bn_resolve(c, bn, bn_C, x, x_sB, ldx, B, P, C, &r));
+  VFX_TRY(bn_resolve(c, bn, bn_C, x, x_sB, ldx, B, P, C, seq, per_row, &r));
   if (c.dry) return VFX_OK;
   ProfScope ps(c, "bn_act", 0.0, (double)B * P * C * (4 + prec_esz(prec)));
   return bn_act(prec, x, x_sB, ldx, B, P, C, r.scale, r.shift, bn_C, r.stat_sB, act, slope, y,
@@ -230,7 +231,8 @@ struct BlockScratch { void* opA; float* rawH; void* opH; float* rawS; void* opX;
 struct BlockFuse { bool opA_ready = false; const char* next_bn = nullptr; float next_slope = 0.01f; };
 
 // seq: the items' extents along H at this level (ragged batch; NULL = all H rows).  The eval BatchNorms (bn_act) are
-// pointwise, so rows beyond an item's extent only carry values that the convolutions never read.
+// pointwise, so rows beyond an item's extent only carry values that the convolutions never read; the train-mode
+// statistics cover each item's own rows (seq[b] * W positions).
 int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, int B, int H, int W,
                int Cin, int Cout, float* out, long long ld_out, const BlockScratch& s, const int* seq,
                const BlockFuse& fz = BlockFuse()) {
@@ -246,7 +248,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
   }
   if (!(fuse && fz.opA_ready)) {
     BnRef r;
-    VFX_TRY(bn_resolve(c, p + ".bn1", Cin, in, P * ld_in, ld_in, B, P, Cin, &r));
+    VFX_TRY(bn_resolve(c, p + ".bn1", Cin, in, P * ld_in, ld_in, B, P, Cin, seq, W, &r));
     if (!c.dry) {
       ProfScope ps(c, "bn_act", 0.0, (double)B * P * Cin * (4 + prec_esz(prec)));
       VFX_TRY(bn_act(prec, in, P * ld_in, ld_in, B, P, Cin, r.scale, r.shift, Cin, r.stat_sB, VFX_ACT_LRELU, 0.01f, s.opA,
@@ -269,7 +271,7 @@ int conv_block(Ctx& c, const std::string& p, const float* in, long long ld_in, i
     set_raw(d, s.rawH, Cout, 0);
     snprintf(tg, sizeof(tg), "unet.conv3x3.W%d.%dto%d", W, Cin, Cout);
     VFX_TRY(run_conv(c, prec, d, c.e->profile > 1 ? tg : "unet.conv3x3"));
-    VFX_TRY(bn_act_op(c, prec, p + ".bn2", Cout, s.rawH, P * Cout, Cout, B, P, Cout, VFX_ACT_LRELU, 0.01f, s.opH));
+    VFX_TRY(bn_act_op(c, prec, p + ".bn2", Cout, s.rawH, P * Cout, Cout, B, P, Cout, seq, W, VFX_ACT_LRELU, 0.01f, s.opH));
   }
   const float* res = in; long long ld_res = ld_in;
   if (Cin != Cout) {
@@ -364,7 +366,8 @@ int unet_forward(Ctx& c, const float* unet_in, int B, int Tp, float** feat_out) 
     const std::string p(name);
     const long long Pin = (long long)H * W;
     if (!fuse)   // eval: relu(bn1(x)) was written into s.opA by the producing conv2's epilogue
-      VFX_TRY(bn_act_op(c, prec, p + ".bn1", Cd, xd, Pin * Cd, Cd, B, Pin, Cd, VFX_ACT_LRELU, 0.0f, s.opA));
+      VFX_TRY(bn_act_op(c, prec, p + ".bn1", Cd, xd, Pin * Cd, Cd, B, Pin, Cd, c.ext_at(EXT_UNET0 + l), W, VFX_ACT_LRELU,
+                        0.0f, s.opA));
     const void* wt = getw(c, p + ".up.w", (size_t)9 * Cout * Cd, prec);
     for (int rh = 0; rh < 2; ++rh)
       for (int rw = 0; rw < 2; ++rw) {
@@ -435,7 +438,8 @@ int bn_gru(Ctx& c, const std::string& p, const float* x, int B, int T, void* op,
   const long long M = (long long)B * T;
   const int prec = c.prec();
   // BN2d(1) over the (T,512) plane of each item
-  VFX_TRY(bn_act_op(c, prec, p + ".bn", 1, x, (long long)T * 512, 512, B, T, 512, VFX_ACT_NONE, 0.f, op));
+  VFX_TRY(bn_act_op(c, prec, p + ".bn", 1, x, (long long)T * 512, 512, B, T, 512, c.ext_at(EXT_FRAMES), 1, VFX_ACT_NONE,
+                    0.f, op));
   const void* in = op;
   float* outs[2] = {y0, y1};
   for (int layer = 0; layer < 2; ++layer) {
@@ -464,8 +468,9 @@ int relu_inplace(Ctx& c, float* x, int B, int T, int C) {
                 (long long)T * C, C, c.st);
 }
 
-// Ragged batch: every op but the GRU recurrence is per frame (Linear GEMMs over B*T rows, eval BatchNorm and ReLU via
-// bn_act), so frames beyond an item's end only produce values that no later kernel reads.
+// Ragged batch: every op but the GRU recurrence and the train-mode statistics is per frame (Linear GEMMs over B*T rows,
+// BatchNorm and ReLU via bn_act, dropout), so frames beyond an item's end only produce values that no later kernel reads;
+// the GRU and the statistics take the items' frame counts (EXT_FRAMES).
 int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop, float* lin_out) {
   const long long M = (long long)B * T;
   const int prec = c.prec();
@@ -474,19 +479,20 @@ int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop
   float* y0 = c.ws->alloc<float>(M * 512);
   float* gi = c.ws->alloc<float>(M * 1536);
   const std::string p = "dn.";
-  VFX_TRY(bn_act_op(c, prec, p + "bn0", 1, mel, (long long)T * 128, 128, B, T, 128, VFX_ACT_NONE, 0.f, a));
+  const int* fr = c.ext_at(EXT_FRAMES);
+  VFX_TRY(bn_act_op(c, prec, p + "bn0", 1, mel, (long long)T * 128, 128, B, T, 128, fr, 1, VFX_ACT_NONE, 0.f, a));
   VFX_TRY(linear(c, a, M, 128, p + "lin1", 256, b, nullptr, 0));
   VFX_TRY(relu_inplace(c, b, B, T, 256));
-  VFX_TRY(bn_act_op(c, prec, p + "bn3", 1, b, (long long)T * 256, 256, B, T, 256, VFX_ACT_NONE, 0.f, a));
+  VFX_TRY(bn_act_op(c, prec, p + "bn3", 1, b, (long long)T * 256, 256, B, T, 256, fr, 1, VFX_ACT_NONE, 0.f, a));
   VFX_TRY(linear(c, a, M, 256, p + "lin4", 512, b, nullptr, 0));
   if (c.train() && drop && !c.dry) VFX_TRY(dropout_apply(b, drop, M * 512, c.st));
   VFX_TRY(relu_inplace(c, b, B, T, 512));
   VFX_TRY(bn_gru(c, p + "g7", b, B, T, a, gi, y0, b));       // result in b
   VFX_TRY(bn_gru(c, p + "g8", b, B, T, a, gi, y0, b));
-  VFX_TRY(bn_act_op(c, prec, p + "bn9", 1, b, (long long)T * 512, 512, B, T, 512, VFX_ACT_LRELU, 0.f, a));
+  VFX_TRY(bn_act_op(c, prec, p + "bn9", 1, b, (long long)T * 512, 512, B, T, 512, fr, 1, VFX_ACT_LRELU, 0.f, a));
   VFX_TRY(linear(c, a, M, 512, p + "lin11", 512, b, nullptr, 0));
   if (c.train() && drop && !c.dry) VFX_TRY(dropout_apply(b, drop + M * 512, M * 512, c.st));
-  VFX_TRY(bn_act_op(c, prec, p + "bn13", 1, b, (long long)T * 512, 512, B, T, 512, VFX_ACT_LRELU, 0.f, a));
+  VFX_TRY(bn_act_op(c, prec, p + "bn13", 1, b, (long long)T * 512, 512, B, T, 512, fr, 1, VFX_ACT_LRELU, 0.f, a));
   VFX_TRY(linear(c, a, M, 512, p + "lin15", 128, lin_out, nullptr, 0));
   return c.rc;
 }
@@ -494,7 +500,8 @@ int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop
 int analysis_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop, float* mel_log_out) {
   const int Tp = (T + 63) / 64 * 64;
   // mode 2: the reference's train-mode BatchNorm raises "Expected more than 1 value per channel when training"
-  // when the UNet centre is 1x1, i.e. for segments of at most 64 frames
+  // when the UNet centre is 1x1, i.e. for segments of at most 64 frames (checked on the capacity; a ragged item that
+  // breaks it gets finite, unspecified samples: its 1 x 1 centre statistics have zero variance)
   if (c.train() && !c.dry) VFX_REQUIRE(Tp > 64, "mode 2 needs more than 64 frames per segment (got T=%d): Expected more than 1 value per channel when training", T);
   const size_t m0 = c.ws->mark();
   float* xlog = c.ws->alloc<float>((size_t)B * T * 128);
@@ -721,7 +728,7 @@ int frontend_forward(Ctx& c, const float* wav, int B, int L, float* mel, float* 
                   sp, c.st);
 }
 
-// lens (ragged batch, mode 0): per-item lengths on the device; L is then the capacity (row stride of wav / wav_out)
+// lens (ragged batch): per-item lengths on the device; L is then the capacity (row stride of wav / wav_out)
 int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop, const int* lens, float* wav_out) {
   const int T = 1 + L / 441;
   if (lens) {
@@ -1017,17 +1024,32 @@ int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const u
   return restore_entry(e, wav, B, L, mode, drop_masks, nullptr, wav_out, workspace, workspace_bytes, stream);
 }
 
+int vfx_restore_ragged_mode(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, int mode,
+                            const uint8_t* drop_masks, float* wav_out, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  VFX_REQUIRE(lens, "restore_ragged: lens is null");
+  return restore_entry(e, wav, B, L_cap, mode, drop_masks, lens, wav_out, workspace, workspace_bytes, stream);
+}
+
 int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* wav_out,
                        void* workspace, size_t workspace_bytes, void* stream) {
-  VFX_REQUIRE(lens, "restore_ragged: lens is null");
-  return restore_entry(e, wav, B, L_cap, VFX_MODE_EVAL, nullptr, lens, wav_out, workspace, workspace_bytes, stream);
+  return vfx_restore_ragged_mode(e, wav, B, L_cap, lens, VFX_MODE_EVAL, nullptr, wav_out, workspace, workspace_bytes,
+                                 stream);
 }
 
 int vfx_hf_cut(vfx_engine* e, const float* wav, int B, int L, float ratio, float* wav_out, int* cut_bins,
                void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
-  return hf_cut(wav, B, L, ratio, e->d_window, e->d_tw, wav_out, cut_bins, workspace, workspace_bytes,
+  return hf_cut(wav, B, L, nullptr, ratio, e->d_window, e->d_tw, wav_out, nullptr, cut_bins, workspace, workspace_bytes,
                 (cudaStream_t)stream);
+}
+
+int vfx_hf_cut_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float ratio, float* wav_out,
+                      int* lens_out, int* cut_bins, void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_REQUIRE(lens, "hf_cut_ragged: lens is null");
+  return hf_cut(wav, B, L_cap, lens, ratio, e->d_window, e->d_tw, wav_out, lens_out, cut_bins, workspace,
+                workspace_bytes, (cudaStream_t)stream);
 }
 
 int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream) {

@@ -15,12 +15,20 @@ namespace {
 
 constexpr int NF = 2048, HOP = 512, NB = 1025;
 
+// Per-item lengths (ragged batch, `lens` non-NULL): item b is L_b = clamp(lens[b], HOP, L) samples long in a row of L
+// (= L_cap) samples and is processed as if it were alone: nfr_b = 1 + L_b / HOP frames, samples at or after L_b read as
+// zero (librosa's constant padding at the item's own end), istft length out_len_b = HOP * (nfr_b - 1).
+__device__ __forceinline__ int item_len(const int* lens, int b, int L) { return lens ? min(max(lens[b], HOP), L) : L; }
+
 __global__ void __launch_bounds__(256) hf_fwd_kernel(const float* __restrict__ wav, int L, int nfr,
+                                                     const int* __restrict__ lens,
                                                      const float* __restrict__ window,
                                                      const float2* __restrict__ tw, float2* __restrict__ S,
                                                      double* __restrict__ energy) {
   __shared__ float2 bufA[1024], bufB[1024];
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int Lb = item_len(lens, b, L);
+  if (t >= 1 + Lb / HOP) return;                 // past the item's last frame: no spectrum, no energy
   const float* x = wav + (long long)b * L;
   const int base = t * HOP - NF / 2;
   for (int n = tid; n < 1024; n += 256) {
@@ -28,7 +36,7 @@ __global__ void __launch_bounds__(256) hf_fwd_kernel(const float* __restrict__ w
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int i = base + 2 * n + h;
-      v[h] = (i >= 0 && i < L) ? x[i] * window[2 * n + h] : 0.f;
+      v[h] = (i >= 0 && i < Lb) ? x[i] * window[2 * n + h] : 0.f;
     }
     bufA[n] = make_float2(v[0], v[1]);
   }
@@ -43,9 +51,11 @@ __global__ void __launch_bounds__(256) hf_fwd_kernel(const float* __restrict__ w
   }
 }
 
-__global__ void hf_cut_index_kernel(const double* __restrict__ energy, float ratio, int* __restrict__ cut) {
+__global__ void hf_cut_index_kernel(const double* __restrict__ energy, float ratio, int* __restrict__ cut,
+                                    const int* __restrict__ lens, int L, int* __restrict__ lens_out) {
   const int b = blockIdx.x;
   if (threadIdx.x != 0) return;
+  if (lens_out) lens_out[b] = HOP * (item_len(lens, b, L) / HOP);      // the item's filtered length out_len_b
   const double* e = energy + (long long)b * NB;
   double total = 0.0;
   for (int k = 0; k < NB; ++k) total += e[k];
@@ -57,13 +67,15 @@ __global__ void hf_cut_index_kernel(const double* __restrict__ energy, float rat
   cut[b] = i;
 }
 
-__global__ void __launch_bounds__(256) hf_inv_kernel(const float2* __restrict__ S, int nfr,
+__global__ void __launch_bounds__(256) hf_inv_kernel(const float2* __restrict__ S, int nfr, int L,
+                                                     const int* __restrict__ lens,
                                                      const int* __restrict__ cut,
                                                      const float* __restrict__ window,
                                                      const float2* __restrict__ tw, float* __restrict__ frames) {
   __shared__ float2 X[NB];
   __shared__ float2 bufA[1024], bufB[1024];
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  if (t >= 1 + item_len(lens, b, L) / HOP) return;
   const float2* Sp = S + ((long long)b * nfr + t) * NB;
   const int ci = cut[b];
   for (int k = tid; k <= 1024; k += 256) {
@@ -100,13 +112,17 @@ __global__ void __launch_bounds__(256) hf_inv_kernel(const float2* __restrict__ 
   }
 }
 
-__global__ void hf_ola_kernel(const float* __restrict__ frames, int nfr, int out_len,
-                              const float* __restrict__ window, float* __restrict__ out) {
+// out_len: row stride of `out` (HOP * (nfr - 1); L_cap on a ragged batch, whose item b fills out_len_b samples of its
+// row from its own frames and zeros the rest)
+__global__ void hf_ola_kernel(const float* __restrict__ frames, int nfr, int out_len, int L,
+                              const int* __restrict__ lens, const float* __restrict__ window, float* __restrict__ out) {
   const int b = blockIdx.y;
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= out_len) return;
+  const int nfr_b = lens ? 1 + item_len(lens, b, L) / HOP : nfr;
+  if (n >= HOP * (nfr_b - 1)) { out[(long long)b * out_len + n] = 0.f; return; }
   const int p = n + NF / 2;                      // position in the un-trimmed overlap-add buffer
-  const int t_hi = min(p / HOP, nfr - 1);
+  const int t_hi = min(p / HOP, nfr_b - 1);
   const int t_lo = max(0, (p - NF) / HOP + 1);
   float acc = 0.f, wss = 0.f;
   for (int t = t_lo; t <= t_hi; ++t) {
@@ -128,11 +144,11 @@ size_t hf_cut_workspace(int B, int L) {
          (size_t)B * 4 + 4096;
 }
 
-int hf_cut(const float* wav, int B, int L, float ratio, const float* window, const float2* tw, float* out,
-           int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st) {
+int hf_cut(const float* wav, int B, int L, const int* lens, float ratio, const float* window, const float2* tw, float* out,
+           int* lens_out, int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st) {
   VFX_REQUIRE(wav && out && ws && B > 0 && L >= HOP, "hf_cut: bad arguments (L=%d)", L);
   const int nfr = 1 + L / HOP;
-  const int out_len = HOP * (nfr - 1);
+  const int out_len = lens ? L : HOP * (nfr - 1);
   if (ws_bytes < hf_cut_workspace(B, L)) {
     set_error("hf_cut: workspace too small: need %zu bytes", hf_cut_workspace(B, L));
     return VFX_ERR_WORKSPACE;
@@ -143,13 +159,13 @@ int hf_cut(const float* wav, int B, int L, float ratio, const float* window, con
   float* frames = reinterpret_cast<float*>(p); p += (((size_t)B * nfr * NF * sizeof(float)) + 255) & ~(size_t)255;
   int* cut = cut_bins ? cut_bins : reinterpret_cast<int*>(p);
   VFX_CUDA_CHECK(cudaMemsetAsync(energy, 0, (size_t)B * NB * sizeof(double), st));
-  hf_fwd_kernel<<<dim3(nfr, B), 256, 0, st>>>(wav, L, nfr, window, tw, S, energy);
+  hf_fwd_kernel<<<dim3(nfr, B), 256, 0, st>>>(wav, L, nfr, lens, window, tw, S, energy);
   VFX_LAUNCH_CHECK();
-  hf_cut_index_kernel<<<B, 32, 0, st>>>(energy, ratio, cut);
+  hf_cut_index_kernel<<<B, 32, 0, st>>>(energy, ratio, cut, lens, L, lens ? lens_out : nullptr);
   VFX_LAUNCH_CHECK();
-  hf_inv_kernel<<<dim3(nfr, B), 256, 0, st>>>(S, nfr, cut, window, tw, frames);
+  hf_inv_kernel<<<dim3(nfr, B), 256, 0, st>>>(S, nfr, L, lens, cut, window, tw, frames);
   VFX_LAUNCH_CHECK();
-  hf_ola_kernel<<<dim3(ceil_div(out_len, 256), B), 256, 0, st>>>(frames, nfr, out_len, window, out);
+  hf_ola_kernel<<<dim3(ceil_div(out_len, 256), B), 256, 0, st>>>(frames, nfr, out_len, L, lens, window, out);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

@@ -104,10 +104,11 @@ int bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, 
            const float* scale, const float* shift, int bn_C, int stat_sB, int act, float act_param,
            void* y, long long y_sB, long long ldy, cudaStream_t st);
 // per-item biased batch statistics -> scale/shift [B][C] (train-mode BN, eps 1e-5)
-// acc: scratch of 2*B*bn_C doubles.
+// acc: scratch of 2*B*bn_C doubles.  seq (ragged batch, NULL = all P positions): item b's statistics cover its first
+// min(seq[b] * per_row, P) positions only (per_row = W of a [B][H][W][C] map, 1 for a [B][T][C] plane).
 int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, int C, int bn_C,
              const float* gamma, const float* beta, float* scale, float* shift, double* acc,
-             cudaStream_t st);
+             const int* seq, int per_row, cudaStream_t st);
 int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st);
 int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W,
                int C, float* y, cudaStream_t st);
@@ -149,8 +150,11 @@ int reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precisi
 // (lo_b = (S_b - L_b) / 2) and writes zeros from L_b to out_len
 int voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len,
              const int* ext_gen, const int* ext_len, float scale, float* out, cudaStream_t st);
-int hf_cut(const float* wav, int B, int L, float ratio, const float* window, const float2* tw,
-           float* out, int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st);
+// lens (ragged batch, NULL = every item has L samples): L is the capacity and the row stride of wav and out; item b is
+// filtered as if alone with clamp(lens[b], 512, L) samples, out holds its 512 * (L_b / 512) samples and zeros after, and
+// lens_out[b] (optional) receives that length
+int hf_cut(const float* wav, int B, int L, const int* lens, float ratio, const float* window, const float2* tw,
+           float* out, int* lens_out, int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t hf_cut_workspace(int B, int L);
 
 }  // namespace vfx

@@ -154,12 +154,13 @@ class Engine:
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{self.device}")
         return self._ws
 
-    def max_batch(self, L, cap=64, reserve=2 << 30):
+    def max_batch(self, L, cap=64, reserve=2 << 30, extra_per_item=0):
         """Largest number of equal-length items (<= cap) whose restore() workspace fits the memory that is free right now
-        (plus the workspace this engine already holds), keeping `reserve` bytes back.  At least 1."""
+        (plus the workspace this engine already holds), keeping `reserve` bytes back.  At least 1.  extra_per_item: other
+        device bytes each item needs alongside (e.g. the mode-1 pre-filter's workspace and output)."""
         free, _ = torch.cuda.mem_get_info(self.device)
         avail = free + (self._ws.numel() if self._ws is not None else 0) - reserve
-        per_item = max(1, self.workspace_bytes(2, L) - self.workspace_bytes(1, L))
+        per_item = max(1, self.workspace_bytes(2, L) - self.workspace_bytes(1, L) + int(extra_per_item))
         return int(max(1, min(cap, avail // per_item)))
 
     def workspace_bytes(self, B, L):
@@ -223,26 +224,27 @@ class Engine:
     def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None, lens=None):
         """wav (B, L) on device -> restored wav (B, L) on device (one launch sequence).
 
-        lens (ragged batch, mode 0): int32 device tensor (B,) of per-item lengths <= L.  Row b of `wav` then holds
-        item b in its first lens[b] samples; row b of the result is bit-identical to restoring that item alone, followed
-        by zeros.  Lengths are read on the device (vfx_restore_ragged), so a captured graph serves any lengths."""
+        lens (ragged batch): int32 device tensor (B,) of per-item lengths <= L.  Row b of `wav` then holds item b in its
+        first lens[b] samples; row b of the result is bit-identical to restoring that item alone, followed by zeros.
+        Lengths are read on the device (vfx_restore_ragged_mode), so a captured graph serves any lengths.  In mode 2,
+        drop_masks is (2, B, T_cap, 512) with T_cap = 1 + L // 441 (item b reads [:, b, :T_b]) and every item needs more
+        than 64 frames (1 + lens[b] // 441 > 64; an item below that gets finite, unspecified samples)."""
         wav = self._dev(wav)
         B, L = wav.shape
         if out is None:
             out = torch.empty_like(wav)
         if ws is None:
             ws = self._workspace(self.workspace_bytes(B, L))
-        if lens is not None:
-            if mode != 0 or drop_masks is not None:
-                raise ValueError("a ragged batch (lens) runs mode 0 only")
-            if not (lens.is_cuda and lens.dtype == torch.int32 and tuple(lens.shape) == (B,) and lens.is_contiguous()):
-                raise ValueError(f"lens must be a contiguous int32 CUDA tensor of shape ({B},)")
-            _lib.check(self.lib.vfx_restore_ragged(self.h, _ptr(wav), B, L, _ptr(lens), _ptr(out), _ptr(ws), ws.numel(),
-                                                   _stream()), "vfx_restore_ragged")
-            return out
         dm = None
         if drop_masks is not None:
             dm = drop_masks.to(device=wav.device, dtype=torch.uint8).contiguous()
+        if lens is not None:
+            _check_lens(lens, B)
+            if dm is not None and tuple(dm.shape) != (2, B, 1 + L // 441, 512):
+                raise ValueError(f"drop_masks must have shape (2, {B}, {1 + L // 441}, 512), got {tuple(dm.shape)}")
+            _lib.check(self.lib.vfx_restore_ragged_mode(self.h, _ptr(wav), B, L, _ptr(lens), int(mode), _ptr(dm), _ptr(out),
+                                                        _ptr(ws), ws.numel(), _stream()), "vfx_restore_ragged_mode")
+            return out
         _lib.check(self.lib.vfx_restore(self.h, _ptr(wav), B, L, int(mode), _ptr(dm), _ptr(out), _ptr(ws), ws.numel(),
                                         _stream()), "vfx_restore")
         return out
@@ -269,13 +271,35 @@ class Engine:
         g._keep = (ws, wav, out, lens, self.arena)
         return g
 
-    def hf_cut(self, wav, ratio=0.95):
+    @staticmethod
+    def hf_cut_workspace_bytes(B, L):
+        nfr = 1 + L // 512
+        return B * nfr * (1025 * 8 + 2048 * 4) + B * 1025 * 8 + (1 << 16)
+
+    def hf_cut(self, wav, ratio=0.95, lens=None):
+        """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
+
+        lens (ragged batch): int32 device tensor (B,); item b is the first lens[b] samples of row b and is filtered as if
+        alone.  Returns (out (B, L), cut bins, lens_out): row b holds 512 * (lens[b] // 512) samples, then zeros, and
+        lens_out (int32 device tensor) holds those lengths, ready for restore(..., lens=lens_out)."""
         wav = self._dev(wav)
         B, L = wav.shape
-        out = torch.empty(B, 512 * (L // 512), device=wav.device)
         cut = torch.empty(B, dtype=torch.int32, device=wav.device)
-        nfr = 1 + L // 512
-        ws = self._workspace(B * nfr * (1025 * 8 + 2048 * 4) + B * 1025 * 8 + (1 << 16))
+        ws = self._workspace(self.hf_cut_workspace_bytes(B, L))
+        if lens is not None:
+            _check_lens(lens, B)
+            out = torch.empty(B, L, device=wav.device)
+            lens_out = torch.empty(B, dtype=torch.int32, device=wav.device)
+            _lib.check(self.lib.vfx_hf_cut_ragged(self.h, _ptr(wav), B, L, _ptr(lens), float(ratio), _ptr(out),
+                                                  _ptr(lens_out), _ptr(cut), _ptr(ws), ws.numel(), _stream()),
+                       "vfx_hf_cut_ragged")
+            return out, cut, lens_out
+        out = torch.empty(B, 512 * (L // 512), device=wav.device)
         _lib.check(self.lib.vfx_hf_cut(self.h, _ptr(wav), B, L, float(ratio), _ptr(out), _ptr(cut), _ptr(ws), ws.numel(),
                                        _stream()), "vfx_hf_cut")
         return out, cut
+
+
+def _check_lens(lens, B):
+    if not (lens.is_cuda and lens.dtype == torch.int32 and tuple(lens.shape) == (B,) and lens.is_contiguous()):
+        raise ValueError(f"lens must be a contiguous int32 CUDA tensor of shape ({B},)")
