@@ -119,6 +119,35 @@ int vfx_vocoder(vfx_engine* e, const float* mel, int B, int T, int input_is_log,
 int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav_out, int trim_len,
                      float scale, void* workspace, size_t workspace_bytes, void* stream);
 
+/* vfx_vocoder (trim_len = -1) for B mels of DIFFERENT lengths, Vocoder.forward (voicefixer/vocoder/base.py:42-56) item by
+ * item: mel[B][T_cap][128] holds item b in its first frames[b] rows (device int32, clamped into [1, T_cap]; the other rows
+ * are never read).  wav_out[B][Tc_cap*441], Tc_cap = T_cap + T_cap%2 + 4: row b is bit-identical to vfx_vocoder on item b
+ * alone, its (T_b + T_b%2 + 4)*441 samples untrimmed, followed by zeros.  A small kernel turns frames into per-item extents
+ * that the kernels read on the device, so one captured graph of shape (B, T_cap) serves any lengths.
+ * Workspace: vfx_workspace_bytes_frames(e, B, T_cap). */
+int vfx_vocoder_ragged(vfx_engine* e, const float* mel, int B, int T_cap, const int* frames, int input_is_log,
+                       float* wav_out, float scale, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Front end of Vocoder.oracle (voicefixer/vocoder/base.py:61-73; the counterpart of vfx_frontend_mel) on the device:
+ * wav[B][L_cap] holds item b in its first lens[b] samples (device int32, clamped into [1, L_cap]; lens NULL = every item
+ * is L_cap long).  Per item: peak-normalise (wav / max|wav|, IEEE division), |STFT| (n_fft 2048, hop 441, periodic Hann,
+ * center with librosa 0.10's zero padding, no clamp), the Slaney-normalised HTK mel basis, 20 log10(max(1e-5, mel)) - 20,
+ * normalise and clip to [-4, 4], and pre()'s -4 tail.  cond_out: fp32 [B][Tc_cap][128], Tc_cap = T_cap + T_cap%2 + 4,
+ * T_cap = 1 + L_cap/441; item b fills rows < Tc_b (rows T_b .. Tc_b - 1 are -4, T_b = 1 + L_b/441) and zeros after.
+ * An all-zero item divides by a zero peak, as the reference does.  Workspace: 4*B bytes (the per-item peaks). */
+int vfx_oracle_cond(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* cond_out, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
+/* Vocoder.oracle (voicefixer/vocoder/base.py:58-77) up to the file write: the front end of vfx_oracle_cond into the
+ * workspace in the operand format, then the Generator on the frame-based extents.  wav_out[B][Tc_cap*441]: row b holds
+ * item b's (T_b + T_b%2 + 4)*441 samples times scale (oracle(): 2^15), then zeros; bit-identical to the same call on
+ * item b alone (B = 1, L_cap = L_b). */
+int vfx_oracle(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float scale, float* wav_out,
+               void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace of vfx_oracle for (B, L_cap): the vfx_oracle pass run dry (works on a planning-only
+ * engine); 0 for B <= 0 or L_cap <= 0. */
+size_t vfx_oracle_workspace_bytes(const vfx_engine* e, int B, int L_cap);
+
 /* Whole restore_inmem loop body (voicefixer/base.py:120-135) for B equal-length segments (vfx_restore_ragged below for
  * segments of different lengths):
  * wav[B][L] -> wav_out[B][L].  Equivalent to frontend -> analysis -> vocoder(trim_len = L). */

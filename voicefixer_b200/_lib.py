@@ -69,6 +69,10 @@ SIGNATURES = {
     "vfx_restore_ragged": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_restore_ragged_mode": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_hf_cut_ragged": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_vocoder_ragged": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _f, _vp, _sz, _vp]),
+    "vfx_oracle_cond": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_oracle": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _sz, _vp]),
+    "vfx_oracle_workspace_bytes": (_sz, [_vp, _i, _i]),
 }
 
 _lib = None

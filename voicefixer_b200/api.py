@@ -111,6 +111,46 @@ def plan_many(lengths, mode, max_items):
     return batches
 
 
+def plan_vocoder_many(items, kind, max_items):
+    """Packs the items of Vocoder.forward_many (kind "mel": [1, 1, T, 128] mels) or Vocoder.oracle_many (kind "wav": 1-D
+    float32 recordings) into ragged batches.  Items are ordered by length, longest first (stable, so equal lengths keep
+    their order), and each batch takes the longest item left plus up to max_items(cap) - 1 of the next ones, cap being
+    that first item's length in frames (mels) or samples (recordings): the batch's capacity.  Returns
+    [(cap, [item, ...]), ...].
+
+    Raises before anything is sized or launched, naming the item: ValueError for an empty list, a mel that is not
+    [1, 1, T >= 1, 128], or a recording that is empty, not 1-D or all zeros (the reference divides by its zero peak);
+    AssertionError for a mel whose last dimension is not 128, as Vocoder.forward asserts."""
+    what = {"mel": "forward_many", "wav": "oracle_many"}[kind]
+    if len(items) == 0:
+        raise ValueError(f"{what} takes a non-empty list")
+    lengths = []
+    for i, x in enumerate(items):
+        shape = tuple(x.shape)
+        if kind == "mel":
+            if len(shape) >= 1 and shape[-1] != 128:
+                raise AssertionError(f"{what}: item {i} has shape {shape}; the mel must have 128 bins")
+            if len(shape) != 4 or shape[:2] != (1, 1) or shape[2] < 1:
+                raise ValueError(f"{what}: item {i} has shape {shape}; each mel must be [1, 1, T >= 1, 128]")
+            lengths.append(shape[2])
+        else:
+            if len(shape) != 1:
+                raise ValueError(f"{what}: item {i} has shape {shape}; each recording must be 1-D")
+            if shape[0] == 0:
+                raise ValueError(f"{what}: item {i} is empty")
+            if not np.any(x):
+                raise ValueError(f"{what}: item {i} is all zeros; its peak normalisation would divide by zero")
+            lengths.append(shape[0])
+    order = sorted(range(len(items)), key=lambda i: -lengths[i])
+    batches, k = [], 0
+    while k < len(order):
+        cap = lengths[order[k]]
+        n = max(1, int(max_items(cap)))
+        batches.append((cap, order[k:k + n]))
+        k += n
+    return batches
+
+
 class _ModelShim:
     """Stands in for `VoiceFixer._model` (the reference nn.Module): callers poke
     `.parameters()`, `.to()`, `.eval()`, `.train()` and `.vocoder` (test/streamlit.py:40-42)."""
@@ -157,6 +197,33 @@ class Vocoder:
 
     __call__ = forward
 
+    @torch.no_grad()
+    def forward_many(self, mels, cuda=False):
+        """Extension of the reference API: forward() on a list of [1, 1, T_i, 128] mels (tensors or arrays) of any lengths.
+        Element i is bit-identical to forward(mels[i], cuda), on the device or the CPU as forward places it.  The mels run
+        as ragged batches ordered by length (plan_vocoder_many, vfx_vocoder_ragged), each sized to the device memory that
+        is free (Engine.max_batch_frames).  Bad input raises before anything is launched."""
+        _check_cuda(cuda)
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+
+        def max_items(T):
+            S = (T + T % 2 + 4) * 441
+            return eng.max_batch_frames(T, extra_per_item=4 * (T * 128 + S))          # + the batch's input and output
+
+        outs = [None] * len(mels)
+        for T_cap, idx in plan_vocoder_many(mels, "mel", max_items):
+            x = torch.zeros((len(idx), T_cap, 128), device=dev)
+            for k, i in enumerate(idx):
+                x[k, :mels[i].shape[2]] = torch.as_tensor(mels[i])[0, 0].to(device=dev, dtype=torch.float32)
+            lens = torch.tensor([mels[i].shape[2] for i in idx], dtype=torch.int32).to(dev)
+            y = eng.vocoder(x, lens=lens)
+            for k, i in enumerate(idx):
+                T = mels[i].shape[2]
+                o = y[k:k + 1, None, :(T + T % 2 + 4) * 441]
+                outs[i] = o.clone() if cuda else o.cpu()
+        return outs
+
     def oracle(self, fpath, out_path, cuda=False):
         """vocoder/base.py:58-77: wav file -> |STFT| -> Slaney mel -> normalise -> Generator -> file."""
         _check_cuda(cuda)
@@ -164,6 +231,35 @@ class Vocoder:
         cond = oracle_conditions(wav)
         out = self._engine.vocoder_cond(torch.from_numpy(cond), scale=2.0 ** 15)
         wavio.save_wave(out[:, None, :].cpu().numpy(), out_path, sample_rate=self.rate)
+
+    @torch.no_grad()
+    def oracle_many(self, wavs, cuda=True):
+        """Extension of the reference API: oracle()'s computation on a list of 1-D float32 recordings of any lengths, each
+        one whole sequence (no 30 s segments), front end included on the device (vfx_oracle).  Element i is a
+        (1, (T_i + T_i % 2 + 4) * 441) float32 array, T_i = 1 + L_i // 441: the Generator output before oracle()'s x 2^15
+        and int16 file write.  The recordings run as ragged batches ordered by length (plan_vocoder_many), each sized to
+        the device memory that is free.  Bad input raises before anything is launched."""
+        _check_cuda(cuda)
+        items = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+
+        def max_items(L):
+            T = 1 + L // 441
+            per_item = eng.oracle_workspace_bytes(2, L) - eng.oracle_workspace_bytes(1, L) + 4 * (L + (T + T % 2 + 4) * 441)
+            return eng._fit(per_item, 64, 2 << 30)
+
+        outs = [None] * len(items)
+        for L_cap, idx in plan_vocoder_many(items, "wav", max_items):
+            x = torch.zeros((len(idx), L_cap))
+            for k, i in enumerate(idx):
+                x[k, :items[i].shape[0]] = torch.from_numpy(items[i])
+            lens = torch.tensor([items[i].shape[0] for i in idx], dtype=torch.int32).to(dev)
+            y = eng.oracle(x.to(dev), lens=lens).cpu().numpy()
+            for k, i in enumerate(idx):
+                T = 1 + items[i].shape[0] // 441
+                outs[i] = y[k:k + 1, :(T + T % 2 + 4) * 441].copy()
+        return outs
 
 
 def oracle_conditions(wav):

@@ -353,6 +353,26 @@ __global__ void ragged_extents_kernel(const int* __restrict__ lens, int B, int L
   ext[(EXT_UP0 + 3) * B + b] = Tc * 441;
 }
 
+// The same table for the vocoder alone, from per-item mel frame counts (frames clamped into [1, T_cap]).  The samples
+// row is the generated length S_b, so voc_post's centred trim is lo = 0 and item b's output is untrimmed, as
+// Vocoder.forward returns it.  The UNet rows are unused by the vocoder; they hold the values restore() would use.
+__global__ void frame_extents_kernel(const int* __restrict__ frames, int B, int T_cap, int* __restrict__ ext) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int T = min(max(frames[b], 1), T_cap);
+  const int Tp = (T + 63) / 64 * 64;
+  const int Tc = T + T % 2 + 4;
+  ext[EXT_SAMPLES * B + b] = Tc * 441;
+  ext[EXT_FRAMES * B + b] = T;
+  for (int k = 0; k < 7; ++k) ext[(EXT_UNET0 + k) * B + b] = Tp >> k;
+  ext[EXT_COND * B + b] = Tc;
+  ext[EXT_COND_PAD * B + b] = Tc + 6;
+  ext[(EXT_UP0 + 0) * B + b] = Tc * 7;
+  ext[(EXT_UP0 + 1) * B + b] = Tc * 49;
+  ext[(EXT_UP0 + 2) * B + b] = Tc * 147;
+  ext[(EXT_UP0 + 3) * B + b] = Tc * 441;
+}
+
 inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
   if (g > 132LL * 32) g = 132LL * 32;      // 32 blocks per SM of an H100 SXM
@@ -448,6 +468,13 @@ int voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames,
 int ragged_extents(const int* lens, int B, int L_cap, int* ext, cudaStream_t st) {
   VFX_REQUIRE(lens && ext && B > 0 && L_cap > 1024, "ragged_extents: bad arguments");
   ragged_extents_kernel<<<ceil_div(B, 128), 128, 0, st>>>(lens, B, L_cap, ext);
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+int frame_extents(const int* frames, int B, int T_cap, int* ext, cudaStream_t st) {
+  VFX_REQUIRE(frames && ext && B > 0 && T_cap > 0, "frame_extents: bad arguments");
+  frame_extents_kernel<<<ceil_div(B, 128), 128, 0, st>>>(frames, B, T_cap, ext);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

@@ -1,7 +1,7 @@
 // vfx_b200 engine: weight registry, workspace planning and the launch sequence of the restore()
 // hot path behind the C ABI of include/vfx_b200.h.  One engine per process/GPU; all device memory
-// (weights, workspace, inputs, outputs) is owned by the caller; only two small constant tables
-// (Hann window, FFT twiddles) are allocated here at create time.
+// (weights, workspace, inputs, outputs) is owned by the caller; only small constant tables (Hann window, FFT twiddles,
+// the oracle's Slaney mel basis) are allocated here at create time.
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -41,6 +41,8 @@ struct vfx_engine {
   std::unordered_map<std::string, vfx::Tensor> tensors;
   float* d_window = nullptr;    // periodic Hann, 2048
   float2* d_tw = nullptr;       // exp(-2 pi i k / 2048), k < 1024
+  float* d_obasis = nullptr;    // Vocoder.oracle's Slaney HTK mel basis [128][1025] (a constant, not a checkpoint weight)
+  int* d_oband = nullptr;       // its band of non-zero bins per row: start[128] ++ len[128]
   std::vector<std::string> missing;
   int parts = 0;    // VFX_PART_* bits of the weight sets found complete by vfx_engine_finalize
   int tf32_stream = 1;  // TF32: vocoder residual streams are kept as ONE encoded fp32 tensor (operand + residual carrier)
@@ -728,6 +730,72 @@ int frontend_forward(Ctx& c, const float* wav, int B, int L, float* mel, float* 
                   sp, c.st);
 }
 
+// Vocoder.forward on a ragged batch of mels: item b is the first frames[b] rows of mel[B][T_cap][128]; the frame-based
+// extent table gives every vocoder kernel the item's own lengths, and voc_post writes its S_b samples untrimmed, then zeros.
+int vocoder_ragged_forward(Ctx& c, const float* mel, int B, int T_cap, const int* frames, int input_is_log,
+                           float* wav_out, float scale) {
+  int* ext = c.ws->alloc<int>((size_t)EXT_LEVELS * B);
+  if (!c.dry) VFX_TRY(frame_extents(frames, B, T_cap, ext, c.st));
+  c.ext = ext; c.ext_B = B;
+  return vocoder_forward(c, mel, B, T_cap, input_is_log, wav_out, -1, scale);
+}
+
+// Vocoder.oracle (vocoder/base.py:58-77 up to the file write) on wav[B][L_cap]: the device front end writes the
+// conditions in the operand format straight into the workspace, and the generator consumes them.  lens (ragged batch,
+// NULL = L_cap each): the front end also writes each item's frame count, from which the frame-based extent table is built.
+// The table is allocated either way, so that one dry pass sizes both forms.
+int oracle_forward(Ctx& c, const float* wav, int B, int L_cap, const int* lens, float scale, float* wav_out) {
+  const int T = 1 + L_cap / 441, Tc = T + T % 2 + 4;
+  unsigned int* peak = c.ws->alloc<unsigned int>(B);
+  int* frames = c.ws->alloc<int>(B);
+  int* ext = c.ws->alloc<int>((size_t)EXT_LEVELS * B);
+  void* cond = c.ws->raw((size_t)B * Tc * 128 * c.e->esz());
+  if (!c.dry) {
+    VFX_TRY(oracle_frontend(wav, B, L_cap, lens, c.e->d_window, c.e->d_obasis, c.e->d_oband,
+                            c.e->d_oband + 128, peak, lens ? frames : nullptr, cond, c.prec(), nullptr, c.st));
+    if (lens) VFX_TRY(frame_extents(frames, B, T, ext, c.st));
+  }
+  if (lens) { c.ext = ext; c.ext_B = B; }
+  return vocoder_generator(c, cond, B, Tc, wav_out, -1, scale);
+}
+
+// the front end of oracle_forward alone, into fp32 conditions [B][Tc_cap][128]
+int oracle_cond_forward(Ctx& c, const float* wav, int B, int L_cap, const int* lens, float* cond_out) {
+  unsigned int* peak = c.ws->alloc<unsigned int>(B);
+  if (c.dry) return VFX_OK;
+  return oracle_frontend(wav, B, L_cap, lens, c.e->d_window, c.e->d_obasis, c.e->d_oband, c.e->d_oband + 128,
+                         peak, nullptr, nullptr, c.prec(), cond_out, c.st);
+}
+
+// Vocoder.oracle's mel basis: librosa.filters.mel(sr=44100, n_fft=2048, n_mels=128, fmin=0, fmax=22050, htk=True) with
+// its default norm="slaney" (vocoder/model/util.py:115-123), built in float64 as librosa builds it and cast to float32
+// (wavio.slaney_htk_mel_basis is the same formula on the host).  band: start[128] ++ len[128] of each row's non-zeros.
+void slaney_htk_mel_basis(std::vector<float>& basis, std::vector<int>& band) {
+  const int n_mels = 128, nbin = 1025;
+  double mel_f[130];
+  const double mmax = 2595.0 * log10(1.0 + 22050.0 / 700.0), step = mmax / 129.0;
+  for (int i = 0; i < 130; ++i) {
+    const double m = i == 129 ? mmax : i * step;                     // np.linspace(0, mmax, 130)
+    mel_f[i] = 700.0 * (pow(10.0, m / 2595.0) - 1.0);
+  }
+  basis.assign((size_t)n_mels * nbin, 0.f);
+  band.assign(2 * n_mels, 0);
+  for (int i = 0; i < n_mels; ++i) {
+    const double enorm = 2.0 / (mel_f[i + 2] - mel_f[i]);
+    int lo = -1, hi = -1;
+    for (int k = 0; k < nbin; ++k) {
+      const double f = k * (22050.0 / 1024.0);                       // np.linspace(0, sr / 2, 1025): exact steps
+      const double lower = -(mel_f[i] - f) / (mel_f[i + 1] - mel_f[i]);
+      const double upper = (mel_f[i + 2] - f) / (mel_f[i + 2] - mel_f[i + 1]);
+      const float w = (float)(std::max(0.0, std::min(lower, upper)) * enorm);
+      basis[(size_t)i * nbin + k] = w;
+      if (w != 0.f) { if (lo < 0) lo = k; hi = k; }
+    }
+    band[i] = lo < 0 ? 0 : lo;
+    band[n_mels + i] = lo < 0 ? 0 : hi - lo + 1;
+  }
+}
+
 // lens (ragged batch): per-item lengths on the device; L is then the capacity (row stride of wav / wav_out)
 int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop, const int* lens, float* wav_out) {
   const int T = 1 + L / 441;
@@ -788,6 +856,13 @@ int vfx_engine_create(vfx_engine** out, int device, int precision) {
   VFX_CUDA_CHECK(cudaMalloc(&e->d_tw, 1024 * sizeof(float2)));
   VFX_CUDA_CHECK(cudaMemcpy(e->d_window, win.data(), 2048 * sizeof(float), cudaMemcpyHostToDevice));
   VFX_CUDA_CHECK(cudaMemcpy(e->d_tw, tw.data(), 1024 * sizeof(float2), cudaMemcpyHostToDevice));
+  std::vector<float> basis;
+  std::vector<int> band;
+  slaney_htk_mel_basis(basis, band);
+  VFX_CUDA_CHECK(cudaMalloc(&e->d_obasis, basis.size() * sizeof(float)));
+  VFX_CUDA_CHECK(cudaMalloc(&e->d_oband, band.size() * sizeof(int)));
+  VFX_CUDA_CHECK(cudaMemcpy(e->d_obasis, basis.data(), basis.size() * sizeof(float), cudaMemcpyHostToDevice));
+  VFX_CUDA_CHECK(cudaMemcpy(e->d_oband, band.data(), band.size() * sizeof(int), cudaMemcpyHostToDevice));
   *out = e;
   return VFX_OK;
 }
@@ -797,6 +872,8 @@ int vfx_engine_destroy(vfx_engine* e) {
   if (e->device >= 0) {
     cudaFree(e->d_window);
     cudaFree(e->d_tw);
+    cudaFree(e->d_obasis);
+    cudaFree(e->d_oband);
   }
   delete e;
   return VFX_OK;
@@ -925,6 +1002,15 @@ size_t vfx_workspace_bytes_frames(const vfx_engine* e, int B, int T) {
   return bytes;
 }
 
+// oracle(): the planner is the dry pass of the whole call (front end, frame table, generator)
+size_t vfx_oracle_workspace_bytes(const vfx_engine* e, int B, int L_cap) {
+  if (!e || B <= 0 || L_cap <= 0 || (long long)(1 + L_cap / 441 + 5) * 441 > 0x7fffffffLL) return 0;
+  Bump ws(nullptr, 0);
+  Ctx c{const_cast<vfx_engine*>(e), nullptr, &ws, true, VFX_MODE_EVAL};
+  const int r = oracle_forward(c, nullptr, B, L_cap, nullptr, 1.f, nullptr);
+  return r == VFX_OK && c.rc == VFX_OK ? ws.peak : 0;
+}
+
 #define VFX_ENTER(e)                                                                     \
   VFX_REQUIRE((e) != nullptr, "null engine");                                            \
   VFX_REQUIRE((e)->finalized, "engine not finalized (call vfx_engine_finalize)");        \
@@ -1000,6 +1086,48 @@ int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav
   int r = cast_rows(cond, (long long)B * Tc * 128, op, e->precision, c.st);
   if (r != VFX_OK) return r;
   r = vocoder_generator(c, op, B, Tc, wav_out, trim_len, scale);
+  if (r != VFX_OK) return r;
+  VFX_FINISH(c, ws);
+}
+
+int vfx_vocoder_ragged(vfx_engine* e, const float* mel, int B, int T_cap, const int* frames, int input_is_log,
+                       float* wav_out, float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_REQUIRE(mel && frames && wav_out && B > 0 && T_cap > 0 && workspace, "vocoder_ragged: bad arguments");
+  VFX_PREFLIGHT(VFX_MODE_EVAL, vocoder_ragged_forward(c, mel, B, T_cap, frames, input_is_log, wav_out, scale));
+  Bump ws(workspace, workspace_bytes);
+  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
+  int r = vocoder_ragged_forward(c, mel, B, T_cap, frames, input_is_log, wav_out, scale);
+  if (r != VFX_OK) return r;
+  VFX_FINISH(c, ws);
+}
+
+#define VFX_ORACLE_ARGS(what)                                                                                       \
+  VFX_REQUIRE(wav && B > 0 && L_cap > 0 && workspace, what ": bad arguments");                                       \
+  VFX_REQUIRE((long long)(1 + L_cap / 441 + 5) * 441 <= 0x7fffffffLL, what ": L_cap=%d is too long", L_cap)
+
+int vfx_oracle_cond(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* cond_out, void* workspace,
+                    size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_ORACLE_ARGS("oracle_cond");
+  VFX_REQUIRE(cond_out, "oracle_cond: cond_out is null");
+  VFX_PREFLIGHT(VFX_MODE_EVAL, oracle_cond_forward(c, wav, B, L_cap, lens, cond_out));
+  Bump ws(workspace, workspace_bytes);
+  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
+  int r = oracle_cond_forward(c, wav, B, L_cap, lens, cond_out);
+  if (r != VFX_OK) return r;
+  VFX_FINISH(c, ws);
+}
+
+int vfx_oracle(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float scale, float* wav_out,
+               void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_ORACLE_ARGS("oracle");
+  VFX_REQUIRE(wav_out, "oracle: wav_out is null");
+  VFX_PREFLIGHT(VFX_MODE_EVAL, oracle_forward(c, wav, B, L_cap, lens, scale, wav_out));
+  Bump ws(workspace, workspace_bytes);
+  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
+  int r = oracle_forward(c, wav, B, L_cap, lens, scale, wav_out);
   if (r != VFX_OK) return r;
   VFX_FINISH(c, ws);
 }

@@ -125,6 +125,17 @@ enum {
 };
 // lens[B] -> ext[EXT_LEVELS][B]; every length is clamped into [1025, L_cap] first
 int ragged_extents(const int* lens, int B, int L_cap, int* ext, cudaStream_t st);
+// the same table for the vocoder alone, from mel frame counts frames[B] (clamped into [1, T_cap]): samples = S_b =
+// Tc_b * 441 (the untrimmed generated length), frames = T_b, the conditioning and up-sampler rows as above
+int frame_extents(const int* frames, int B, int T_cap, int* ext, cudaStream_t st);
+// Vocoder.oracle's front end (oracle_fe.cu).  wav[B][L_cap], item b = its first L_b = clamp(lens[b], 1, L_cap) samples
+// (lens NULL: L_cap each); peak_bits: B uint32 of workspace; frames (optional) receives T_b = 1 + L_b / 441.
+// Writes the normalised conditions [B][Tc_cap][128] in the operand format `precision` to cond_op and / or in fp32 to
+// cond_f32 (either may be NULL): rows T_b .. Tc_b - 1 are -4; rows from Tc_b on are -4 in cond_op and 0 in cond_f32.
+// basis / b_start / b_len: the Slaney HTK mel basis [128][1025] fp32 and its band of non-zero bins per row.
+int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const float* window,
+                    const float* basis, const int* b_start, const int* b_len, unsigned int* peak_bits, int* frames,
+                    void* cond_op, int precision, float* cond_f32, cudaStream_t st);
 int stft_mel(const float* wav, int B, int L, int T, const int* ext_len, const int* ext_frames, const float* window,
              const float2* tw, const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
              cudaStream_t st);

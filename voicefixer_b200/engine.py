@@ -55,6 +55,10 @@ class Planner:
         """analysis / vocoder entry points on B items of T mel frames."""
         return int(self.lib.vfx_workspace_bytes_frames(self.h, int(B), int(T)))
 
+    def oracle_workspace_bytes(self, B, L):
+        """Vocoder.oracle's device path on B recordings of L samples (0 for an out-of-range shape)."""
+        return int(self.lib.vfx_oracle_workspace_bytes(self.h, int(B), int(L)))
+
     def __del__(self):
         if getattr(self, "h", None):
             self.lib.vfx_engine_destroy(self.h)
@@ -163,8 +167,26 @@ class Engine:
         per_item = max(1, self.workspace_bytes(2, L) - self.workspace_bytes(1, L) + int(extra_per_item))
         return int(max(1, min(cap, avail // per_item)))
 
+    def max_batch_frames(self, T, cap=64, reserve=2 << 30, extra_per_item=0):
+        """max_batch for the vocoder: the largest number of mels of T frames (<= cap) whose vocoder() workspace fits the
+        memory that is free right now, keeping `reserve` bytes back.  At least 1."""
+        return self._fit(self.workspace_bytes_frames(2, T) - self.workspace_bytes_frames(1, T) + int(extra_per_item),
+                         cap, reserve)
+
+    def _fit(self, per_item, cap, reserve):
+        free, _ = torch.cuda.mem_get_info(self.device)
+        avail = free + (self._ws.numel() if self._ws is not None else 0) - reserve
+        return int(max(1, min(cap, avail // max(1, per_item))))
+
     def workspace_bytes(self, B, L):
         return int(self.lib.vfx_workspace_bytes(self.h, B, L))
+
+    def workspace_bytes_frames(self, B, T):
+        return int(self.lib.vfx_workspace_bytes_frames(self.h, int(B), int(T)))
+
+    def oracle_workspace_bytes(self, B, L):
+        """Workspace of oracle() on B recordings of (at most) L samples."""
+        return int(self.lib.vfx_oracle_workspace_bytes(self.h, int(B), int(L)))
 
     def _dev(self, x):
         if isinstance(x, np.ndarray):
@@ -198,15 +220,29 @@ class Engine:
                                          _stream()), "vfx_analysis")
         return out
 
-    def vocoder(self, mel, input_is_log=False, trim_len=-1, scale=1.0):
-        """mel (B, T, 128) -> wav (B, out_len)."""
+    def vocoder(self, mel, input_is_log=False, trim_len=-1, scale=1.0, lens=None, ws=None):
+        """mel (B, T, 128) -> wav (B, out_len).
+
+        lens (ragged batch): int32 device tensor (B,) of per-item frame counts <= T.  Row b of `mel` then holds item b in
+        its first lens[b] frames, and row b of the result (B, (T + T % 2 + 4) * 441) is bit-identical to the vocoder on
+        that item alone, its (T_b + T_b % 2 + 4) * 441 samples untrimmed, followed by zeros (vfx_vocoder_ragged).  Lengths
+        are read on the device, so a captured graph serves any lengths.  trim_len must stay -1."""
         mel = self._dev(mel)
         B, T, F = mel.shape
         if F != 128:
             raise AssertionError("mel must have 128 bins")
         S = (T + T % 2 + 4) * 441
+        if ws is None:
+            ws = self._workspace(self.workspace_bytes_frames(B, T))
+        if lens is not None:
+            _check_lens(lens, B)
+            if trim_len != -1:
+                raise ValueError("a ragged vocoder batch is untrimmed: trim_len must be -1")
+            out = torch.empty(B, S, device=mel.device)
+            _lib.check(self.lib.vfx_vocoder_ragged(self.h, _ptr(mel), B, T, _ptr(lens), int(bool(input_is_log)), _ptr(out),
+                                                   float(scale), _ptr(ws), ws.numel(), _stream()), "vfx_vocoder_ragged")
+            return out
         out = torch.empty(B, S if trim_len < 0 else trim_len, device=mel.device)
-        ws = self._workspace(int(self.lib.vfx_workspace_bytes_frames(self.h, B, T)))
         _lib.check(self.lib.vfx_vocoder(self.h, _ptr(mel), B, T, int(bool(input_is_log)), _ptr(out), int(trim_len),
                                         float(scale), _ptr(ws), ws.numel(), _stream()), "vfx_vocoder")
         return out
@@ -219,6 +255,31 @@ class Engine:
         ws = self._workspace(int(self.lib.vfx_workspace_bytes_frames(self.h, B, Tc)))
         _lib.check(self.lib.vfx_vocoder_cond(self.h, _ptr(cond), B, Tc, _ptr(out), int(trim_len), float(scale), _ptr(ws),
                                              ws.numel(), _stream()), "vfx_vocoder_cond")
+        return out
+
+    def oracle(self, wav, lens=None, scale=1.0, return_cond=False):
+        """Vocoder.oracle on the device (vfx_oracle): wav (B, L) -> wav (B, Tc * 441), Tc = T + T % 2 + 4, T = 1 + L // 441,
+        times `scale` (oracle() writes 2^15 x the Generator output).  Each row is peak-normalised on its own.
+
+        lens (ragged batch): int32 device tensor (B,) of per-item lengths <= L; row b of the result then holds item b's
+        (T_b + T_b % 2 + 4) * 441 samples and zeros after.  return_cond: run the front end only (vfx_oracle_cond) and
+        return its fp32 conditions (B, Tc, 128), channels-last, with zeros after each item's Tc_b rows."""
+        wav = self._dev(wav)
+        B, L = wav.shape
+        if lens is not None:
+            _check_lens(lens, B)
+        T = 1 + L // 441
+        Tc = T + T % 2 + 4
+        if return_cond:                                    # the front end's workspace: its per-item peaks
+            ws = self._workspace((4 * B + 255) // 256 * 256)
+            cond = torch.empty(B, Tc, 128, device=wav.device)
+            _lib.check(self.lib.vfx_oracle_cond(self.h, _ptr(wav), B, L, _ptr(lens), _ptr(cond), _ptr(ws), ws.numel(),
+                                                _stream()), "vfx_oracle_cond")
+            return cond
+        ws = self._workspace(self.oracle_workspace_bytes(B, L))
+        out = torch.empty(B, Tc * 441, device=wav.device)
+        _lib.check(self.lib.vfx_oracle(self.h, _ptr(wav), B, L, _ptr(lens), float(scale), _ptr(out), _ptr(ws), ws.numel(),
+                                       _stream()), "vfx_oracle")
         return out
 
     def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None, lens=None):
