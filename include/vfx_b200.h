@@ -176,15 +176,18 @@ int vfx_restore_ragged_mode(vfx_engine* e, const float* wav, int B, int L_cap, c
 
 /* mode 1 pre-filter, VoiceFixer.remove_higher_frequency (voicefixer/base.py:87-104) with the
  * librosa 0.10.1 stft/istft defaults (n_fft 2048, hop 512, Hann, center, zero pad):
- * wav[B][L] -> wav_out[B][512*(L/512)].  Returns the per-item cut bin in cut_bins[B] (optional). */
+ * wav[B][L] -> wav_out[B][512*(L/512)].  Returns the per-item cut bin in cut_bins[B] (optional).
+ * Workspace: vfx_hf_cut_workspace_bytes(B, L). */
 int vfx_hf_cut(vfx_engine* e, const float* wav, int B, int L, float ratio, float* wav_out,
                int* cut_bins, void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace of vfx_hf_cut for (B, L) and of vfx_hf_cut_ragged for (B, L_cap); needs no engine.  0 for a negative B or L. */
+size_t vfx_hf_cut_workspace_bytes(int B, int L);
 
 /* vfx_hf_cut for B items of DIFFERENT lengths: wav[B][L_cap] holds item b in its first lens[b] samples (device int32;
  * clamped into [512, L_cap]; the rest of the row is never read).  Item b is filtered as if it were alone: its own
  * 1 + L_b/512 frames set its cut bin, and wav_out[B][L_cap] receives its 512*(L_b/512) filtered samples followed by
  * zeros.  lens_out[B] (device int32, optional) receives those lengths, so the result can feed vfx_restore_ragged(_mode)
- * without a host round trip (mode 1 of a ragged batch).  Workspace: that of vfx_hf_cut for (B, L_cap). */
+ * without a host round trip (mode 1 of a ragged batch).  Workspace: vfx_hf_cut_workspace_bytes(B, L_cap). */
 int vfx_hf_cut_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float ratio, float* wav_out,
                       int* lens_out, int* cut_bins, void* workspace, size_t workspace_bytes, void* stream);
 

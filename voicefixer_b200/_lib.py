@@ -61,6 +61,7 @@ SIGNATURES = {
     "vfx_vocoder_cond": (_i, [_vp, _vp, _i, _i, _vp, _i, _f, _vp, _sz, _vp]),
     "vfx_restore": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_hf_cut": (_i, [_vp, _vp, _i, _i, _f, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_hf_cut_workspace_bytes": (_sz, [_i, _i]),
     "vfx_conv_gemm": (_i, [_i, _i, _c.POINTER(ConvDesc), _vp]),
     "vfx_resstack_pair": (_i, [_c.POINTER(PairDesc), _vp]),
     "vfx_resstack_pair_scratch_bytes": (_sz, []),

@@ -719,6 +719,13 @@ int vocoder_forward(Ctx& c, const float* mel, int B, int T, int input_is_log, fl
   return c.rc;
 }
 
+// the Generator on fp32 conditions cond[B][Tc][128], cast into the operand format in the workspace first
+int vocoder_cond_forward(Ctx& c, const float* cond, int B, int Tc, float* wav_out, int trim_len, float scale) {
+  void* op = c.ws->raw((size_t)B * Tc * 128 * c.e->esz());
+  if (!c.dry) VFX_TRY(cast_rows(cond, (long long)B * Tc * 128, op, c.prec(), c.st));
+  return vocoder_generator(c, op, B, Tc, wav_out, trim_len, scale);
+}
+
 int frontend_forward(Ctx& c, const float* wav, int B, int L, float* mel, float* sp) {
   const int T = 1 + L / 441;
   const float* fbT = getf(c, "fe.fbT", (size_t)128 * 1025);
@@ -809,6 +816,36 @@ int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop,
   VFX_TRY(frontend_forward(c, wav, B, L, mel, nullptr));
   VFX_TRY(analysis_forward(c, mel, B, T, drop, mel_log));
   VFX_TRY(vocoder_forward(c, mel_log, B, T, 1, wav_out, L, 1.0f));
+  return c.rc;
+}
+
+// The planner: runs fwd(Ctx&) on a null allocator, which makes no CUDA call, and returns the peak of its workspace.
+// *rc receives fwd's status.
+template <typename F>
+size_t dry_peak(vfx_engine* e, int mode, F&& fwd, int* rc) {
+  Bump ws(nullptr, 0);
+  Ctx c{e, nullptr, &ws, true, mode};
+  const int r = fwd(c);
+  *rc = r != VFX_OK ? r : c.rc;
+  return ws.peak;
+}
+
+// One launching call: fwd(Ctx&) runs dry first, so that a workspace below its peak is refused before the first launch (a
+// bump allocator that overflows mid-sequence would alias buffers), then the same fwd runs live.  Because one callable
+// serves both passes, the size the call checks is the size its launches use.
+template <typename F>
+int planned_call(vfx_engine* e, int mode, void* workspace, size_t workspace_bytes, void* stream, F&& fwd) {
+  int r;
+  const size_t need = dry_peak(e, mode, fwd, &r);
+  if (r != VFX_OK) return r;
+  if (need > workspace_bytes) {
+    set_error("workspace too small: %zu bytes given, this call needs %zu", workspace_bytes, need);
+    return VFX_ERR_WORKSPACE;
+  }
+  Bump ws(workspace, workspace_bytes);
+  Ctx c{e, (cudaStream_t)stream, &ws, false, mode};
+  VFX_TRY(fwd(c));
+  if (ws.overflow) { set_error("workspace too small: need %zu bytes", ws.peak); return VFX_ERR_WORKSPACE; }
   return c.rc;
 }
 
@@ -928,33 +965,28 @@ int vfx_engine_set_tensor(vfx_engine* e, const char* name, const void* dev_ptr, 
   return VFX_OK;
 }
 
-static int dry_run(vfx_engine* e, int B, int T, int L, size_t* bytes) {
-  Bump ws(nullptr, 0);
-  Ctx c{e, nullptr, &ws, true, VFX_MODE_TRAIN_BN};
-  int r;
-  if (L > 0) r = restore_forward(c, nullptr, B, L, nullptr, nullptr, nullptr);
-  else {
-    float* mel = ws.alloc<float>((size_t)B * T * 128);
+// The restore planner (L > 0) or the frames planner (B items of T frames: analysis + vocoder, or the vocoder alone on a
+// vocoder-only engine), in mode 2, whose batch statistics take the most workspace.  The slack also holds
+// vfx_restore_ragged's extent table, so one workspace size serves both entry points.
+static size_t dry_run(vfx_engine* e, int B, int T, int L, int* rc) {
+  const size_t peak = dry_peak(e, VFX_MODE_TRAIN_BN, [&](Ctx& c) {
+    if (L > 0) return restore_forward(c, nullptr, B, L, nullptr, nullptr, nullptr);
+    float* mel = c.ws->alloc<float>((size_t)B * T * 128);
     const bool voc_only = e->finalized && !(e->parts & VFX_PART_ANALYSIS);
-    r = voc_only ? VFX_OK : analysis_forward(c, mel, B, T, nullptr, mel);
-    if (r == VFX_OK) r = vocoder_forward(c, mel, B, T, 1, nullptr, -1, 1.f);
-  }
-  // the slack also holds vfx_restore_ragged's extent table, so one workspace size serves both entry points
-  *bytes = ws.peak + std::max<size_t>(4096, ext_table_bytes(B));
-  return r;
+    const int r = voc_only ? VFX_OK : analysis_forward(c, mel, B, T, nullptr, mel);
+    return r != VFX_OK ? r : vocoder_forward(c, mel, B, T, 1, nullptr, -1, 1.f);
+  }, rc);
+  return peak + std::max<size_t>(4096, ext_table_bytes(B));
 }
 
 int vfx_engine_finalize(vfx_engine* e) {
   VFX_REQUIRE(e, "finalize: null engine");
   e->missing.clear();
-  size_t bytes = 0;
-  int r = dry_run(e, 1, 64, 0, &bytes);
-  {   // also the front-end tables
-    Bump ws(nullptr, 0);
-    Ctx c{e, nullptr, &ws, true, VFX_MODE_EVAL};
-    int r2 = frontend_forward(c, nullptr, 1, 44100, nullptr, nullptr);
-    if (r == VFX_OK) r = r2;
-  }
+  int r, r2;
+  dry_run(e, 1, 64, 0, &r);
+  // also the front-end tables
+  dry_peak(e, VFX_MODE_EVAL, [](Ctx& c) { return frontend_forward(c, nullptr, 1, 44100, nullptr, nullptr); }, &r2);
+  if (r == VFX_OK) r = r2;
   if (!e->missing.empty()) {
     // The reference's stand-alone Vocoder class (voicefixer/vocoder/base.py:10-40) loads the synthesis checkpoint only.
     // An engine that holds nothing but "voc." tensors, all of them present, is complete for vfx_vocoder /
@@ -964,16 +996,17 @@ int vfx_engine_finalize(vfx_engine* e) {
     if (voc_only) {
       std::vector<std::string> analysis_missing;
       analysis_missing.swap(e->missing);
-      Bump ws(nullptr, 0);
-      Ctx c{e, nullptr, &ws, true, VFX_MODE_EVAL};
-      float* mel = ws.alloc<float>((size_t)64 * 128);
-      const int rv = vocoder_forward(c, mel, 1, 64, 1, nullptr, -1, 1.f);
-      if (rv == VFX_OK && c.rc == VFX_OK && e->missing.empty()) {
+      int rv;
+      dry_peak(e, VFX_MODE_EVAL, [](Ctx& c) {
+        float* mel = c.ws->alloc<float>((size_t)64 * 128);
+        return vocoder_forward(c, mel, 1, 64, 1, nullptr, -1, 1.f);
+      }, &rv);
+      if (rv == VFX_OK && e->missing.empty()) {
         e->parts = VFX_PART_VOCODER;
         e->finalized = true;
         return VFX_OK;
       }
-      if (e->missing.empty()) return rv != VFX_OK ? rv : c.rc;     // e.g. a tensor of the wrong size: message already set
+      if (e->missing.empty()) return rv;     // e.g. a tensor of the wrong size: message already set
     }
     std::string s = "missing weight tensors:";
     for (size_t i = 0; i < e->missing.size() && i < 12; ++i) s += " " + e->missing[i];
@@ -990,25 +1023,23 @@ int vfx_engine_finalize(vfx_engine* e) {
 size_t vfx_workspace_bytes(const vfx_engine* e, int B, int L) {
   if (!e || B <= 0 || L <= 1024) return 0;
   if (e->finalized && !(e->parts & VFX_PART_ANALYSIS)) return 0;   // restore() needs the analysis weights
-  size_t bytes = 0;
-  dry_run(const_cast<vfx_engine*>(e), B, 0, L, &bytes);
-  return bytes;
+  int rc;
+  return dry_run(const_cast<vfx_engine*>(e), B, 0, L, &rc);
 }
 
 size_t vfx_workspace_bytes_frames(const vfx_engine* e, int B, int T) {
   if (!e || B <= 0 || T <= 0) return 0;
-  size_t bytes = 0;
-  dry_run(const_cast<vfx_engine*>(e), B, T, 0, &bytes);
-  return bytes;
+  int rc;
+  return dry_run(const_cast<vfx_engine*>(e), B, T, 0, &rc);
 }
 
 // oracle(): the planner is the dry pass of the whole call (front end, frame table, generator)
 size_t vfx_oracle_workspace_bytes(const vfx_engine* e, int B, int L_cap) {
   if (!e || B <= 0 || L_cap <= 0 || (long long)(1 + L_cap / 441 + 5) * 441 > 0x7fffffffLL) return 0;
-  Bump ws(nullptr, 0);
-  Ctx c{const_cast<vfx_engine*>(e), nullptr, &ws, true, VFX_MODE_EVAL};
-  const int r = oracle_forward(c, nullptr, B, L_cap, nullptr, 1.f, nullptr);
-  return r == VFX_OK && c.rc == VFX_OK ? ws.peak : 0;
+  int rc;
+  const size_t peak = dry_peak(const_cast<vfx_engine*>(e), VFX_MODE_EVAL,
+                               [&](Ctx& c) { return oracle_forward(c, nullptr, B, L_cap, nullptr, 1.f, nullptr); }, &rc);
+  return rc == VFX_OK ? peak : 0;
 }
 
 #define VFX_ENTER(e)                                                                     \
@@ -1021,31 +1052,13 @@ size_t vfx_oracle_workspace_bytes(const vfx_engine* e, int B, int L_cap) {
   VFX_REQUIRE((e)->parts & VFX_PART_ANALYSIS,                                            \
               "this engine holds the vocoder weights only (stand-alone Vocoder); the analysis module is not loaded")
 
-// Pre-flight: the same forward pass on a null allocator gives the exact workspace need of THIS call; a too-small
-// workspace is refused before the first launch (a bump allocator that overflows mid-sequence would alias buffers).
-#define VFX_PREFLIGHT(mode_, call_)                                                                       \
-  do {                                                                                                    \
-    Bump dry_(nullptr, 0);                                                                                \
-    Ctx c{e, nullptr, &dry_, true, (mode_)};                                                              \
-    int r_ = (call_);                                                                                     \
-    if (r_ != VFX_OK) return r_;                                                                          \
-    if (dry_.peak > workspace_bytes) {                                                                    \
-      set_error("workspace too small: %zu bytes given, this call needs %zu", (size_t)workspace_bytes, dry_.peak); \
-      return VFX_ERR_WORKSPACE;                                                                           \
-    }                                                                                                     \
-  } while (0)
-
-#define VFX_FINISH(c, ws)                                                                \
-  if ((ws).overflow) { set_error("workspace too small: need %zu bytes", (ws).peak); return VFX_ERR_WORKSPACE; } \
-  return (c).rc
-
 int vfx_frontend_mel(vfx_engine* e, const float* wav, int B, int L, float* mel, float* sp_out, void* stream) {
   VFX_ENTER(e);
   VFX_NEED_ANALYSIS(e);
   VFX_REQUIRE(wav && mel && B > 0, "frontend: bad arguments");
-  Bump ws(nullptr, 0);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  return frontend_forward(c, wav, B, L, mel, sp_out);
+  // no workspace: an allocation the front end might make is refused by the dry pass
+  return planned_call(e, VFX_MODE_EVAL, nullptr, 0, stream,
+                      [&](Ctx& c) { return frontend_forward(c, wav, B, L, mel, sp_out); });
 }
 
 int vfx_analysis(vfx_engine* e, const float* mel, int B, int T, int mode, const uint8_t* drop_masks,
@@ -1054,52 +1067,33 @@ int vfx_analysis(vfx_engine* e, const float* mel, int B, int T, int mode, const 
   VFX_NEED_ANALYSIS(e);
   VFX_REQUIRE(mel && mel_log_out && B > 0 && T > 0 && workspace, "analysis: bad arguments");
   VFX_REQUIRE(mode == VFX_MODE_EVAL || mode == VFX_MODE_TRAIN_BN, "analysis: bad mode %d", mode);
-  VFX_PREFLIGHT(mode, analysis_forward(c, mel, B, T, nullptr, mel_log_out));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, mode};
-  int r = analysis_forward(c, mel, B, T, drop_masks, mel_log_out);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, mode, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return analysis_forward(c, mel, B, T, drop_masks, mel_log_out); });
 }
 
 int vfx_vocoder(vfx_engine* e, const float* mel, int B, int T, int input_is_log, float* wav_out, int trim_len,
                 float scale, void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
   VFX_REQUIRE(mel && wav_out && B > 0 && T > 0 && workspace, "vocoder: bad arguments");
-  VFX_PREFLIGHT(VFX_MODE_EVAL, vocoder_forward(c, mel, B, T, input_is_log, wav_out, trim_len, scale));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  int r = vocoder_forward(c, mel, B, T, input_is_log, wav_out, trim_len, scale);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return vocoder_forward(c, mel, B, T, input_is_log, wav_out, trim_len, scale); });
 }
 
 int vfx_vocoder_cond(vfx_engine* e, const float* cond, int B, int Tc, float* wav_out, int trim_len, float scale,
                      void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
   VFX_REQUIRE(cond && wav_out && B > 0 && Tc >= 4 && workspace, "vocoder_cond: bad arguments");
-  VFX_PREFLIGHT(VFX_MODE_EVAL, (dry_.raw((size_t)B * Tc * 128 * e->esz()), vocoder_generator(c, nullptr, B, Tc, wav_out, trim_len, scale)));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  void* op = ws.raw((size_t)B * Tc * 128 * e->esz());
-  if (ws.overflow) { set_error("workspace too small"); return VFX_ERR_WORKSPACE; }
-  int r = cast_rows(cond, (long long)B * Tc * 128, op, e->precision, c.st);
-  if (r != VFX_OK) return r;
-  r = vocoder_generator(c, op, B, Tc, wav_out, trim_len, scale);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return vocoder_cond_forward(c, cond, B, Tc, wav_out, trim_len, scale); });
 }
 
 int vfx_vocoder_ragged(vfx_engine* e, const float* mel, int B, int T_cap, const int* frames, int input_is_log,
                        float* wav_out, float scale, void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
   VFX_REQUIRE(mel && frames && wav_out && B > 0 && T_cap > 0 && workspace, "vocoder_ragged: bad arguments");
-  VFX_PREFLIGHT(VFX_MODE_EVAL, vocoder_ragged_forward(c, mel, B, T_cap, frames, input_is_log, wav_out, scale));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  int r = vocoder_ragged_forward(c, mel, B, T_cap, frames, input_is_log, wav_out, scale);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream, [&](Ctx& c) {
+    return vocoder_ragged_forward(c, mel, B, T_cap, frames, input_is_log, wav_out, scale);
+  });
 }
 
 #define VFX_ORACLE_ARGS(what)                                                                                       \
@@ -1111,12 +1105,8 @@ int vfx_oracle_cond(vfx_engine* e, const float* wav, int B, int L_cap, const int
   VFX_ENTER(e);
   VFX_ORACLE_ARGS("oracle_cond");
   VFX_REQUIRE(cond_out, "oracle_cond: cond_out is null");
-  VFX_PREFLIGHT(VFX_MODE_EVAL, oracle_cond_forward(c, wav, B, L_cap, lens, cond_out));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  int r = oracle_cond_forward(c, wav, B, L_cap, lens, cond_out);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return oracle_cond_forward(c, wav, B, L_cap, lens, cond_out); });
 }
 
 int vfx_oracle(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float scale, float* wav_out,
@@ -1124,12 +1114,8 @@ int vfx_oracle(vfx_engine* e, const float* wav, int B, int L_cap, const int* len
   VFX_ENTER(e);
   VFX_ORACLE_ARGS("oracle");
   VFX_REQUIRE(wav_out, "oracle: wav_out is null");
-  VFX_PREFLIGHT(VFX_MODE_EVAL, oracle_forward(c, wav, B, L_cap, lens, scale, wav_out));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, VFX_MODE_EVAL};
-  int r = oracle_forward(c, wav, B, L_cap, lens, scale, wav_out);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return oracle_forward(c, wav, B, L_cap, lens, scale, wav_out); });
 }
 
 static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
@@ -1139,12 +1125,8 @@ static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode
   VFX_REQUIRE(wav && wav_out && B > 0 && workspace, "restore: bad arguments");
   VFX_REQUIRE(mode == VFX_MODE_EVAL || mode == VFX_MODE_TRAIN_BN, "restore: bad mode %d", mode);
   VFX_REQUIRE(L > 1024, "restore: L=%d must exceed 1024 samples", L);
-  VFX_PREFLIGHT(mode, restore_forward(c, wav, B, L, nullptr, lens, wav_out));
-  Bump ws(workspace, workspace_bytes);
-  Ctx c{e, (cudaStream_t)stream, &ws, false, mode};
-  int r = restore_forward(c, wav, B, L, drop_masks, lens, wav_out);
-  if (r != VFX_OK) return r;
-  VFX_FINISH(c, ws);
+  return planned_call(e, mode, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return restore_forward(c, wav, B, L, drop_masks, lens, wav_out); });
 }
 
 int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
@@ -1164,6 +1146,8 @@ int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const 
   return vfx_restore_ragged_mode(e, wav, B, L_cap, lens, VFX_MODE_EVAL, nullptr, wav_out, workspace, workspace_bytes,
                                  stream);
 }
+
+size_t vfx_hf_cut_workspace_bytes(int B, int L) { return B < 0 || L < 0 ? 0 : hf_cut_workspace(B, L); }
 
 int vfx_hf_cut(vfx_engine* e, const float* wav, int B, int L, float ratio, float* wav_out, int* cut_bins,
                void* workspace, size_t workspace_bytes, void* stream) {

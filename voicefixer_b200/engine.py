@@ -30,7 +30,23 @@ def default_precision():
     return os.environ.get("VFX_PRECISION", "tf32")
 
 
-class Planner:
+class _WorkspaceQueries:
+    """The library's workspace planners on the engine handle `self.h`."""
+
+    def workspace_bytes(self, B, L):
+        """restore() on B items of L samples; 0 for a vocoder-only weight set."""
+        return int(self.lib.vfx_workspace_bytes(self.h, int(B), int(L)))
+
+    def workspace_bytes_frames(self, B, T):
+        """analysis / vocoder entry points on B items of T mel frames."""
+        return int(self.lib.vfx_workspace_bytes_frames(self.h, int(B), int(T)))
+
+    def oracle_workspace_bytes(self, B, L):
+        """Vocoder.oracle's device path on B recordings of (at most) L samples (0 for an out-of-range shape)."""
+        return int(self.lib.vfx_oracle_workspace_bytes(self.h, int(B), int(L)))
+
+
+class Planner(_WorkspaceQueries):
     """Planning-only engine (vfx_engine_create with device -1): validates a packed weight set against what the
     kernels expect (names, byte sizes) and sizes the activation workspace for a batch -- no GPU, no CUDA call.
     `packed`: {name: CPU tensor} from weights.pack_analysis / pack_vocoder (either both, or the vocoder alone)."""
@@ -47,25 +63,13 @@ class Planner:
                        f"set_tensor({name})")
         _lib.check(self.lib.vfx_engine_finalize(self.h), "vfx_engine_finalize")
 
-    def workspace_bytes(self, B, L):
-        """restore() on B items of L samples; 0 for a vocoder-only weight set."""
-        return int(self.lib.vfx_workspace_bytes(self.h, int(B), int(L)))
-
-    def workspace_bytes_frames(self, B, T):
-        """analysis / vocoder entry points on B items of T mel frames."""
-        return int(self.lib.vfx_workspace_bytes_frames(self.h, int(B), int(T)))
-
-    def oracle_workspace_bytes(self, B, L):
-        """Vocoder.oracle's device path on B recordings of L samples (0 for an out-of-range shape)."""
-        return int(self.lib.vfx_oracle_workspace_bytes(self.h, int(B), int(L)))
-
     def __del__(self):
         if getattr(self, "h", None):
             self.lib.vfx_engine_destroy(self.h)
             self.h = None
 
 
-class Engine:
+class Engine(_WorkspaceQueries):
     """One engine per process / GPU.  `ana`, `voc`: reference-layout state dicts (CPU tensors)."""
 
     def __init__(self, ana=None, voc=None, device=None, precision=None, packed=None):
@@ -162,10 +166,7 @@ class Engine:
         """Largest number of equal-length items (<= cap) whose restore() workspace fits the memory that is free right now
         (plus the workspace this engine already holds), keeping `reserve` bytes back.  At least 1.  extra_per_item: other
         device bytes each item needs alongside (e.g. the mode-1 pre-filter's workspace and output)."""
-        free, _ = torch.cuda.mem_get_info(self.device)
-        avail = free + (self._ws.numel() if self._ws is not None else 0) - reserve
-        per_item = max(1, self.workspace_bytes(2, L) - self.workspace_bytes(1, L) + int(extra_per_item))
-        return int(max(1, min(cap, avail // per_item)))
+        return self._fit(self.workspace_bytes(2, L) - self.workspace_bytes(1, L) + int(extra_per_item), cap, reserve)
 
     def max_batch_frames(self, T, cap=64, reserve=2 << 30, extra_per_item=0):
         """max_batch for the vocoder: the largest number of mels of T frames (<= cap) whose vocoder() workspace fits the
@@ -177,16 +178,6 @@ class Engine:
         free, _ = torch.cuda.mem_get_info(self.device)
         avail = free + (self._ws.numel() if self._ws is not None else 0) - reserve
         return int(max(1, min(cap, avail // max(1, per_item))))
-
-    def workspace_bytes(self, B, L):
-        return int(self.lib.vfx_workspace_bytes(self.h, B, L))
-
-    def workspace_bytes_frames(self, B, T):
-        return int(self.lib.vfx_workspace_bytes_frames(self.h, int(B), int(T)))
-
-    def oracle_workspace_bytes(self, B, L):
-        """Workspace of oracle() on B recordings of (at most) L samples."""
-        return int(self.lib.vfx_oracle_workspace_bytes(self.h, int(B), int(L)))
 
     def _dev(self, x):
         if isinstance(x, np.ndarray):
@@ -211,7 +202,7 @@ class Engine:
         if F != 128:
             raise AssertionError("mel must have 128 bins")
         out = torch.empty_like(mel)
-        ws = self._workspace(int(self.lib.vfx_workspace_bytes_frames(self.h, B, T)))
+        ws = self._workspace(self.workspace_bytes_frames(B, T))
         dm = None
         if drop_masks is not None:
             dm = drop_masks.to(device=mel.device, dtype=torch.uint8).contiguous()
@@ -252,7 +243,7 @@ class Engine:
         cond = self._dev(cond)
         B, Tc, F = cond.shape
         out = torch.empty(B, Tc * 441 if trim_len < 0 else trim_len, device=cond.device)
-        ws = self._workspace(int(self.lib.vfx_workspace_bytes_frames(self.h, B, Tc)))
+        ws = self._workspace(self.workspace_bytes_frames(B, Tc))
         _lib.check(self.lib.vfx_vocoder_cond(self.h, _ptr(cond), B, Tc, _ptr(out), int(trim_len), float(scale), _ptr(ws),
                                              ws.numel(), _stream()), "vfx_vocoder_cond")
         return out
@@ -334,8 +325,8 @@ class Engine:
 
     @staticmethod
     def hf_cut_workspace_bytes(B, L):
-        nfr = 1 + L // 512
-        return B * nfr * (1025 * 8 + 2048 * 4) + B * 1025 * 8 + (1 << 16)
+        """Workspace of hf_cut() on B items of (at most) L samples (vfx_hf_cut_workspace_bytes; no engine needed)."""
+        return int(_lib.load().vfx_hf_cut_workspace_bytes(int(B), int(L)))
 
     def hf_cut(self, wav, ratio=0.95, lens=None):
         """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
