@@ -191,6 +191,37 @@ size_t vfx_hf_cut_workspace_bytes(int B, int L);
 int vfx_hf_cut_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float ratio, float* wav_out,
                       int* lens_out, int* cut_bins, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- sample-rate conversion ------------------------------------------------------------ */
+
+/* One item of vfx_resample: output samples [y_first, y_first + y_len) of one recording's 44.1 kHz stream, computed from
+ * a window of its samples.  The recording has n_in samples; x[x_off .. x_off + x_len) holds its samples
+ * [x_first, x_first + x_len).  up / down: 44100 / rate in lowest terms (1 / 1 = a copy).  h[h_off .. h_off + h_len) holds
+ * the ratio's taps h', pre-padded with zeros and scaled by up, and rem is their output offset (a copy needs neither). */
+typedef struct vfx_resample_item {
+  long long x_off, x_first, n_in;
+  long long y_first;
+  long long h_off;
+  int x_len, y_len;
+  int up, down, rem, h_len;
+} vfx_resample_item;
+
+/* Resampling as librosa.load(path, sr=44100) does it in this project: scipy.signal.resample_poly(x, up, down) on float32
+ * input (the host loader, wavio._resample), bit for bit, for B items of mixed rates in one launch.  Output j of an
+ * item's stream is the sum, in float32 from 0 with a separate multiply and add per tap, over ascending inputs
+ * i = max(0, ceil((p - h_len + 1) / up)) .. min(n_in - 1, floor(p / up)), p = (j + rem) * down, of x[i] * h'[p - i*up].
+ * voicefixer_b200/resample.py builds the taps and the windows.
+ * y[B][L_cap]: row b receives item b's y_len samples, then zeros.  lens_out[B] (device int32, optional) receives y_len,
+ * ready for vfx_restore_ragged_mode / vfx_hf_cut_ragged / vfx_oracle.  items_host is a host array; the library
+ * validates every item before any launch: up, down >= 1; the window lies inside x[0, x_elems) and inside the recording;
+ * the taps lie inside h[0, h_elems); 0 <= y_len <= L_cap; the outputs lie inside the stream's ceil(n_in * up / down)
+ * samples; and the window holds every input those outputs read.  A bad item returns VFX_ERR_INVALID naming it, and
+ * nothing is launched or written.  The table is staged into the workspace: vfx_resample_workspace_bytes(B) bytes
+ * (needs no engine; 0 for B <= 0).  B <= 65535. */
+int vfx_resample(vfx_engine* e, const float* x, long long x_elems, const float* h, long long h_elems,
+                 const vfx_resample_item* items_host, int B, float* y, int L_cap, int* lens_out,
+                 void* workspace, size_t workspace_bytes, void* stream);
+size_t vfx_resample_workspace_bytes(int B);
+
 /* ---- per-kernel test entry points (tests/ call the kernels through these) --------------- */
 
 /* Generic channels-last "shifted-window" convolution GEMM; the one kernel family behind every

@@ -42,6 +42,12 @@ class PairDesc(ctypes.Structure):
                 ("scratch", _vp), ("scratch_bytes", _sz), ("lens", _vp)]
 
 
+class ResampleItem(ctypes.Structure):
+    """struct vfx_resample_item (include/vfx_b200.h)."""
+    _fields_ = [("x_off", _ll), ("x_first", _ll), ("n_in", _ll), ("y_first", _ll), ("h_off", _ll),
+                ("x_len", _i), ("y_len", _i), ("up", _i), ("down", _i), ("rem", _i), ("h_len", _i)]
+
+
 # name -> (restype, argtypes); must list every symbol include/vfx_b200.h declares
 SIGNATURES = {
     "vfx_last_error": (_c.c_char_p, []),
@@ -74,6 +80,8 @@ SIGNATURES = {
     "vfx_oracle_cond": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_oracle": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _sz, _vp]),
     "vfx_oracle_workspace_bytes": (_sz, [_vp, _i, _i]),
+    "vfx_resample": (_i, [_vp, _vp, _ll, _vp, _ll, _c.POINTER(ResampleItem), _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "vfx_resample_workspace_bytes": (_sz, [_i]),
 }
 
 _lib = None

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from .engine import Engine, default_precision
-from . import wavio
+from . import resample, wavio
 
 SEG_LENGTH = 44100 * 30                      # voicefixer/base.py:116
 ANALYSIS_CKPT = ".cache/voicefixer/analysis_module/checkpoints/vf.ckpt"
@@ -111,12 +111,13 @@ def plan_many(lengths, mode, max_items):
     return batches
 
 
-def plan_vocoder_many(items, kind, max_items):
+def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
     """Packs the items of Vocoder.forward_many (kind "mel": [1, 1, T, 128] mels) or Vocoder.oracle_many (kind "wav": 1-D
     float32 recordings) into ragged batches.  Items are ordered by length, longest first (stable, so equal lengths keep
     their order), and each batch takes the longest item left plus up to max_items(cap) - 1 of the next ones, cap being
     that first item's length in frames (mels) or samples (recordings): the batch's capacity.  Returns
-    [(cap, [item, ...]), ...].
+    [(cap, [item, ...]), ...].  pack_lengths (optional): the lengths to pack by in place of the items' own, e.g. recordings'
+    lengths at 44.1 kHz when they are resampled on the device; the items are validated all the same.
 
     Raises before anything is sized or launched, naming the item: ValueError for an empty list, a mel that is not
     [1, 1, T >= 1, 128], or a recording that is empty, not 1-D or all zeros (the reference divides by its zero peak);
@@ -141,6 +142,8 @@ def plan_vocoder_many(items, kind, max_items):
             if not np.any(x):
                 raise ValueError(f"{what}: item {i} is all zeros; its peak normalisation would divide by zero")
             lengths.append(shape[0])
+    if pack_lengths is not None:
+        lengths = [int(n) for n in pack_lengths]
     order = sorted(range(len(items)), key=lambda i: -lengths[i])
     batches, k = [], 0
     while k < len(order):
@@ -233,33 +236,63 @@ class Vocoder:
         wavio.save_wave(out[:, None, :].cpu().numpy(), out_path, sample_rate=self.rate)
 
     @torch.no_grad()
-    def oracle_many(self, wavs, cuda=True):
+    def oracle_many(self, wavs, cuda=True, sample_rate=44100):
         """Extension of the reference API: oracle()'s computation on a list of 1-D float32 recordings of any lengths, each
         one whole sequence (no 30 s segments), front end included on the device (vfx_oracle).  Element i is a
         (1, (T_i + T_i % 2 + 4) * 441) float32 array, T_i = 1 + L_i // 441: the Generator output before oracle()'s x 2^15
         and int16 file write.  The recordings run as ragged batches ordered by length (plan_vocoder_many), each sized to
-        the device memory that is free.  Bad input raises before anything is launched."""
+        the device memory that is free.  Bad input raises before anything is launched.
+
+        sample_rate: the recordings' rate in Hz, one positive int or one per recording.  A recording at another rate than
+        44100 is resampled on the device (vfx_resample) straight into the batch, bit-identical to oracle_many on
+        wavio._resample(wavs[i], rate_i, 44100), the host resampler oracle() reads files with; L_i is then its length at
+        44.1 kHz.  A call in which every rate is 44100 launches nothing for it."""
         _check_cuda(cuda)
         items = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
+        rates = resample.rates(sample_rate, len(items), "oracle_many")
+        convert = any(r != resample.RATE for r in rates)
         eng = self._engine
         dev = f"cuda:{eng.device}"
 
         def max_items(L):
             T = 1 + L // 441
             per_item = eng.oracle_workspace_bytes(2, L) - eng.oracle_workspace_bytes(1, L) + 4 * (L + (T + T % 2 + 4) * 441)
+            if convert:       # the staged input windows and the resampler's item table
+                per_item += 4 * max(resample.staging_bound(L, r) for r in set(rates)) + 64
             return eng._fit(per_item, 64, 2 << 30)
 
+        lengths = None
+        if convert:
+            lengths = [resample.out_len(a.shape[0], r) if a.ndim == 1 else 0 for a, r in zip(items, rates)]
         outs = [None] * len(items)
-        for L_cap, idx in plan_vocoder_many(items, "wav", max_items):
-            x = torch.zeros((len(idx), L_cap))
+        for L_cap, idx in plan_vocoder_many(items, "wav", max_items, pack_lengths=lengths):
+            if convert:
+                y, lens = eng.resample(*_stage(items, rates, [(i, 0, lengths[i]) for i in idx], dev), L_cap)
+            else:
+                x = torch.zeros((len(idx), L_cap))
+                for k, i in enumerate(idx):
+                    x[k, :items[i].shape[0]] = torch.from_numpy(items[i])
+                y = x.to(dev)
+                lens = torch.tensor([items[i].shape[0] for i in idx], dtype=torch.int32).to(dev)
+            y = eng.oracle(y, lens=lens).cpu().numpy()
             for k, i in enumerate(idx):
-                x[k, :items[i].shape[0]] = torch.from_numpy(items[i])
-            lens = torch.tensor([items[i].shape[0] for i in idx], dtype=torch.int32).to(dev)
-            y = eng.oracle(x.to(dev), lens=lens).cpu().numpy()
-            for k, i in enumerate(idx):
-                T = 1 + items[i].shape[0] // 441
+                T = 1 + (lengths[i] if convert else items[i].shape[0]) // 441
                 outs[i] = y[k:k + 1, :(T + T % 2 + 4) * 441].copy()
         return outs
+
+
+def _stage(items, rates, segs, dev):
+    """The device resampler's input for output ranges segs = [(recording, a, b), ...] of the 44.1 kHz streams: each
+    range's input window (resample.window), concatenated on the host and uploaded as one staging buffer, and the items
+    of Engine.resample."""
+    windows, table, off = [], [], 0
+    for i, a, b in segs:
+        n = items[i].shape[0]
+        first, stop = resample.window(n, rates[i], a, b)
+        windows.append(items[i][first:stop])
+        table.append((rates[i], n, off, first, stop - first, a, b - a))
+        off += stop - first
+    return torch.from_numpy(np.concatenate(windows)).to(dev), table
 
 
 def oracle_conditions(wav):
@@ -398,7 +431,7 @@ class VoiceFixer:
         return out.cpu().numpy()
 
     @torch.no_grad()
-    def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None):
+    def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None, sample_rate=44100):
         """Extension of the reference API: restores a list of 1-D recordings of any lengths, in any mode, and returns a
         list of (1, L_i') arrays, element i what restore_inmem(wavs[i], cuda=True, mode=mode) returns -- bit-identical in
         modes 0 and 1 and in mode 2 with drop_masks_fn=False; in mode 2 with dropout, the same distribution.
@@ -409,7 +442,14 @@ class VoiceFixer:
         drop_masks_fn (mode 2): None = Bernoulli(0.5) keep-masks from torch's CPU generator, as restore_inmem draws them;
         a callable (B, T_cap) -> uint8 (2, B, T_cap, 512) supplies them for each launch (item b of a batch reads
         [:, b, :T_b]); False = no dropout.  Bad input raises ValueError before anything is launched.  The vocoder hook of
-        restore_inmem (your_vocoder_func) runs per segment on the host and is not offered here."""
+        restore_inmem (your_vocoder_func) runs per segment on the host and is not offered here.
+
+        sample_rate: the recordings' rate in Hz, one positive int or one per recording (a bad one raises ValueError naming
+        the recording).  Recordings at another rate than 44100 are resampled on the device (vfx_resample): each segment
+        of the 44.1 kHz stream is computed from its own window of input samples, uploaded alone, straight into the
+        batch.  Element i is then bit-identical to restore_many on wavio._resample(wavs[i], rate_i, 44100), the host
+        resampler VoiceFixer.restore() reads files with; the plan is the same, so mode 2's default masks are drawn at the
+        same points.  A call in which every rate is 44100 launches nothing for it."""
         _check_cuda(cuda)
         items = []
         for i, w in enumerate(wavs):
@@ -417,6 +457,8 @@ class VoiceFixer:
             if a.ndim != 1:
                 raise ValueError(f"restore_many: recording {i} has shape {a.shape}; the list takes 1-D arrays")
             items.append(a)
+        rates = resample.rates(sample_rate, len(items), "restore_many")
+        convert = any(r != resample.RATE for r in rates)
         eng = self._engine
         dev = f"cuda:{eng.device}"
 
@@ -424,17 +466,22 @@ class VoiceFixer:
             extra = 0
             if mode == 1:     # the pre-filter's workspace and its (B, L_cap) output live alongside the restore
                 extra = eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
+            if convert:       # the staged input windows and the resampler's item table
+                extra += 4 * max(resample.staging_bound(L_cap, r) for r in set(rates)) + 64
             return eng.max_batch(L_cap, extra_per_item=extra)
 
-        plan = plan_many([a.shape[0] for a in items], mode, max_items)
+        plan = plan_many([resample.out_len(a.shape[0], r) for a, r in zip(items, rates)], mode, max_items)
         pieces = {}                                                      # (recording, start) -> restored segment
         for L_cap, segs in plan:
             B = len(segs)
-            x = torch.zeros((B, L_cap))
-            for k, (i, a, b) in enumerate(segs):
-                x[k, :b - a] = torch.from_numpy(items[i][a:b])
-            x = x.to(dev)
-            lens = torch.tensor([b - a for _, a, b in segs], dtype=torch.int32).to(dev)
+            if convert:
+                x, lens = eng.resample(*_stage(items, rates, segs, dev), L_cap)
+            else:
+                x = torch.zeros((B, L_cap))
+                for k, (i, a, b) in enumerate(segs):
+                    x[k, :b - a] = torch.from_numpy(items[i][a:b])
+                x = x.to(dev)
+                lens = torch.tensor([b - a for _, a, b in segs], dtype=torch.int32).to(dev)
             if mode == 1:
                 x, _, lens = eng.hf_cut(x, lens=lens)
                 out_lens = [512 * ((b - a) // 512) for _, a, b in segs]
@@ -451,8 +498,8 @@ class VoiceFixer:
             y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens).cpu().numpy()
             for k, (i, a, _) in enumerate(segs):
                 pieces[(i, a)] = y[k, :out_lens[k]]
-        return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(it.shape[0])])[None]
-                for i, it in enumerate(items)]
+        return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(resample.out_len(it.shape[0], r))])[None]
+                for i, (it, r) in enumerate(zip(items, rates))]
 
     # ------------------------------------------------------------------ batch entry point (extension)
     def pinned_empty(self, shape):

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvfx_b200.so")
 SOURCES = ["engine.cu", "conv_gemm_simt.cu", "conv_gemm_tc.cu", "resstack_pair.cu", "elementwise.cu", "frontend.cu",
-           "gru.cu", "hf_cut.cu", "oracle_fe.cu"]
+           "gru.cu", "hf_cut.cu", "oracle_fe.cu", "resample.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

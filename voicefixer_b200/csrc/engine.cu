@@ -774,6 +774,48 @@ int oracle_cond_forward(Ctx& c, const float* wav, int B, int L_cap, const int* l
                          peak, nullptr, nullptr, c.prec(), cond_out, c.st);
 }
 
+// vfx_resample: the item table is staged into the workspace, then one launch
+int resample_forward(Ctx& c, const float* x, const float* h, const vfx_resample_item* items_host, int B, int L_cap,
+                     float* y, int* lens_out) {
+  vfx_resample_item* items = c.ws->alloc<vfx_resample_item>(B);
+  if (c.dry) return VFX_OK;
+  VFX_CUDA_CHECK(cudaMemcpyAsync(items, items_host, sizeof(vfx_resample_item) * B, cudaMemcpyHostToDevice, c.st));
+  return resample(x, h, items, B, L_cap, y, lens_out, c.st);
+}
+
+// One item of vfx_resample against the buffers (include/vfx_b200.h): VFX_ERR_INVALID with a message naming item b.
+int check_resample_item(const vfx_resample_item& it, int b, long long x_elems, long long h_elems, int L_cap) {
+  VFX_REQUIRE(it.up >= 1 && it.down >= 1 && it.up <= (1 << 20), "resample: item %d: ratio %d/%d (up must lie in [1, 2^20], "
+              "down >= 1)", b, it.up, it.down);
+  VFX_REQUIRE(it.n_in >= 0 && it.n_in <= (1LL << 40), "resample: item %d: recording length %lld", b, it.n_in);
+  VFX_REQUIRE(it.x_off >= 0 && it.x_len >= 0 && it.x_off + it.x_len <= x_elems, "resample: item %d: window "
+              "x[%lld, %lld) is not inside the %lld staged samples", b, it.x_off, it.x_off + it.x_len, x_elems);
+  VFX_REQUIRE(it.x_first >= 0 && it.x_first + it.x_len <= it.n_in, "resample: item %d: window [%lld, %lld) is not inside "
+              "its recording of %lld samples", b, it.x_first, it.x_first + it.x_len, it.n_in);
+  const bool copy = it.up == 1 && it.down == 1;
+  if (!copy)
+    VFX_REQUIRE(it.h_off >= 0 && it.h_len >= 1 && it.h_off + it.h_len <= h_elems && it.rem >= 0, "resample: item %d: "
+                "taps h[%lld, %lld) (rem %d) are not inside the %lld given", b, it.h_off, it.h_off + it.h_len, it.rem,
+                h_elems);
+  const long long n_out = (it.n_in * it.up + it.down - 1) / it.down;
+  VFX_REQUIRE(it.y_len >= 0 && it.y_len <= L_cap, "resample: item %d: y_len %d is not in [0, L_cap = %d]", b, it.y_len,
+              L_cap);
+  VFX_REQUIRE(it.y_first >= 0 && it.y_first + it.y_len <= n_out, "resample: item %d: outputs [%lld, %lld) are not inside "
+              "the stream's %lld samples", b, it.y_first, it.y_first + it.y_len, n_out);
+  if (it.y_len == 0) return VFX_OK;
+  long long lo = it.y_first, hi = it.y_first + it.y_len - 1;           // the inputs the outputs read (a copy: the same)
+  if (!copy) {
+    const long long num = (it.y_first + it.rem) * it.down - it.h_len + 1;
+    lo = num <= 0 ? 0 : (num + it.up - 1) / it.up;
+    hi = std::min(it.n_in - 1, (hi + it.rem) * it.down / it.up);
+  }
+  if (lo <= hi)
+    VFX_REQUIRE(it.x_first <= lo && hi < it.x_first + it.x_len, "resample: item %d: outputs [%lld, %lld) read inputs "
+                "[%lld, %lld); the window holds [%lld, %lld)", b, it.y_first, it.y_first + it.y_len, lo, hi + 1, it.x_first,
+                it.x_first + it.x_len);
+  return VFX_OK;
+}
+
 // Vocoder.oracle's mel basis: librosa.filters.mel(sr=44100, n_fft=2048, n_mels=128, fmin=0, fmax=22050, htk=True) with
 // its default norm="slaney" (vocoder/model/util.py:115-123), built in float64 as librosa builds it and cast to float32
 // (wavio.slaney_htk_mel_basis is the same formula on the host).  band: start[128] ++ len[128] of each row's non-zeros.
@@ -1162,6 +1204,28 @@ int vfx_hf_cut_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const i
   VFX_REQUIRE(lens, "hf_cut_ragged: lens is null");
   return hf_cut(wav, B, L_cap, lens, ratio, e->d_window, e->d_tw, wav_out, lens_out, cut_bins, workspace,
                 workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t vfx_resample_workspace_bytes(int B) {
+  if (B <= 0) return 0;
+  int rc;
+  const size_t peak = dry_peak(nullptr, VFX_MODE_EVAL, [&](Ctx& c) {
+    return resample_forward(c, nullptr, nullptr, nullptr, B, 1, nullptr, nullptr);
+  }, &rc);
+  return rc == VFX_OK ? peak : 0;
+}
+
+int vfx_resample(vfx_engine* e, const float* x, long long x_elems, const float* h, long long h_elems,
+                 const vfx_resample_item* items_host, int B, float* y, int L_cap, int* lens_out,
+                 void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_REQUIRE(items_host && y && B > 0 && B <= 65535 && L_cap > 0 && workspace && x_elems >= 0 && h_elems >= 0,
+              "resample: bad arguments");
+  VFX_REQUIRE(x || x_elems == 0, "resample: x is null");
+  VFX_REQUIRE(h || h_elems == 0, "resample: h is null");
+  for (int b = 0; b < B; ++b) VFX_TRY(check_resample_item(items_host[b], b, x_elems, h_elems, L_cap));
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return resample_forward(c, x, h, items_host, B, L_cap, y, lens_out); });
 }
 
 int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream) {

@@ -167,5 +167,9 @@ int voc_post(const float* x, int B, int L, const float* w, const float* bias, in
 int hf_cut(const float* wav, int B, int L, const int* lens, float ratio, const float* window, const float2* tw,
            float* out, int* lens_out, int* cut_bins, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t hf_cut_workspace(int B, int L);
+// polyphase rate conversion (resample.cu): row b of y[B][L_cap] <- items[b]'s output samples (items: the device copy of
+// a table vfx_resample has validated), then zeros; lens_out[b] (optional) <- y_len
+int resample(const float* x, const float* h, const vfx_resample_item* items, int B, int L_cap, float* y, int* lens_out,
+             cudaStream_t st);
 
 }  // namespace vfx

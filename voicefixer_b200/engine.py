@@ -7,7 +7,7 @@ import os
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, resample
 from .weights import pack_analysis, pack_vocoder
 
 ALIGN = 256
@@ -327,6 +327,56 @@ class Engine(_WorkspaceQueries):
     def hf_cut_workspace_bytes(B, L):
         """Workspace of hf_cut() on B items of (at most) L samples (vfx_hf_cut_workspace_bytes; no engine needed)."""
         return int(_lib.load().vfx_hf_cut_workspace_bytes(int(B), int(L)))
+
+    @staticmethod
+    def resample_workspace_bytes(B):
+        """Workspace of resample() on B items (vfx_resample_workspace_bytes; no engine needed)."""
+        return int(_lib.load().vfx_resample_workspace_bytes(int(B)))
+
+    def _taps_for(self, rates):
+        """{(up, down): (offset, length)} of the rates' taps in the engine's device tap buffer, which holds every ratio
+        this engine has resampled so far; a new ratio re-uploads the buffer once."""
+        if not hasattr(self, "_taps_off"):
+            self._taps_off, self._taps_host, self._taps_dev = {}, [], None
+        fresh = False
+        for r in rates:
+            key = resample.ratio(r)
+            if key != (1, 1) and key not in self._taps_off:
+                h, _ = resample.taps(r)
+                self._taps_off[key] = (sum(len(t) for t in self._taps_host), len(h))
+                self._taps_host.append(h)
+                fresh = True
+        if fresh:
+            self._taps_dev = torch.from_numpy(np.concatenate(self._taps_host)).to(f"cuda:{self.device}")
+        return self._taps_off
+
+    def resample(self, x, items, L_cap):
+        """Rate conversion to 44.1 kHz on the device (vfx_resample), bit-identical to wavio._resample on the host.
+
+        x: 1-D float32 device tensor, the staged input windows.  items: one (rate, n_in, x_off, x_first, x_len, y_first,
+        y_len) per row: output samples [y_first, y_first + y_len) of a recording of n_in samples at `rate`, whose samples
+        [x_first, x_first + x_len) are x[x_off : x_off + x_len] (resample.window gives the window an output range needs).
+        Returns (y (B, L_cap) with row b's y_len samples then zeros, lens (B,) int32 device tensor of the y_len)."""
+        x = x.reshape(-1)
+        if not (x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
+            raise ValueError("x must be a contiguous float32 CUDA tensor")
+        B = len(items)
+        offs = self._taps_for([it[0] for it in items])
+        table = (_lib.ResampleItem * B)()
+        for b, (rate, n_in, x_off, x_first, x_len, y_first, y_len) in enumerate(items):
+            up, down = resample.ratio(rate)
+            h_off, h_len = offs.get((up, down), (0, 0))
+            t = table[b]
+            t.x_off, t.x_first, t.n_in, t.x_len = int(x_off), int(x_first), int(n_in), int(x_len)
+            t.y_first, t.y_len = int(y_first), int(y_len)
+            t.up, t.down, t.rem, t.h_off, t.h_len = up, down, resample.taps(rate)[1], h_off, h_len
+        h = self._taps_dev
+        y = torch.empty(B, int(L_cap), device=x.device)
+        lens = torch.empty(B, dtype=torch.int32, device=x.device)
+        ws = self._workspace(self.resample_workspace_bytes(B))
+        _lib.check(self.lib.vfx_resample(self.h, _ptr(x), x.numel(), _ptr(h), 0 if h is None else h.numel(), table, B,
+                                         _ptr(y), int(L_cap), _ptr(lens), _ptr(ws), ws.numel(), _stream()), "vfx_resample")
+        return y, lens
 
     def hf_cut(self, wav, ratio=0.95, lens=None):
         """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
