@@ -375,10 +375,11 @@ def slaney_htk_mel_basis():
 def oracle_cond(wav):
     """Vocoder.oracle front end vocoder/base.py:61-73: peak-normalise, |librosa.stft|
     (n_fft 2048, hop 441, hann, center, pad_mode='constant' per librosa 0.10.1), Slaney mel,
-    dB-20, normalise, pre() -> cond (1,128,T+T%2+4)."""
+    dB-20, normalise, pre() -> cond (1,128,T+T%2+4).  librosa's stft multiplies the float32 frames by
+    get_window's float64 window without a cast: the windowed frames are float64."""
     wav = np.asarray(wav, dtype=np.float32)
     wav = wav / np.max(np.abs(wav))
-    win = (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(N_FFT) / N_FFT)).astype(np.float32)
+    win = 0.5 - 0.5 * np.cos(2 * np.pi * np.arange(N_FFT) / N_FFT)
     x = np.pad(wav, (N_FFT // 2, N_FFT // 2), mode="constant")
     nfr = 1 + (len(x) - N_FFT) // HOP
     idx = np.arange(N_FFT)[None, :] + HOP * np.arange(nfr)[:, None]

@@ -143,7 +143,7 @@ def test_hf_cut_mode1_prefilter_vs_oracle(engine):
     for b in range(2):
         ref = O.remove_higher_frequency(wav[b])
         assert out.shape[1] == ref.shape[0] == 512 * (wav.shape[1] // 512)
-        assert rel_rms(out[b].cpu().numpy(), ref) < 1e-4
+        assert rel_rms(out[b].cpu().numpy(), ref) < 5e-7       # measured 1.4e-7 on an H100 (700 W)
     assert all(0 < int(c) < 1025 for c in cut.cpu())
 
 

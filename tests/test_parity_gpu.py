@@ -361,10 +361,9 @@ def test_api_modes_1_2_and_vocoder_oracle(tmp_path, monkeypatch, states):
     out1 = vf.restore_inmem(wav, cuda=True, mode=1)                         # mode 1: pre-filter, shorter output
     ref1 = O.restore_inmem(wav, states[0], states[1], mode=1)
     assert out1.shape == ref1.shape == (1, 512 * (wav.shape[0] // 512))
-    # mode 1 tolerance 1e-3: the fp32 rFFT -> irFFT round trip of the pre-filter differs from numpy's by ~4e-5 on a
-    # noisy input (cut bins identical), which the network amplifies ~6x; with the oracle's filtered input the
-    # restore matches to 4e-6
-    assert rel_rms(out1, ref1) < 1e-3
+    # mode 1: measured 3.7e-6 on an H100 (700 W).  The pre-filter agrees with the oracle's to 1.4e-7; when its
+    # overlap-add left frame 0 out of samples 513..1023 this was 2.6e-4.
+    assert rel_rms(out1, ref1) < 2e-5
     # mode 2 (train-mode BN, no dropout masks): <= 64 frames is an error in the reference too (1x1 UNet centre)
     with pytest.raises(ValueError, match="more than 1 value per channel"):
         vf.restore_inmem(wav, cuda=True, mode=2)

@@ -298,11 +298,12 @@ def _stage(items, rates, segs, dev):
 def oracle_conditions(wav):
     """Host front end of Vocoder.oracle (vocoder/base.py:61-73; numpy in the reference too):
     peak-normalise, |STFT| (2048/441/Hann/center, librosa-0.10 zero padding), Slaney-normalised
-    HTK mel (librosa.filters.mel defaults), dB - 20, normalise, pad -> (1, Tc, 128) channels-last."""
+    HTK mel (librosa.filters.mel defaults), dB - 20, normalise, pad -> (1, Tc, 128) channels-last.  The window is
+    float64, as librosa's get_window returns it, so the windowed frames are float64 like librosa.stft's."""
     wav = np.asarray(wav, dtype=np.float32)
     wav = wav / np.max(np.abs(wav))
     n_fft, hop = 2048, 441
-    win = (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(n_fft) / n_fft)).astype(np.float32)
+    win = 0.5 - 0.5 * np.cos(2 * np.pi * np.arange(n_fft) / n_fft)
     x = np.pad(wav, (n_fft // 2, n_fft // 2), mode="constant")
     nfr = 1 + (len(x) - n_fft) // hop
     idx = np.arange(n_fft)[None, :] + hop * np.arange(nfr)[:, None]

@@ -758,7 +758,7 @@ int oracle_forward(Ctx& c, const float* wav, int B, int L_cap, const int* lens, 
   int* ext = c.ws->alloc<int>((size_t)EXT_LEVELS * B);
   void* cond = c.ws->raw((size_t)B * Tc * 128 * c.e->esz());
   if (!c.dry) {
-    VFX_TRY(oracle_frontend(wav, B, L_cap, lens, c.e->d_window, c.e->d_obasis, c.e->d_oband,
+    VFX_TRY(oracle_frontend(wav, B, L_cap, lens, c.e->d_obasis, c.e->d_oband,
                             c.e->d_oband + 128, peak, lens ? frames : nullptr, cond, c.prec(), nullptr, c.st));
     if (lens) VFX_TRY(frame_extents(frames, B, T, ext, c.st));
   }
@@ -770,7 +770,7 @@ int oracle_forward(Ctx& c, const float* wav, int B, int L_cap, const int* lens, 
 int oracle_cond_forward(Ctx& c, const float* wav, int B, int L_cap, const int* lens, float* cond_out) {
   unsigned int* peak = c.ws->alloc<unsigned int>(B);
   if (c.dry) return VFX_OK;
-  return oracle_frontend(wav, B, L_cap, lens, c.e->d_window, c.e->d_obasis, c.e->d_oband, c.e->d_oband + 128,
+  return oracle_frontend(wav, B, L_cap, lens, c.e->d_obasis, c.e->d_oband, c.e->d_oband + 128,
                          peak, nullptr, nullptr, c.prec(), cond_out, c.st);
 }
 

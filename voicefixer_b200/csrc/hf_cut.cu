@@ -123,7 +123,7 @@ __global__ void hf_ola_kernel(const float* __restrict__ frames, int nfr, int out
   if (n >= HOP * (nfr_b - 1)) { out[(long long)b * out_len + n] = 0.f; return; }
   const int p = n + NF / 2;                      // position in the un-trimmed overlap-add buffer
   const int t_hi = min(p / HOP, nfr_b - 1);
-  const int t_lo = max(0, (p - NF) / HOP + 1);
+  const int t_lo = p >= NF ? (p - NF) / HOP + 1 : 0;   // first frame with p - t * HOP < NF (floor, not truncation)
   float acc = 0.f, wss = 0.f;
   for (int t = t_lo; t <= t_hi; ++t) {
     const int j = p - t * HOP;

@@ -33,16 +33,17 @@ __global__ void __launch_bounds__(256) oracle_peak_kernel(const float* __restric
 }
 
 // One block per (conditioning row t, item b).  Row t < T_b is STFT frame t: samples t * 441 - 1024 + n, zero outside
-// [0, L_b), each divided by the item's peak (IEEE division, numpy's float32 wav / max), windowed, packed into a 1024-point
-// complex FFT in double (numpy's rfft computes in float64; a float32 transform of a pure tone is off by up to 1e-3 in the
-// normalised output, where the tone's packed mirror bin cancels) and untangled; rounded to complex64 and |X| in float32
+// [0, L_b), each divided by the item's peak (IEEE division, numpy's float32 wav / max), times the periodic Hann in double
+// (librosa's stft takes a float64 window from get_window and multiplies the float32 frames by it without a cast; a
+// float32 window product moves a full-scale tone's output by up to 1e-3), packed into a 1024-point complex FFT in double
+// (numpy's rfft computes in float64; a float32 transform of a pure tone is off by up to 1e-3 in the normalised output,
+// where the tone's packed mirror bin cancels) and untangled; rounded to complex64 and |X| in float32
 // without a clamp (np.abs), the banded mel basis, and the dB / normalise epilogue in double as numpy evaluates it (the
 // float64 min_level promotes it), rounded to fp32 and then to the operand format.
 template <typename T>
 __global__ void __launch_bounds__(256) oracle_mel_kernel(const float* __restrict__ wav, int L_cap, int Tc_cap,
                                                          const int* __restrict__ lens,
                                                          const unsigned int* __restrict__ peak_bits,
-                                                         const float* __restrict__ window,
                                                          const float* __restrict__ basis, const int* __restrict__ b_start,
                                                          const int* __restrict__ b_len, T* __restrict__ cond_op,
                                                          float* __restrict__ cond_f32) {
@@ -67,12 +68,12 @@ __global__ void __launch_bounds__(256) oracle_mel_kernel(const float* __restrict
     tw[k] = make_double2(c, s);
   }
   for (int n = tid; n < 1024; n += 256) {
-    float v[2];
+    double v[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int i = base + 2 * n + h;
+      const int j = 2 * n + h, i = base + j;
       const float s = (i >= 0 && i < Lb) ? __fdiv_rn(x[i], peak) : 0.0f;
-      v[h] = __fmul_rn(s, window[2 * n + h]);
+      v[h] = (double)s * (0.5 - 0.5 * cospi(j / 1024.0));      // 0.5 - 0.5 cos(2 pi j / 2048)
     }
     bufA[n] = make_double2(v[0], v[1]);
   }
@@ -101,9 +102,8 @@ __global__ void __launch_bounds__(256) oracle_mel_kernel(const float* __restrict
 
 }  // namespace
 
-int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const float* window,
-                    const float* basis, const int* b_start, const int* b_len, unsigned int* peak_bits, int* frames,
-                    void* cond_op, int precision, float* cond_f32, cudaStream_t st) {
+int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const float* basis, const int* b_start,
+                    const int* b_len, unsigned int* peak_bits, int* frames, void* cond_op, int precision, float* cond_f32, cudaStream_t st) {
   VFX_REQUIRE(wav && B > 0 && L_cap > 0 && peak_bits && (cond_op || cond_f32), "oracle_frontend: bad arguments");
   const int T = 1 + L_cap / 441, Tc = T + T % 2 + 4;
   VFX_CUDA_CHECK(cudaMemsetAsync(peak_bits, 0, sizeof(unsigned int) * B, st));
@@ -112,7 +112,7 @@ int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const f
   VFX_LAUNCH_CHECK();
   dim3 grid(Tc, B);
 #define VFX_ORACLE_LAUNCH(TY)                                                                                     \
-  oracle_mel_kernel<TY><<<grid, 256, 0, st>>>(wav, L_cap, Tc, lens, peak_bits, window, basis, b_start, b_len, \
+  oracle_mel_kernel<TY><<<grid, 256, 0, st>>>(wav, L_cap, Tc, lens, peak_bits, basis, b_start, b_len, \
                                               reinterpret_cast<TY*>(cond_op), cond_f32)
   if (cond_op && precision == VFX_PREC_BF16) VFX_ORACLE_LAUNCH(__nv_bfloat16);
   else if (cond_op && precision == VFX_PREC_FP16) VFX_ORACLE_LAUNCH(__half);

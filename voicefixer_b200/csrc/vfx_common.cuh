@@ -133,9 +133,9 @@ int frame_extents(const int* frames, int B, int T_cap, int* ext, cudaStream_t st
 // Writes the normalised conditions [B][Tc_cap][128] in the operand format `precision` to cond_op and / or in fp32 to
 // cond_f32 (either may be NULL): rows T_b .. Tc_b - 1 are -4; rows from Tc_b on are -4 in cond_op and 0 in cond_f32.
 // basis / b_start / b_len: the Slaney HTK mel basis [128][1025] fp32 and its band of non-zero bins per row.
-int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const float* window,
-                    const float* basis, const int* b_start, const int* b_len, unsigned int* peak_bits, int* frames,
-                    void* cond_op, int precision, float* cond_f32, cudaStream_t st);
+int oracle_frontend(const float* wav, int B, int L_cap, const int* lens, const float* basis, const int* b_start,
+                    const int* b_len, unsigned int* peak_bits, int* frames, void* cond_op, int precision, float* cond_f32,
+                    cudaStream_t st);
 int stft_mel(const float* wav, int B, int L, int T, const int* ext_len, const int* ext_frames, const float* window,
              const float2* tw, const float* fbT, const int* fb_start, const int* fb_len, float* mel, float* sp,
              cudaStream_t st);
