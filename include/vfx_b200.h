@@ -312,6 +312,55 @@ int vfx_gru_layer(const float* gi, const float* whh_t, const float* bhh, int B, 
 int vfx_gru_layer_ragged(const float* gi, const float* whh_t, const float* bhh, int B, int T, const int* lens,
                          float* out, void* stream);
 
+/* The element-wise, batch-statistics and waveform-output kernels (elementwise.cu), each as the engine launches it.  A bad
+ * call (null pointer, non-positive size, misaligned vector access, B beyond a grid dimension) returns VFX_ERR_INVALID
+ * before any launch.  Per-item tables (seq, ext_*, lens, frames) are device int32 [B]; NULL = every item spans the tensor. */
+/* Train-mode BatchNorm statistics, F.batch_norm(training=True) (restorer/modules.py:70, restorer/model.py:69-99): x fp32
+ * [B][P][C] (pitch ldx) -> scale / shift [B][bn_C] = gamma / sqrt(var + 1e-5), beta - mean * scale; bn_C = 1 pools all
+ * P x C values, bn_C = C is per channel; acc: caller scratch of 16 * B * bn_C bytes; seq: item b covers its first
+ * min(seq[b] * per_row, P) positions.  B <= 65535. */
+int vfx_bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, int C, int bn_C, const float* gamma,
+                 const float* beta, float* scale, float* shift, double* acc, const int* seq, int per_row, void* stream);
+/* y = act(x * scale + shift) in the operand format, F.leaky_relu_(bn(x)) (restorer/modules.py:70-71); scale / shift
+ * [b * stat_sB + (bn_C == 1 ? 0 : c)], NULL = 1 / 0; columns >= C of y are not written. */
+int vfx_bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, long long P, int C,
+               const float* scale, const float* shift, int bn_C, int stat_sB, int act, float act_param, void* y,
+               long long y_sB, long long ldy, void* stream);
+/* nn.Dropout(0.5) in train mode (restorer/model.py:75,94) in place: x[i] = keep[i] ? 2 x[i] : 0. */
+int vfx_dropout_apply(float* x, const uint8_t* keep, long long n, void* stream);
+/* F.avg_pool2d(x, (2, 2)) (restorer/modules.py:103): x [B][H][W][C] (element strides, multiples of 4; x and y 16-byte
+ * aligned, C % 4 == 0) -> dense y [B][H/2][W/2][C]. */
+int vfx_avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W, int C, float* y,
+                   void* stream);
+/* Generator.forward's mask and to_log (restorer/model.py:105-109) + the UNet input pad (restorer/model_kqq_bn.py:144-151):
+ * xlog[B][T][128] = log10(max(sigmoid(lin) mel, 1e-8)); unet_in[B][Tp][127][2] = (log10(max(mel, 1e-8)), xlog) for
+ * t < T_b = ext_frames[b], zeros for T_b <= t < Tp. */
+int vfx_mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, const int* ext_frames, float* xlog,
+                      float* unet_in, void* stream);
+/* after_conv2 (1x1, 32 -> 1) + F.pad + crop + residual (restorer/model_kqq_bn.py:174-178, restorer/model.py:113):
+ * out[B][T][128] = (f < 127 ? bias + sum_c w[c] x[b][t][f][c] : 0) + xlog; x [B][Tp][127][32], 16-byte aligned. */
+int vfx_unet_head(const float* x, int B, int T, int Tp, const float* w, const float* bias, const float* xlog, float* out,
+                  void* stream);
+/* Vocoder.forward's conditions (vocoder/base.py:51-54, vocoder/model/util.py:8-36,69-80): from_log (input_is_log),
+ * / mel_weight, dB, normalise and clip to [-4, 4], pre()'s -4 tail: mel [B][T][128] -> cond [B][Tc][128] in the operand
+ * format; tab = mel_weight[128] ++ [min_level]. */
+int vfx_voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames, int input_is_log, const float* tab,
+                      void* cond, int precision, void* stream);
+/* nn.ReflectionPad1d(3) (vocoder/model/generator.py:74,94) in place on buf [B][L + 6][C]: rows 0..2 and L_b + 3..L_b + 5
+ * from the interior rows 3..L_b + 2 (L_b = ext_len[b], else L >= 4); 2-byte elements in bf16 / fp16, 4 otherwise. */
+int vfx_reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precision, void* stream);
+/* generator[14..17] + _trim_center (vocoder/model/generator.py:93-99, base.py:63-76): x [B][L][64] fp32, w [7][64],
+ * out[B][out_len] = tanh(conv1d(reflect_pad3(lrelu_0.2(x)), w) + bias)[lo + j] * scale; ext_gen / ext_len (both or
+ * neither): item b has S_b = ext_gen[b] rows, lo_b = (S_b - L_b) / 2, L_b = ext_len[b], zeros from L_b on.  B <= 65535. */
+int vfx_voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len, const int* ext_gen,
+                 const int* ext_len, float scale, float* out, void* stream);
+/* fp32 -> the operand format (bf16 / fp16 round to nearest even, tf32 ties away from zero) over n elements. */
+int vfx_cast_rows(const float* x, long long n, void* y, int precision, void* stream);
+/* The per-item extent table of a ragged restore (DESIGN.md §3): lens[B] clamped into [1025, L_cap] -> ext[15][B]. */
+int vfx_ragged_extents(const int* lens, int B, int L_cap, int* ext, void* stream);
+/* The same table for the vocoder alone (DESIGN.md §3): frames[B] clamped into [1, T_cap] -> ext[15][B]. */
+int vfx_frame_extents(const int* frames, int B, int T_cap, int* ext, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

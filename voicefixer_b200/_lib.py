@@ -82,6 +82,18 @@ SIGNATURES = {
     "vfx_oracle_workspace_bytes": (_sz, [_vp, _i, _i]),
     "vfx_resample": (_i, [_vp, _vp, _ll, _vp, _ll, _c.POINTER(ResampleItem), _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "vfx_resample_workspace_bytes": (_sz, [_i]),
+    "vfx_bn_stats": (_i, [_vp, _ll, _ll, _i, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    "vfx_bn_act": (_i, [_i, _vp, _ll, _ll, _i, _ll, _i, _vp, _vp, _i, _i, _i, _f, _vp, _ll, _ll, _vp]),
+    "vfx_dropout_apply": (_i, [_vp, _vp, _ll, _vp]),
+    "vfx_avgpool2x2": (_i, [_vp, _ll, _ll, _ll, _i, _i, _i, _i, _vp, _vp]),
+    "vfx_mask_log_pack": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "vfx_unet_head": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "vfx_voc_normalize": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i, _vp]),
+    "vfx_reflect_pad3": (_i, [_vp, _i, _i, _i, _vp, _i, _vp]),
+    "vfx_voc_post": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _f, _vp, _vp]),
+    "vfx_cast_rows": (_i, [_vp, _ll, _vp, _i, _vp]),
+    "vfx_ragged_extents": (_i, [_vp, _i, _i, _vp, _vp]),
+    "vfx_frame_extents": (_i, [_vp, _i, _i, _vp, _vp]),
 }
 
 _lib = None

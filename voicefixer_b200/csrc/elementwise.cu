@@ -380,11 +380,22 @@ inline int grid_for(long long total, int block = 256) {
   return (int)g;
 }
 
+inline bool valid_prec(int precision) { return precision >= VFX_PREC_FP32 && precision <= VFX_PREC_FP16; }
+inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
 }  // namespace
+
+// The launchers refuse a bad call before any launch: they also serve the C ABI's per-kernel test entry points, whose
+// arguments come from outside the library.
 
 int bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, long long P, int C,
            const float* scale, const float* shift, int bn_C, int stat_sB, int act, float act_param,
            void* y, long long y_sB, long long ldy, cudaStream_t st) {
+  VFX_REQUIRE(x && y && B > 0 && P > 0 && C > 0 && ldx >= C && ldy >= C && x_sB >= 0 && y_sB >= 0,
+              "bn_act: bad arguments (B %d, P %lld, C %d, ldx %lld, ldy %lld)", B, P, C, ldx, ldy);
+  VFX_REQUIRE((bn_C == 1 || bn_C == C) && stat_sB >= 0 && valid_prec(precision),
+              "bn_act: bad statistics layout or precision (bn_C %d, C %d, stat_sB %d, precision %d)", bn_C, C, stat_sB,
+              precision);
   const bool vec = (C % 4 == 0) && (ldx % 4 == 0) && (x_sB % 4 == 0) && ((uintptr_t)x % 16 == 0);
   const long long total = (long long)B * P * (vec ? C / 4 : C);
   const int g = grid_for(total);
@@ -408,6 +419,10 @@ int bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, 
 int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, int C, int bn_C,
              const float* gamma, const float* beta, float* scale, float* shift, double* acc,
              const int* seq, int per_row, cudaStream_t st) {
+  VFX_REQUIRE(x && gamma && beta && scale && shift && acc, "bn_stats: null pointer");
+  VFX_REQUIRE(B > 0 && B <= 65535 && P > 0 && C > 0 && ldx >= C && x_sB >= 0 && (bn_C == 1 || bn_C == C),
+              "bn_stats: bad shape (B %d, P %lld, C %d, bn_C %d, ldx %lld; B <= 65535)", B, P, C, bn_C, ldx);
+  VFX_REQUIRE(!seq || per_row > 0, "bn_stats: per_row %d must be positive with seq", per_row);
   VFX_CUDA_CHECK(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * B * bn_C, st));
   const long long rows_per_block = 256;
   dim3 grid(ceil_div(P, rows_per_block), ceil_div(C, 32), B), block(32, 8);
@@ -420,6 +435,7 @@ int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, 
 }
 
 int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st) {
+  VFX_REQUIRE(x && keep && n > 0, "dropout_apply: bad arguments (n %lld)", n);
   dropout_kernel<<<grid_for(n), 256, 0, st>>>(x, keep, n);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
@@ -427,6 +443,8 @@ int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st) {
 
 int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W,
                int C, float* y, cudaStream_t st) {
+  VFX_REQUIRE(x && y && B > 0 && H > 0 && W > 0 && C > 0, "avgpool: bad arguments (B %d, H %d, W %d, C %d)", B, H, W, C);
+  VFX_REQUIRE(aligned16(x) && aligned16(y), "avgpool: x and y must be 16-byte aligned");
   VFX_REQUIRE(C % 4 == 0 && x_sW % 4 == 0 && x_sH % 4 == 0 && x_sB % 4 == 0, "avgpool: C/strides must be multiples of 4");
   const int Ho = H / 2, Wo = W / 2;
   avgpool_kernel<<<grid_for((long long)B * Ho * Wo * C / 4), 256, 0, st>>>(x, x_sB, x_sH, x_sW, B, Ho, Wo, C, y);
@@ -436,6 +454,9 @@ int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, i
 
 int mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, const int* ext_frames, float* xlog,
                   float* unet_in, cudaStream_t st) {
+  VFX_REQUIRE(lin && mel && xlog && unet_in && B > 0 && T > 0 && Tp >= T,
+              "mask_log_pack: bad arguments (B %d, T %d, Tp %d)", B, T, Tp);
+  VFX_REQUIRE(((uintptr_t)unet_in & 7) == 0, "mask_log_pack: unet_in must be 8-byte aligned");
   mask_log_pack_kernel<<<grid_for((long long)B * Tp * 128), 256, 0, st>>>(lin, mel, B, T, Tp, ext_frames, xlog, unet_in);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
@@ -443,6 +464,9 @@ int mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, cons
 
 int unet_head(const float* x, int B, int T, int Tp, const float* w, const float* bias,
               const float* xlog, float* out, cudaStream_t st) {
+  VFX_REQUIRE(x && w && bias && xlog && out && B > 0 && T > 0 && Tp >= T,
+              "unet_head: bad arguments (B %d, T %d, Tp %d)", B, T, Tp);
+  VFX_REQUIRE(aligned16(x), "unet_head: x must be 16-byte aligned");
   unet_head_kernel<<<grid_for((long long)B * T * 128), 256, 0, st>>>(x, B, T, Tp, w, bias, xlog, out);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
@@ -450,6 +474,8 @@ int unet_head(const float* x, int B, int T, int Tp, const float* w, const float*
 
 int voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames, int input_is_log, const float* tab,
                   void* cond, int precision, cudaStream_t st) {
+  VFX_REQUIRE(mel && tab && cond && B > 0 && T > 0 && Tc > 0 && valid_prec(precision),
+              "voc_normalize: bad arguments (B %d, T %d, Tc %d, precision %d)", B, T, Tc, precision);
   const int g = grid_for((long long)B * Tc * 128);
   if (precision == VFX_PREC_BF16)
     voc_normalize_kernel<__nv_bfloat16><<<g, 256, 0, st>>>(mel, B, T, Tc, ext_frames, input_is_log, tab,
@@ -480,6 +506,7 @@ int frame_extents(const int* frames, int B, int T_cap, int* ext, cudaStream_t st
 }
 
 int cast_rows(const float* x, long long n, void* y, int precision, cudaStream_t st) {
+  VFX_REQUIRE(x && y && n > 0 && valid_prec(precision), "cast_rows: bad arguments (n %lld, precision %d)", n, precision);
   if (precision == VFX_PREC_BF16)
     cast_kernel<__nv_bfloat16><<<grid_for(n), 256, 0, st>>>(x, n, reinterpret_cast<__nv_bfloat16*>(y));
   else if (precision == VFX_PREC_FP16)
@@ -493,6 +520,8 @@ int cast_rows(const float* x, long long n, void* y, int precision, cudaStream_t 
 }
 
 int reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precision, cudaStream_t st) {
+  VFX_REQUIRE(buf && B > 0 && C > 0 && valid_prec(precision), "reflect_pad3: bad arguments (B %d, C %d, precision %d)",
+              B, C, precision);
   VFX_REQUIRE(L >= 4, "reflect_pad3: length %d too short for reflection pad 3", L);
   const int g = grid_for((long long)B * 6 * C);
   if (precision == VFX_PREC_BF16 || precision == VFX_PREC_FP16)      // a 2-byte copy either way
@@ -505,6 +534,11 @@ int reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precisi
 
 int voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len,
              const int* ext_gen, const int* ext_len, float scale, float* out, cudaStream_t st) {
+  VFX_REQUIRE(x && w && bias && out && B > 0 && B <= 65535 && L > 0 && out_len > 0,
+              "voc_post: bad arguments (B %d, L %d, out_len %d; B <= 65535)", B, L, out_len);
+  VFX_REQUIRE(!ext_gen == !ext_len, "voc_post: ext_gen and ext_len go together");
+  VFX_REQUIRE(ext_gen || (lo >= 0 && (long long)lo + out_len <= L),
+              "voc_post: trim [%d, %lld) outside the generated length %d", lo, (long long)lo + out_len, L);
   VFX_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0, "voc_post: x and w must be 16-byte aligned");
   dim3 grid(ceil_div(out_len, POST_RUN * POST_GROUPS), B);
   voc_post_kernel<<<grid, 16 * POST_GROUPS, 0, st>>>(x, L, w, bias, lo, out_len, ext_gen, ext_len, scale, out);

@@ -1259,4 +1259,61 @@ int vfx_gru_layer_ragged(const float* gi, const float* whh_t, const float* bhh, 
   return gru_layer(gi, whh_t, bhh, B, T, lens, out, (cudaStream_t)stream);
 }
 
+int vfx_bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, int C, int bn_C, const float* gamma,
+                 const float* beta, float* scale, float* shift, double* acc, const int* seq, int per_row, void* stream) {
+  return bn_stats(x, x_sB, ldx, B, P, C, bn_C, gamma, beta, scale, shift, acc, seq, per_row, (cudaStream_t)stream);
+}
+
+int vfx_bn_act(int precision, const float* x, long long x_sB, long long ldx, int B, long long P, int C,
+               const float* scale, const float* shift, int bn_C, int stat_sB, int act, float act_param, void* y,
+               long long y_sB, long long ldy, void* stream) {
+  return bn_act(precision, x, x_sB, ldx, B, P, C, scale, shift, bn_C, stat_sB, act, act_param, y, y_sB, ldy,
+                (cudaStream_t)stream);
+}
+
+int vfx_dropout_apply(float* x, const uint8_t* keep, long long n, void* stream) {
+  return dropout_apply(x, keep, n, (cudaStream_t)stream);
+}
+
+int vfx_avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W, int C, float* y,
+                   void* stream) {
+  return avgpool2x2(x, x_sB, x_sH, x_sW, B, H, W, C, y, (cudaStream_t)stream);
+}
+
+int vfx_mask_log_pack(const float* lin, const float* mel, int B, int T, int Tp, const int* ext_frames, float* xlog,
+                      float* unet_in, void* stream) {
+  return mask_log_pack(lin, mel, B, T, Tp, ext_frames, xlog, unet_in, (cudaStream_t)stream);
+}
+
+int vfx_unet_head(const float* x, int B, int T, int Tp, const float* w, const float* bias, const float* xlog, float* out,
+                  void* stream) {
+  return unet_head(x, B, T, Tp, w, bias, xlog, out, (cudaStream_t)stream);
+}
+
+int vfx_voc_normalize(const float* mel, int B, int T, int Tc, const int* ext_frames, int input_is_log, const float* tab,
+                      void* cond, int precision, void* stream) {
+  return voc_normalize(mel, B, T, Tc, ext_frames, input_is_log, tab, cond, precision, (cudaStream_t)stream);
+}
+
+int vfx_reflect_pad3(void* buf, int B, int L, int C, const int* ext_len, int precision, void* stream) {
+  return reflect_pad3(buf, B, L, C, ext_len, precision, (cudaStream_t)stream);
+}
+
+int vfx_voc_post(const float* x, int B, int L, const float* w, const float* bias, int lo, int out_len, const int* ext_gen,
+                 const int* ext_len, float scale, float* out, void* stream) {
+  return voc_post(x, B, L, w, bias, lo, out_len, ext_gen, ext_len, scale, out, (cudaStream_t)stream);
+}
+
+int vfx_cast_rows(const float* x, long long n, void* y, int precision, void* stream) {
+  return cast_rows(x, n, y, precision, (cudaStream_t)stream);
+}
+
+int vfx_ragged_extents(const int* lens, int B, int L_cap, int* ext, void* stream) {
+  return ragged_extents(lens, B, L_cap, ext, (cudaStream_t)stream);
+}
+
+int vfx_frame_extents(const int* frames, int B, int T_cap, int* ext, void* stream) {
+  return frame_extents(frames, B, T_cap, ext, (cudaStream_t)stream);
+}
+
 }  // extern "C"
