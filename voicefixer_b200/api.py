@@ -65,19 +65,37 @@ _MODE2_MSG = ("Expected more than 1 value per channel when training, got input s
 def segment_bounds(n):
     """[(start, stop)] of the 30 s segments restore_inmem cuts a recording of n samples into (voicefixer/base.py:117-119):
     full segments, then the rest; a recording of a whole number of segments has no empty tail."""
-    out = []
-    bp = SEG_LENGTH
-    while bp < n + SEG_LENGTH:
-        out.append((bp - SEG_LENGTH, min(bp, n)))
-        bp += SEG_LENGTH
-    return out
+    return [(a, min(a + SEG_LENGTH, n)) for a in range(0, n, SEG_LENGTH)]
+
+
+def _net_len(L, mode):
+    """Samples a segment of L samples has after the mode-1 pre-filter (512 * (L // 512)); L in the other modes."""
+    return 512 * (L // 512) if mode == 1 else L
+
+
+def _gen_len(T):
+    """Samples the Generator writes for a mel of T frames."""
+    return (T + T % 2 + 4) * 441
+
+
+def _pack(lengths, max_items):
+    """Packs items of the given lengths into ragged batches [(cap, [index, ...]), ...]: longest first (stable on ties), each
+    batch the longest item left, cap being its length, plus up to max_items(cap) - 1 of the next ones (so at least one).
+    max_items is called once per batch, in batch order."""
+    order = sorted(range(len(lengths)), key=lambda i: -lengths[i])
+    batches, k = [], 0
+    while k < len(order):
+        cap = lengths[order[k]]
+        n = max(1, int(max_items(cap)))
+        batches.append((cap, order[k:k + n]))
+        k += n
+    return batches
 
 
 def plan_many(lengths, mode, max_items):
     """Segments the recordings of the given lengths exactly as restore_inmem does and packs all their segments into ragged
-    batches (VoiceFixer.restore_many).  Segments are ordered by length, longest first, and each batch takes the longest
-    segment left plus up to max_items(L_cap) - 1 of the next ones, L_cap being that first segment's length (the batch's
-    capacity).  Returns [(L_cap, [(recording, start, stop), ...]), ...].
+    batches by length with _pack (VoiceFixer.restore_many), L_cap being a batch's longest segment (its capacity).
+    Returns [(L_cap, [(recording, start, stop), ...]), ...].
 
     Raises ValueError, naming the recording, before anything runs: for an empty list, a segment of 1024 samples or fewer
     (after the mode-1 pre-filter's 512 * (L // 512) in mode 1: the front end reflect-pads 1024), or in mode 2 a segment of
@@ -93,7 +111,7 @@ def plan_many(lengths, mode, max_items):
             raise ValueError(f"restore_many: recording {i} is empty")
         for a, b in bounds:
             L = b - a
-            Lnet = 512 * (L // 512) if mode == 1 else L
+            Lnet = _net_len(L, mode)
             if mode == 2 and 1 + Lnet // 441 <= 64:
                 raise ValueError(f"restore_many: recording {i}, samples {a}..{b}: {_MODE2_MSG}")
             if Lnet <= 1024:
@@ -101,23 +119,15 @@ def plan_many(lengths, mode, max_items):
                 raise ValueError(f"restore_many: recording {i} has a segment (samples {a}..{b}) of {what}; the front end "
                                  "reflect-pads 1024, so every segment needs at least 1025")
             segs.append((i, a, b))
-    segs.sort(key=lambda s: s[1] - s[2])             # longest first; stable, so equal lengths keep their order
-    batches, k = [], 0
-    while k < len(segs):
-        L_cap = segs[k][2] - segs[k][1]
-        n = max(1, int(max_items(L_cap)))
-        batches.append((L_cap, segs[k:k + n]))
-        k += n
-    return batches
+    return [(L_cap, [segs[j] for j in idx]) for L_cap, idx in _pack([b - a for _, a, b in segs], max_items)]
 
 
 def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
     """Packs the items of Vocoder.forward_many (kind "mel": [1, 1, T, 128] mels) or Vocoder.oracle_many (kind "wav": 1-D
-    float32 recordings) into ragged batches.  Items are ordered by length, longest first (stable, so equal lengths keep
-    their order), and each batch takes the longest item left plus up to max_items(cap) - 1 of the next ones, cap being
-    that first item's length in frames (mels) or samples (recordings): the batch's capacity.  Returns
-    [(cap, [item, ...]), ...].  pack_lengths (optional): the lengths to pack by in place of the items' own, e.g. recordings'
-    lengths at 44.1 kHz when they are resampled on the device; the items are validated all the same.
+    float32 recordings) into ragged batches by length with _pack, cap being a batch's longest item in frames (mels) or
+    samples (recordings): its capacity.  Returns [(cap, [item, ...]), ...].  pack_lengths (optional): the lengths to pack
+    by in place of the items' own, e.g. recordings' lengths at 44.1 kHz when they are resampled on the device; the items
+    are validated all the same.
 
     Raises before anything is sized or launched, naming the item: ValueError for an empty list, a mel that is not
     [1, 1, T >= 1, 128], or a recording that is empty, not 1-D or all zeros (the reference divides by its zero peak);
@@ -144,14 +154,7 @@ def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
             lengths.append(shape[0])
     if pack_lengths is not None:
         lengths = [int(n) for n in pack_lengths]
-    order = sorted(range(len(items)), key=lambda i: -lengths[i])
-    batches, k = [], 0
-    while k < len(order):
-        cap = lengths[order[k]]
-        n = max(1, int(max_items(cap)))
-        batches.append((cap, order[k:k + n]))
-        k += n
-    return batches
+    return _pack(lengths, max_items)
 
 
 class _ModelShim:
@@ -211,19 +214,14 @@ class Vocoder:
         dev = f"cuda:{eng.device}"
 
         def max_items(T):
-            S = (T + T % 2 + 4) * 441
-            return eng.max_batch_frames(T, extra_per_item=4 * (T * 128 + S))          # + the batch's input and output
+            return eng.max_batch_frames(T, extra_per_item=4 * (T * 128 + _gen_len(T)))   # + the batch's input and output
 
         outs = [None] * len(mels)
         for T_cap, idx in plan_vocoder_many(mels, "mel", max_items):
-            x = torch.zeros((len(idx), T_cap, 128), device=dev)
-            for k, i in enumerate(idx):
-                x[k, :mels[i].shape[2]] = torch.as_tensor(mels[i])[0, 0].to(device=dev, dtype=torch.float32)
-            lens = torch.tensor([mels[i].shape[2] for i in idx], dtype=torch.int32).to(dev)
+            x, lens = _pad_rows([torch.as_tensor(mels[i])[0, 0] for i in idx], T_cap, dev)
             y = eng.vocoder(x, lens=lens)
             for k, i in enumerate(idx):
-                T = mels[i].shape[2]
-                o = y[k:k + 1, None, :(T + T % 2 + 4) * 441]
+                o = y[k:k + 1, None, :_gen_len(mels[i].shape[2])]
                 outs[i] = o.clone() if cuda else o.cpu()
         return outs
 
@@ -250,35 +248,64 @@ class Vocoder:
         _check_cuda(cuda)
         items = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
         rates = resample.rates(sample_rate, len(items), "oracle_many")
-        convert = any(r != resample.RATE for r in rates)
         eng = self._engine
         dev = f"cuda:{eng.device}"
 
         def max_items(L):
-            T = 1 + L // 441
-            per_item = eng.oracle_workspace_bytes(2, L) - eng.oracle_workspace_bytes(1, L) + 4 * (L + (T + T % 2 + 4) * 441)
-            if convert:       # the staged input windows and the resampler's item table
-                per_item += 4 * max(resample.staging_bound(L, r) for r in set(rates)) + 64
-            return eng._fit(per_item, 64, 2 << 30)
+            per_item = eng.oracle_workspace_bytes(2, L) - eng.oracle_workspace_bytes(1, L) + 4 * (L + _gen_len(1 + L // 441))
+            return eng._fit(per_item + _staging_extra(L, rates), 64, 2 << 30)
 
-        lengths = None
-        if convert:
-            lengths = [resample.out_len(a.shape[0], r) if a.ndim == 1 else 0 for a, r in zip(items, rates)]
+        # the recordings' lengths at 44.1 kHz (a recording that is not 1-D is refused by plan_vocoder_many)
+        lengths = [resample.out_len(a.shape[0], r) if a.ndim == 1 else 0 for a, r in zip(items, rates)]
         outs = [None] * len(items)
         for L_cap, idx in plan_vocoder_many(items, "wav", max_items, pack_lengths=lengths):
-            if convert:
-                y, lens = eng.resample(*_stage(items, rates, [(i, 0, lengths[i]) for i in idx], dev), L_cap)
-            else:
-                x = torch.zeros((len(idx), L_cap))
-                for k, i in enumerate(idx):
-                    x[k, :items[i].shape[0]] = torch.from_numpy(items[i])
-                y = x.to(dev)
-                lens = torch.tensor([items[i].shape[0] for i in idx], dtype=torch.int32).to(dev)
-            y = eng.oracle(y, lens=lens).cpu().numpy()
+            x, lens = _batch_input(eng, items, rates, [(i, 0, lengths[i]) for i in idx], L_cap, dev)
+            y = eng.oracle(x, lens=lens).cpu().numpy()
             for k, i in enumerate(idx):
-                T = 1 + (lengths[i] if convert else items[i].shape[0]) // 441
-                outs[i] = y[k:k + 1, :(T + T % 2 + 4) * 441].copy()
+                outs[i] = y[k:k + 1, :_gen_len(1 + lengths[i] // 441)].copy()
         return outs
+
+
+def _staging_extra(L, rates):
+    """Device bytes per item of L output samples that _batch_input adds for a call at these rates: none when they are all
+    44100, else the staged input window (the largest resample.staging_bound) and the item's row of the resampler's table."""
+    if all(r == resample.RATE for r in rates):
+        return 0
+    return 4 * max(resample.staging_bound(L, r) for r in set(rates)) + 64
+
+
+def _pad_rows(rows, cap, dev):
+    """Tensors [n_k, ...] as one float32 batch (B, cap, ...) on dev, row k holding rows[k] then zeros, and the n_k as an
+    int32 (B,) tensor on dev.  Host rows are assembled on the host and uploaded in one copy; if any row is already on
+    the GPU, the batch is assembled there, so no row goes through the host."""
+    on_gpu = any(r.is_cuda for r in rows)
+    x = torch.zeros((len(rows), cap) + tuple(rows[0].shape[1:]), device=dev if on_gpu else "cpu")
+    for k, r in enumerate(rows):
+        x[k, :r.shape[0]] = r
+    return x.to(dev), torch.tensor([r.shape[0] for r in rows], dtype=torch.int32).to(dev)
+
+
+def _batch_input(eng, items, rates, ranges, cap, dev):
+    """(x (B, cap), lens (B,) int32), both on dev: row k of x holds range k of ranges [(item, a, b), ...] of the items'
+    44.1 kHz streams, then zeros.  If any of `rates` (one per item) is not 44100, every row is resampled on the device
+    from its own input window (_stage, Engine.resample); otherwise the samples are copied (_pad_rows), no resampler runs."""
+    if any(r != resample.RATE for r in rates):
+        return eng.resample(*_stage(items, rates, ranges, dev), cap)
+    return _pad_rows([torch.from_numpy(items[i][a:b]) for i, a, b in ranges], cap, dev)
+
+
+def _drop_masks(drop_masks_fn, B, T):
+    """Mode 2's dropout keep-masks for B segments of up to T frames: uint8 (2, B, T, 512) from drop_masks_fn(B, T), or
+    None for drop_masks_fn=False.  The reference's mode 2 is module.train(): both Dropout(0.5) of the denoiser draw from
+    torch's global RNG (base.py:114-115, restorer/model.py:76,90).  Without drop_masks_fn, same distribution here (from
+    torch's CPU generator, so torch.manual_seed controls it); the RNG *stream* differs, which no reference test pins."""
+    if drop_masks_fn is False:
+        return None
+    masks = drop_masks_fn(B, T) if drop_masks_fn else (torch.rand(2, B, T, 512) >= 0.5)
+    masks = torch.as_tensor(masks).to(torch.uint8)
+    if tuple(masks.shape) != (2, B, T, 512):
+        raise ValueError(f"dropout masks must have shape (2, {B}, {T}, 512), got {tuple(masks.shape)}")
+    return masks
 
 
 def _stage(items, rates, segs, dev):
@@ -374,12 +401,7 @@ class VoiceFixer:
         if mode not in (0, 1, 2):
             raise ValueError("mode must be 0, 1 or 2")
         wav = np.ascontiguousarray(wav_10k, dtype=np.float32)
-        n = wav.shape[0]
-        segs = []
-        bp = SEG_LENGTH
-        while bp < n + SEG_LENGTH:                                       # base.py:117-119
-            segs.append(wav[bp - SEG_LENGTH: bp])
-            bp += SEG_LENGTH
+        segs = [wav[a:b] for a, b in segment_bounds(wav.shape[0])]
         eng = self._engine
         dev = f"cuda:{eng.device}"
         groups = {}
@@ -387,11 +409,9 @@ class VoiceFixer:
             groups.setdefault(len(s), []).append(i)
         outs = [None] * len(segs)
         for L, all_idxs in groups.items():
-            Lnet = 512 * (L // 512) if mode == 1 else L                  # mode 1's pre-filter shortens the segment
-            if mode == 2 and 1 + Lnet // 441 <= 64:
+            if mode == 2 and 1 + _net_len(L, mode) // 441 <= 64:
                 # torch.nn.functional.batch_norm in the reference (train mode, 1x1 UNet centre)
-                raise ValueError("Expected more than 1 value per channel when training, got input size "
-                                 "torch.Size([1, 384, 1, 1])")
+                raise ValueError(_MODE2_MSG)
             # the reference walks the segments one at a time in constant memory; here they are batched, in chunks
             # sized to the device memory that is free right now (a 100-minute recording does not fit one launch sequence)
             chunk = eng.max_batch(L)
@@ -399,18 +419,8 @@ class VoiceFixer:
                 idxs = all_idxs[c0:c0 + chunk]
                 x = torch.from_numpy(np.stack([segs[i] for i in idxs])).to(dev)
                 if mode == 1:
-                    x, _ = eng.hf_cut(x)                                 # shorter: 512*(L//512)
-                masks = None
-                if mode == 2 and drop_masks_fn is not False:
-                    T = 1 + x.shape[1] // 441
-                    # the reference's mode 2 is module.train(): both Dropout(0.5) of the denoiser are live and draw
-                    # from torch's global RNG (base.py:114-115, restorer/model.py:76,90).  Same distribution here
-                    # (keep-masks from torch's CPU generator, so torch.manual_seed controls it); the RNG *stream*
-                    # differs from the reference's, which no reference test pins.  drop_masks_fn=False disables it.
-                    masks = drop_masks_fn(x.shape[0], T) if drop_masks_fn else (torch.rand(2, x.shape[0], T, 512) >= 0.5)
-                    masks = torch.as_tensor(masks).to(torch.uint8)
-                    if tuple(masks.shape) != (2, x.shape[0], T, 512):
-                        raise ValueError(f"dropout masks must have shape (2, {x.shape[0]}, {T}, 512), got {tuple(masks.shape)}")
+                    x, _ = eng.hf_cut(x)                                 # shorter: _net_len(L, 1)
+                masks = _drop_masks(drop_masks_fn, x.shape[0], 1 + x.shape[1] // 441) if mode == 2 else None
                 if your_vocoder_func is None:
                     y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks)
                 else:                                                    # base.py:126-129
@@ -459,48 +469,26 @@ class VoiceFixer:
                 raise ValueError(f"restore_many: recording {i} has shape {a.shape}; the list takes 1-D arrays")
             items.append(a)
         rates = resample.rates(sample_rate, len(items), "restore_many")
-        convert = any(r != resample.RATE for r in rates)
         eng = self._engine
         dev = f"cuda:{eng.device}"
 
         def max_items(L_cap):
-            extra = 0
+            extra = _staging_extra(L_cap, rates)
             if mode == 1:     # the pre-filter's workspace and its (B, L_cap) output live alongside the restore
-                extra = eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
-            if convert:       # the staged input windows and the resampler's item table
-                extra += 4 * max(resample.staging_bound(L_cap, r) for r in set(rates)) + 64
+                extra += eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
             return eng.max_batch(L_cap, extra_per_item=extra)
 
-        plan = plan_many([resample.out_len(a.shape[0], r) for a, r in zip(items, rates)], mode, max_items)
+        lengths = [resample.out_len(a.shape[0], r) for a, r in zip(items, rates)]
         pieces = {}                                                      # (recording, start) -> restored segment
-        for L_cap, segs in plan:
-            B = len(segs)
-            if convert:
-                x, lens = eng.resample(*_stage(items, rates, segs, dev), L_cap)
-            else:
-                x = torch.zeros((B, L_cap))
-                for k, (i, a, b) in enumerate(segs):
-                    x[k, :b - a] = torch.from_numpy(items[i][a:b])
-                x = x.to(dev)
-                lens = torch.tensor([b - a for _, a, b in segs], dtype=torch.int32).to(dev)
+        for L_cap, segs in plan_many(lengths, mode, max_items):
+            x, lens = _batch_input(eng, items, rates, segs, L_cap, dev)
             if mode == 1:
                 x, _, lens = eng.hf_cut(x, lens=lens)
-                out_lens = [512 * ((b - a) // 512) for _, a, b in segs]
-            else:
-                out_lens = [b - a for _, a, b in segs]
-            masks = None
-            if mode == 2 and drop_masks_fn is not False:
-                T = 1 + L_cap // 441
-                # the reference's train-mode Dropout(0.5) draws from torch's global RNG; see restore_inmem
-                masks = drop_masks_fn(B, T) if drop_masks_fn else (torch.rand(2, B, T, 512) >= 0.5)
-                masks = torch.as_tensor(masks).to(torch.uint8)
-                if tuple(masks.shape) != (2, B, T, 512):
-                    raise ValueError(f"dropout masks must have shape (2, {B}, {T}, 512), got {tuple(masks.shape)}")
+            masks = _drop_masks(drop_masks_fn, len(segs), 1 + L_cap // 441) if mode == 2 else None
             y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens).cpu().numpy()
-            for k, (i, a, _) in enumerate(segs):
-                pieces[(i, a)] = y[k, :out_lens[k]]
-        return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(resample.out_len(it.shape[0], r))])[None]
-                for i, (it, r) in enumerate(zip(items, rates))]
+            for k, (i, a, b) in enumerate(segs):
+                pieces[(i, a)] = y[k, :_net_len(b - a, mode)]
+        return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(n)])[None] for i, n in enumerate(lengths)]
 
     # ------------------------------------------------------------------ batch entry point (extension)
     def pinned_empty(self, shape):
@@ -535,17 +523,16 @@ class VoiceFixer:
             raise ValueError("restore_batch takes (B, L) with L <= 30 s (longer inputs: restore_inmem segments them)")
         eng = self._engine
         dev = f"cuda:{eng.device}"
-        plans = self.__dict__.setdefault("_batch_plans", {})
         key = tuple(x.shape)
-        if key not in plans:
-            if len(plans) >= 4:                                            # a few shapes at most: graphs own workspaces
-                plans.pop(next(iter(plans)))
+
+        def make():
             p = {"dev_in": torch.empty(key, device=dev), "dev_out": torch.empty(key, device=dev),
                  "host_in": torch.empty(key).pin_memory(), "host_out": torch.empty(key).pin_memory()}
             p["dev_in"].copy_(torch.from_numpy(x))
             p["graph"] = eng.make_graph(p["dev_in"], p["dev_out"], mode=0)
-            plans[key] = p
-        p = plans[key]
+            return p
+
+        p = self._graph_plan(key, make)
         src = torch.from_numpy(x)
         if not src.is_pinned():
             p["host_in"].copy_(src)
@@ -564,31 +551,34 @@ class VoiceFixer:
             return out
         return out if out is not None else dst.numpy()
 
+    def _graph_plan(self, key, make):
+        """The restore_batch plan for key (buffers and the CUDA graph that reads them), made by make() on first use.  Each
+        graph owns its workspace, so at most four shapes are kept, the oldest dropped first."""
+        plans = self.__dict__.setdefault("_batch_plans", {})
+        if key not in plans:
+            if len(plans) >= 4:
+                plans.pop(next(iter(plans)))
+            plans[key] = make()
+        return plans[key]
+
     def _restore_ragged(self, wavs):
         items, lens, L_cap = ragged_plan(wavs)
         B = len(items)
         eng = self._engine
         dev = f"cuda:{eng.device}"
-        plans = self.__dict__.setdefault("_batch_plans", {})
-        key = ("ragged", B, L_cap)
-        p = plans.get(key)
-        fresh = p is None
-        if fresh:
-            if len(plans) >= 4:                                            # a few shapes at most: graphs own workspaces
-                plans.pop(next(iter(plans)))
-            p = {"dev_in": torch.zeros((B, L_cap), device=dev), "dev_out": torch.empty((B, L_cap), device=dev),
-                 "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
-                 "host_in": torch.zeros((B, L_cap)).pin_memory(), "host_out": torch.empty((B, L_cap)).pin_memory(),
-                 "host_lens": torch.empty(B, dtype=torch.int32).pin_memory()}
+        p = self._graph_plan(("ragged", B, L_cap), lambda: {
+            "dev_in": torch.zeros((B, L_cap), device=dev), "dev_out": torch.empty((B, L_cap), device=dev),
+            "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
+            "host_in": torch.zeros((B, L_cap)).pin_memory(), "host_out": torch.empty((B, L_cap)).pin_memory(),
+            "host_lens": torch.empty(B, dtype=torch.int32).pin_memory()})
         hin = p["host_in"].numpy()
         for i, a in enumerate(items):            # samples past an item's length are never read: no need to clear them
             hin[i, :lens[i]] = a
         p["host_lens"].copy_(torch.tensor(lens, dtype=torch.int32))
         p["dev_in"].copy_(p["host_in"], non_blocking=True)
         p["dev_lens"].copy_(p["host_lens"], non_blocking=True)
-        if fresh:
+        if "graph" not in p:                     # captured once the lengths are staged: its warm-up runs read them
             p["graph"] = eng.make_graph(p["dev_in"], p["dev_out"], mode=0, lens=p["dev_lens"])
-            plans[key] = p
         p["graph"].replay()
         p["host_out"].copy_(p["dev_out"], non_blocking=True)
         torch.cuda.current_stream().synchronize()
