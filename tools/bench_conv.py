@@ -22,7 +22,7 @@ for C, L in shapes:
     if args.only and C != args.only:
         continue
     B = args.B
-    odt = torch.bfloat16 if args.prec == "bf16" else torch.float32
+    odt = {"bf16": torch.bfloat16, "fp16": torch.float16}.get(args.prec, torch.float32)   # tf32: fp32 storage
     a = (torch.randn(B, 1, L, C, device=dev) * 0.5).to(odt)
     w = (torch.randn(3, C, C, device=dev) * 0.05).to(odt)
     bias = torch.randn(C, device=dev)
@@ -62,6 +62,6 @@ for C, L in shapes:
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / args.iters
         flops = 2.0 * 3 * C * C * L * B
-        e = 2 if args.prec == "bf16" else 4
+        e = 2 if odt != torch.float32 else 4
         byts = B * L * C * {"c1": 2 * e, "c2": 2 * e + 8, "c2enc": e + 8, "raw": e + 4, "rawact": 2 * e + 4, "actnone": 2 * e}[kind]
         print(f"C={C:4d} L={L:7d} B={B} {kind}: {ms:8.3f} ms  {flops/ms/1e9:8.1f} TF/s  {byts/ms/1e6:8.1f} GB/s (algorithmic)", flush=True)

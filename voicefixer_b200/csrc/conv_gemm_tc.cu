@@ -3,16 +3,27 @@
 //
 //   out[b, oh, ow, n] = bias[n % bias_mod] + residual + sum_{tap} sum_{c} W[tap][n][c] * A[b, qh+dh, qw+dw, c]
 //
-// A CTA computes a 128 x BN output tile with two warpgroups (64 rows each, one m64nBN wgmma accumulator in
-// registers).  The K loop runs over (tap, 128-byte channel slice): every thread stages 16-byte chunks of the
-// shifted input rows and of the tap's weight rows with cp.async into a 4-stage ring of 128-byte-swizzled K-major
-// tiles; chunks outside the input (convolution padding), beyond Cin or beyond N are zero-filled by the copy itself,
-// so any tap offset, stride and edge is handled without a separate padded tensor.  kind tf32 reads fp32 operands and
-// ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the encoded stream of
-// vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.  The epilogue (bias, fp32
-// residual, eval-BN affine, activation, operand for the next layer) works on the accumulator registers directly.
+// Persistent, warp-specialised kernel: grid = min(tiles, SMs), each CTA walks a static stride over the 128 x BN output
+// tiles in N-fastest order (the N tiles of one M tile run together, so their A rows come from HBM about once).
+//  - Producer warpgroup (56 registers): for every K slice (tap, 128-byte channel slice) it stages 16-byte chunks of the
+//    shifted input rows and of the tap's weight rows with cp.async into a ring of 128-byte-swizzled K-major tiles;
+//    chunks outside the input (convolution padding), beyond Cin or beyond N are zero-filled by the copy itself, so any
+//    tap offset, stride and edge is handled without a separate padded tensor.  Stages are handed over through full /
+//    empty mbarriers; it fills the ring for the next tile while the consumers run the epilogue.
+//  - Two consumer warpgroups (224 registers), 64 rows each: one m64nBN wgmma group in flight per warpgroup, into one of
+//    two partial accumulators, while the previous slice's partial is added to the fp32 accumulator.
+//  - Staged epilogue: the tile goes through a shared fp32 buffer and is processed row by row (bias, fp32 residual,
+//    eval-BN affine, activation, operand for the next layer), with 16-byte accesses where the host found every pointer,
+//    stride and column offset aligned.
+// kind tf32 reads fp32 operands and ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the
+// encoded stream of vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.
 // Ragged batches (seq_in / seq_out): each item's extent on the sequence axis acts as that item's own edge, so every row
-// inside it is computed from the same operands as with the item alone.
+// inside it is computed from the same operands as with the item alone; a tile none of whose rows is stored is skipped.
+//
+// What still stands between this kernel and the roof: the producer recomputes and issues every 16-byte chunk with
+// cp.async (no TMA), the A halo of the taps is re-read from L2 for every tap, and the per-slice sum costs BN / 2 FADDs
+// per slice in the consumers.
+#include <atomic>
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -20,152 +31,305 @@ namespace vfx {
 
 namespace {
 
-constexpr int BM = 128, NT = 256, STAGES = 4;
+constexpr int BM = 128, NT = 384;                  // warpgroup 0 produces, warpgroups 1 and 2 consume
 constexpr int A_BYTES = BM * 128;
+constexpr int SMEM_MAX = 227 * 1024;               // dynamic shared memory of one sm_90 CTA
+constexpr int PROD_REGS = 56, CONS_REGS = 224;     // 128 x 56 + 256 x 224 <= 384 x 168 (the launch allocation)
 
 template <int KIND> struct OpT;
 template <> struct OpT<0> { using T = tf32_t; static constexpr int ESZ = 4; };
 template <> struct OpT<1> { using T = __nv_bfloat16; static constexpr int ESZ = 2; };
 template <> struct OpT<2> { using T = __half; static constexpr int ESZ = 2; };
 
-template <int BN> constexpr int smem_bytes() { return STAGES * (A_BYTES + BN * 128) + 1024; }
+// epilogue offsets of one tile row (ok == 0: the row is not stored)
+struct OutRow { long long raw, act, res; int ok; };
 
-// SEQ: the descriptor carries per-item extents (seq_in / seq_out); without them the kernel is compiled without the checks
+template <int BN> struct Cfg {
+  static constexpr int STAGE = A_BYTES + BN * 128;
+  static constexpr int EPI_LD = BN + 8;            // fp32 words per epilogue row; +8 keeps the fragment stores conflict-free
+  static constexpr int EPI = BM * EPI_LD * 4;
+  static constexpr int ROWS = BM * 24 + BM * (int)sizeof(OutRow);   // producer and epilogue row tables
+  static constexpr int FIXED = 1024 + EPI + ROWS;  // + 1024: alignment of the ring
+  static constexpr int FIT = (SMEM_MAX - FIXED) / (STAGE + 16);
+  static constexpr int STAGES = FIT < 8 ? FIT : 8;                  // 4 at BN = 128, 7 at 64, 8 at 32
+  // The producer signals slice k full after issuing slice k + AHEAD (cp.async.wait_group AHEAD).  It must wait for an
+  // empty slot before issuing, and the consumers free slot k - 1 only once slice k is full, so AHEAD <= STAGES - 2:
+  // with more, the producer waits for a slot the consumers can only free after a signal it has not sent yet.
+  static constexpr int AHEAD = STAGES - 2;
+  static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
+  static_assert(STAGES >= 3 && SMEM <= SMEM_MAX, "conv_gemm_tc: shared-memory plan");
+};
+
+// output-grid row m -> item b and grid position (qh, qw); false beyond the problem (M < 2^31: 32-bit divisions)
+__device__ __forceinline__ bool grid_row(const vfx_conv_desc& d, int M, int m, int& b, int& qh, int& qw) {
+  if (m >= M) return false;
+  qw = m % d.Wq;
+  const int r = m / d.Wq;
+  qh = r % d.Hq; b = r / d.Hq;
+  return true;
+}
+// whether grid position (b, qh, qw) is stored: inside the output and, in a ragged batch, inside its item's extent.
+// The producer and the consumers both decide a tile's skip from this function alone, so they walk the same tiles.
+template <bool SEQ> __device__ __forceinline__ bool row_stored(const vfx_conv_desc& d, int b, int qh, int qw) {
+  const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
+  return oh < d.OH && ow < d.OW && (!SEQ || !d.seq_out || (d.seq_axis ? ow : oh) < d.seq_out[b]);
+}
+
+// one output element, in the order every path keeps: bias, then the residual (rv, decoded when encoded), then the raw
+// output (encoded when asked), then the BN affine and the activation of the operand
+__device__ __forceinline__ float add_in(const vfx_conv_desc& d, float v, int n, float rv) {
+  if (d.bias) v += d.bias[n % d.bias_mod];
+  if (d.residual) v += d.res_enc ? stream_dec(rv, 1.0f / d.enc_slope) : rv;
+  return v;
+}
+__device__ __forceinline__ float raw_out(const vfx_conv_desc& d, float v) { return d.raw_enc ? stream_enc(v, d.enc_slope) : v; }
+__device__ __forceinline__ float act_out(const vfx_conv_desc& d, float v, int n) {
+  const float va = d.act_scale ? fmaf(v, d.act_scale[n], d.act_shift[n]) : v;
+  return apply_act(va, d.act, d.act_param);
+}
+
+// SEQ: the descriptor carries per-item extents (seq_in / seq_out); without them the kernel is compiled without the checks.
+// vec: every output / residual pointer, stride and column offset allows 4-column vector accesses.
 template <int BN, int KIND, bool SEQ>
-__global__ void __launch_bounds__(NT) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d, const int nkc) {
+__global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d, const int nkc,
+                                                                 const int vec) {
   using T = typename OpT<KIND>::T;
+  using C = Cfg<BN>;
   constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
-  constexpr int STAGE = A_BYTES + BN * 128;
+  constexpr int S = C::STAGES, STAGE = C::STAGE, AHEAD = C::AHEAD;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* const gbase = smem_raw + (sbase - smem_u32(smem_raw));
+  float* const epi = reinterpret_cast<float*>(gbase + S * STAGE);
+  int4* const prow = reinterpret_cast<int4*>(gbase + S * STAGE + C::EPI);
+  long long* const pbase = reinterpret_cast<long long*>(prow + BM);
+  OutRow* const crow = reinterpret_cast<OutRow*>(pbase + BM);
+  const uint32_t full0 = sbase + S * STAGE + C::EPI + C::ROWS, empty0 = full0 + 8 * S;
 
   const int tid = threadIdx.x;
-  const long long M = (long long)d.B * d.Hq * d.Wq;
-  const long long m0 = (long long)blockIdx.x * BM;
-  const int n0 = blockIdx.y * BN;
-  const char* __restrict__ A = reinterpret_cast<const char*>(d.a);
-  const char* __restrict__ Wt = reinterpret_cast<const char*>(d.w);
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full0 + 8 * s, 128);    // every producer thread, after its own copies of the stage have landed
+      mbar_init(empty0 + 8 * s, 8);     // every consumer warp, after its wgmma group has read the stage
+    }
+  }
+  __syncthreads();
 
-  // ---- this thread's staging work: chunk `chunk` of A rows lrow + 32 i and of B rows lrow + 32 i
-  const int chunk = tid & 7, lrow = tid >> 3;
-  int rb[4], rh[4], rw[4], rlim[4];     // rlim: the item's extent on the sequence axis (vfx_conv_desc.seq_in)
-  bool live = false;                    // some row of this thread is stored (checked only with seq_out)
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const long long m = m0 + lrow + 32 * i;
-    if (m < M) {
-      rw[i] = (int)(m % d.Wq);
-      const long long r = m / d.Wq;
-      rh[i] = (int)(r % d.Hq); rb[i] = (int)(r / d.Hq);
-      rlim[i] = SEQ && d.seq_in ? d.seq_in[rb[i]] : 0x7fffffff;
-      if (SEQ && d.seq_out) {
-        const int oh = rh[i] * d.sh + d.rh, ow = rw[i] * d.sw + d.rw;
-        live |= oh < d.OH && ow < d.OW && (d.seq_axis ? ow : oh) < d.seq_out[rb[i]];
+  // derived after each role's setmaxnreg, so that nothing stays live across it
+#define VFX_TILE_WALK                                                                                              \
+  const int M = d.B * d.Hq * d.Wq;                 /* < 2^31, and so is the tile count (conv_gemm_tc) */           \
+  const int ntn = (d.N + BN - 1) / BN, ntiles = (M + BM - 1) / BM * ntn, niter = d.ntaps * nkc;                    \
+  const bool skips = SEQ && d.seq_out;
+
+  if (tid < 128) {
+    // ================================================================ producer
+    setmaxnreg_dec<PROD_REGS>();
+    VFX_TILE_WALK
+    // this thread's staging work: chunk `chunk` of A rows lrow + 16 i and of B rows lrow + 16 i
+    const int chunk = tid & 7, lrow = tid >> 3;
+    uint32_t k = 0;                                   // K slices issued by this CTA
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      const int m0 = t / ntn * BM;
+      const int n0 = t % ntn * BN;
+      named_sync(1, 128);                             // the previous tile's row table is no longer read
+      // row tid: its element offset in A and its valid input ranges ih in [0, hlim), iw in [0, wlim), relative to the
+      // row (the input edges and, in a ragged batch, its item's extent vfx_conv_desc.seq_in); none beyond M
+      int4 q = make_int4(0, 0, 0, 0);
+      long long base = 0;
+      bool live = false;
+      int b, qh, qw;
+      if (grid_row(d, M, m0 + tid, b, qh, qw)) {
+        const int rlim = SEQ && d.seq_in ? d.seq_in[b] : 0x7fffffff;
+        const int hl = SEQ && d.seq_axis == 0 && rlim < d.H ? rlim : d.H, wl = SEQ && d.seq_axis == 1 && rlim < d.W ? rlim : d.W;
+        q = make_int4(qh, hl > 0 ? hl : 0, qw, wl > 0 ? wl : 0);
+        base = (long long)b * d.a_sB + (long long)qh * d.a_sH + (long long)qw * d.a_sW;
+        live = row_stored<SEQ>(d, b, qh, qw);
       }
-    } else {
-      rb[i] = -1; rh[i] = 0; rw[i] = 0; rlim[i] = 0;
+      prow[tid] = q;
+      pbase[tid] = base;
+      if (skips) {
+        if (!named_sync_or(1, 128, live)) continue;   // ragged batch: no row of this tile is stored
+      } else {
+        named_sync(1, 128);
+      }
+      for (int it = 0; it < niter; ++it, ++k) {
+        const int s = k % S;
+        if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+        const int tap = it / nkc;
+        const int c = (it - tap * nkc) * BK + chunk * AL;
+        const bool c_ok = c < d.Cin;
+        const uint32_t sa = sbase + s * STAGE, sb = sa + A_BYTES;
+        const int dh = d.dh[tap], dw = d.dw[tap];
+        const long long toff = (long long)dh * d.a_sH + (long long)dw * d.a_sW + c;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int r = lrow + 16 * i;
+          const int4 p = prow[r];
+          const bool ok = c_ok && (unsigned)(p.x + dh) < (unsigned)p.y && (unsigned)(p.z + dw) < (unsigned)p.w;
+          const char* src = static_cast<const char*>(d.a) + (ok ? (pbase[r] + toff) * ESZ : 0);
+          cp_async16(sa + sw128_offset(r, chunk), src, ok);
+        }
+#pragma unroll 4
+        for (int i = 0; i < BN / 16; ++i) {
+          const int n = lrow + 16 * i;
+          const bool ok = c_ok && n0 + n < d.N;
+          const char* src = static_cast<const char*>(d.w) + (ok ? (d.w_off[tap] + (long long)(n0 + n) * d.Cin + c) * ESZ : 0);
+          cp_async16(sb + sw128_offset(n, chunk), src, ok);
+        }
+        cp_async_commit();
+        if (k >= (uint32_t)AHEAD) {
+          cp_async_wait<AHEAD>();                     // this thread's chunks of slice k - AHEAD have landed
+          fence_proxy_async();                        // ... and are visible to the tensor core's (async-proxy) reads
+          mbar_arrive(full0 + 8 * ((k - AHEAD) % S));
+        }
+      }
     }
-  }
-  // ragged batch: a tile whose 128 rows all lie beyond their items' extents has nothing to store
-  if (SEQ && d.seq_out && !__syncthreads_or(live)) return;
-  const int niter = d.ntaps * nkc;
-  auto load_stage = [&](int it, int s) {
-    const int tap = it / nkc;
-    const int c = (it - tap * nkc) * BK + chunk * AL;
-    const bool c_ok = c < d.Cin;
-    const uint32_t sa = sbase + s * STAGE, sb = sa + A_BYTES;
-    const int dh = d.dh[tap], dw = d.dw[tap];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = lrow + 32 * i;
-      const int ih = rh[i] + dh, iw = rw[i] + dw;
-      const bool ok = c_ok && rb[i] >= 0 && ih >= 0 && ih < d.H && iw >= 0 && iw < d.W && (!SEQ || (d.seq_axis ? iw : ih) < rlim[i]);
-      const char* src = ok ? A + ((long long)rb[i] * d.a_sB + (long long)ih * d.a_sH + (long long)iw * d.a_sW + c) * ESZ : A;
-      cp_async16(sa + sw128_offset(r, chunk), src, ok);
-    }
-#pragma unroll
-    for (int i = 0; i < BN / 32; ++i) {
-      const int n = lrow + 32 * i;
-      const bool ok = c_ok && n0 + n < d.N;
-      const char* src = ok ? Wt + (d.w_off[tap] + (long long)(n0 + n) * d.Cin + c) * ESZ : Wt;
-      cp_async16(sb + sw128_offset(n, chunk), src, ok);
-    }
-  };
-
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  const int wg = tid >> 7;
-
-#pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
-    if (s < niter) load_stage(s, s);
-    cp_async_commit();
-  }
-  for (int it = 0; it < niter; ++it) {
-    cp_async_wait<STAGES - 2>();          // this thread's chunks of stage `it` have landed
+    cp_async_wait<0>();
     fence_proxy_async();
-    __syncthreads();                      // ... everyone's, and stage it-1 is no longer read by either warpgroup
-    if (it + STAGES - 1 < niter) load_stage(it + STAGES - 1, (it + STAGES - 1) % STAGES);
-    cp_async_commit();
-    const uint32_t sa = sbase + (it % STAGES) * STAGE;
-    const uint64_t da = sw128_desc(sa + wg * 64 * 128), db = sw128_desc(sa + A_BYTES);
-    float part[BN / 2];
+    for (uint32_t j = k > (uint32_t)AHEAD ? k - AHEAD : 0; j < k; ++j) mbar_arrive(full0 + 8 * (j % S));
+    return;
+  }
+
+  // ================================================================== consumers
+  setmaxnreg_inc<CONS_REGS>();
+  VFX_TILE_WALK
+#undef VFX_TILE_WALK
+  const int ct = tid - 128, cw = ct >> 7, w = (ct >> 5) & 3, l = tid & 31;
+  T* out_act = reinterpret_cast<T*>(d.out_act);
+  float acc[BN / 2], p0[BN / 2], p1[BN / 2];
+  // issue slice kk's 4 wgmma into p (zeroed: the tensor core's accumulator adds truncate, see retire)
+  auto issue = [&](float (&p)[BN / 2], uint32_t kk) {
+    const uint32_t s = kk % S;
+    mbar_wait(full0 + 8 * s, (kk / S) & 1);
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+    for (int i = 0; i < BN / 2; ++i) p[i] = 0.f;
+    const uint32_t sa = sbase + s * STAGE;
+    const uint64_t da = sw128_desc(sa + cw * 64 * 128), db = sw128_desc(sa + A_BYTES);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) Wgmma<BN, KIND>::mma(part, da + 2 * kk, db + 2 * kk);   // 32 bytes of K each
+    for (int q = 0; q < 4; ++q) Wgmma<BN, KIND>::mma(p, da + 2 * q, db + 2 * q);   // 32 bytes of K each
     wgmma_commit();
-    wgmma_wait<0>();
-    // the tensor core's accumulator adds truncate; summing the K slices here rounds to nearest, so the error of
-    // long reductions (9 taps x 768 channels) does not build up as a bias
+  };
+  // slice kk's group has completed: free its stage and add it.  Summing the K slices here rounds to nearest, so the
+  // error of long reductions (9 taps x 768 channels) does not build up as a bias.
+  auto retire = [&](float (&p)[BN / 2], uint32_t kk) {
+    wgmma_fence_operand(p);                           // the reads of p below stay after the wgmma_wait that precedes
+    __syncwarp();
+    if (l == 0) mbar_arrive(empty0 + 8 * (kk % S));
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-  }
-  cp_async_wait<0>();
+    for (int i = 0; i < BN / 2; ++i) acc[i] += p[i];
+  };
 
-  // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of warpgroup wg is
-  //      row wg*64 + w*16 + l/4 + 8h, column 8j + 2(l%4) + e
-  const int w = (tid >> 5) & 3, l = tid & 31;
-  T* out_act = reinterpret_cast<T*>(d.out_act);
+  uint32_t k = 0;                                     // K slices consumed by this CTA
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int m0 = t / ntn * BM;
+    const int n0 = t % ntn * BN;
+    if (skips) {
+      int b, qh, qw;
+      const bool live = grid_row(d, M, m0 + (ct & 127), b, qh, qw) && row_stored<SEQ>(d, b, qh, qw);
+      if (!named_sync_or(2, 256, live)) continue;
+    }
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const long long m = m0 + wg * 64 + w * 16 + (l >> 2) + 8 * h;
-    if (m >= M) continue;
-    const int qw = (int)(m % d.Wq);
-    const long long r = m / d.Wq;
-    const int qh = (int)(r % d.Hq), b = (int)(r / d.Hq);
-    const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
-    if (oh >= d.OH || ow >= d.OW) continue;
-    if (SEQ && d.seq_out && (d.seq_axis ? ow : oh) >= d.seq_out[b]) continue;
-    const long long o_raw = (long long)b * d.o_sB + (long long)oh * d.o_sH + (long long)ow * d.o_sW + d.o_col;
-    const long long o_act = (long long)b * d.oa_sB + (long long)oh * d.oa_sH + (long long)ow * d.oa_sW + d.oa_col;
-    const long long o_res = (long long)b * d.r_sB + (long long)oh * d.r_sH + (long long)ow * d.r_sW + d.r_col;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // slice it goes to p[it & 1]; slice it - 1 is added while slice it is in flight
+    issue(p0, k);
+    int it = 1;
+    for (; it + 1 < niter; it += 2) {
+      issue(p1, k + it);
+      wgmma_wait<1>();
+      retire(p0, k + it - 1);
+      issue(p0, k + it + 1);
+      wgmma_wait<1>();
+      retire(p1, k + it);
+    }
+    if (it < niter) {
+      issue(p1, k + it);
+      wgmma_wait<1>();
+      retire(p0, k + it - 1);
+      wgmma_wait<0>();
+      retire(p1, k + it);
+    } else {
+      wgmma_wait<0>();
+      retire(p0, k + it - 1);
+    }
+    k += niter;
+
+    // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is
+    //      row cw*64 + w*16 + l/4 + 8h, column 8j + 2(l%4) + e
+    named_sync(2, 256);                               // the previous tile's epilogue has finished reading epi / crow
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = n0 + 8 * j + 2 * (l & 3) + e;
-        if (n >= d.N) continue;
-        float v = acc[4 * j + 2 * h + e];
-        if (d.bias) v += d.bias[n % d.bias_mod];
+      for (int h = 0; h < 2; ++h) {
+        const int row = cw * 64 + w * 16 + (l >> 2) + 8 * h;
+        *reinterpret_cast<float2*>(epi + row * C::EPI_LD + 8 * j + 2 * (l & 3)) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    if (ct < BM) {
+      OutRow o{0, 0, 0, 0};
+      int b, qh, qw;
+      if (grid_row(d, M, m0 + ct, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw)) {
+        const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
+        o.raw = (long long)b * d.o_sB + (long long)oh * d.o_sH + (long long)ow * d.o_sW + d.o_col;
+        o.act = (long long)b * d.oa_sB + (long long)oh * d.oa_sH + (long long)ow * d.oa_sW + d.oa_col;
+        o.res = (long long)b * d.r_sB + (long long)oh * d.r_sH + (long long)ow * d.r_sW + d.r_col;
+        o.ok = 1;
+      }
+      crow[ct] = o;
+    }
+    named_sync(2, 256);
+
+    // row by row: BN / 4 threads per row, 4 consecutive columns each
+    constexpr int TPR = BN / 4, RPP = 256 / TPR;
+    const int c4 = (ct % TPR) * 4, n = n0 + c4;
+    if (n >= d.N) continue;
+    const bool full = vec && n + 4 <= d.N;
+    for (int r = ct / TPR; r < BM; r += RPP) {
+      const OutRow o = crow[r];
+      if (!o.ok) continue;
+      const float* src = epi + r * C::EPI_LD + c4;
+      if (full) {
+        float4 v = *reinterpret_cast<const float4*>(src);
         if (d.residual) {
-          const float rv = d.residual[o_res + n];
-          v += d.res_enc ? stream_dec(rv, 1.0f / d.enc_slope) : rv;
+          const float4 rv = *reinterpret_cast<const float4*>(d.residual + o.res + n);
+          v = make_float4(add_in(d, v.x, n, rv.x), add_in(d, v.y, n + 1, rv.y), add_in(d, v.z, n + 2, rv.z), add_in(d, v.w, n + 3, rv.w));
+        } else {
+          v = make_float4(add_in(d, v.x, n, 0.f), add_in(d, v.y, n + 1, 0.f), add_in(d, v.z, n + 2, 0.f), add_in(d, v.w, n + 3, 0.f));
         }
-        if (d.out_raw) d.out_raw[o_raw + n] = d.raw_enc ? stream_enc(v, d.enc_slope) : v;
+        if (d.out_raw)
+          *reinterpret_cast<float4*>(d.out_raw + o.raw + n) = make_float4(raw_out(d, v.x), raw_out(d, v.y), raw_out(d, v.z), raw_out(d, v.w));
         if (out_act) {
-          const float va = d.act_scale ? fmaf(v, d.act_scale[n], d.act_shift[n]) : v;
-          out_act[o_act + n] = from_f<T>(apply_act(va, d.act, d.act_param));
+          const float y0 = act_out(d, v.x, n), y1 = act_out(d, v.y, n + 1), y2 = act_out(d, v.z, n + 2), y3 = act_out(d, v.w, n + 3);
+          if (ESZ == 4)
+            *reinterpret_cast<float4*>(out_act + o.act + n) = make_float4(round_tf32(y0), round_tf32(y1), round_tf32(y2), round_tf32(y3));
+          else
+            *reinterpret_cast<uint2*>(out_act + o.act + n) = make_uint2(pack16<KIND == 2>(y0, y1), pack16<KIND == 2>(y2, y3));
+        }
+      } else {
+        for (int e = 0; e < 4 && n + e < d.N; ++e) {
+          const float v = add_in(d, src[e], n + e, d.residual ? d.residual[o.res + n + e] : 0.f);
+          if (d.out_raw) d.out_raw[o.raw + n + e] = raw_out(d, v);
+          if (out_act) out_act[o.act + n + e] = from_f<T>(act_out(d, v, n + e));
         }
       }
+    }
   }
 }
 
+int sm_count(int dev) {
+  static std::atomic<int> sms[64];                    // per device, queried once (host threads may drive several devices)
+  if (dev < 64) {
+    const int n = sms[dev].load(std::memory_order_relaxed);
+    if (n) return n;
+  }
+  int n = 0;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 0;
+  if (dev < 64) sms[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
 template <int BN, int KIND, bool SEQ>
-int launch(const vfx_conv_desc& d, cudaStream_t st) {
-  constexpr int smem = smem_bytes<BN>();
+int launch(const vfx_conv_desc& d, int vec, cudaStream_t st) {
+  constexpr int smem = Cfg<BN>::SMEM;
   static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
   int dev = 0;
   VFX_CUDA_CHECK(cudaGetDevice(&dev));
@@ -173,24 +337,32 @@ int launch(const vfx_conv_desc& d, cudaStream_t st) {
     VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, SEQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     if (dev < 64) attr_set |= 1ull << dev;
   }
-  const long long M = (long long)d.B * d.Hq * d.Wq;
+  const int sms = sm_count(dev);
+  VFX_REQUIRE(sms > 0, "conv_gemm_tc: cannot read the SM count of device %d", dev);
   const int nkc = ceil_div(d.Cin, 128 / OpT<KIND>::ESZ);
-  dim3 grid(ceil_div(M, BM), ceil_div(d.N, BN));
-  conv_gemm_wgmma_kernel<BN, KIND, SEQ><<<grid, NT, smem, st>>>(d, nkc);
+  const long long tiles = ((long long)d.B * d.Hq * d.Wq + BM - 1) / BM * ceil_div(d.N, BN);
+  const int grid = (int)(tiles < sms ? tiles : sms);
+  if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
+  conv_gemm_wgmma_kernel<BN, KIND, SEQ><<<grid, NT, smem, st>>>(d, nkc, vec);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }
 
 template <int KIND, bool SEQ>
-int launch_n(const vfx_conv_desc& d, cudaStream_t st) {
-  if (d.N <= 32) return launch<32, KIND, SEQ>(d, st);
-  if (d.N <= 64) return launch<64, KIND, SEQ>(d, st);
-  return launch<128, KIND, SEQ>(d, st);
+int launch_n(const vfx_conv_desc& d, int vec, cudaStream_t st) {
+  if (d.N <= 32) return launch<32, KIND, SEQ>(d, vec, st);
+  if (d.N <= 64) return launch<64, KIND, SEQ>(d, vec, st);
+  return launch<128, KIND, SEQ>(d, vec, st);
 }
 
 template <int KIND>
-int launch_kind(const vfx_conv_desc& d, cudaStream_t st) {
-  return (d.seq_in || d.seq_out) ? launch_n<KIND, true>(d, st) : launch_n<KIND, false>(d, st);
+int launch_kind(const vfx_conv_desc& d, int vec, cudaStream_t st) {
+  return (d.seq_in || d.seq_out) ? launch_n<KIND, true>(d, vec, st) : launch_n<KIND, false>(d, vec, st);
+}
+
+// 4 consecutive columns of every output row start 4 * esz-aligned (16 B for fp32)
+bool vec_ok(const void* p, int esz, long long sB, long long sH, long long sW, int col) {
+  return !p || (((uintptr_t)p & (4 * esz - 1)) == 0 && (sB | sH | sW | col) % 4 == 0);
 }
 
 }  // namespace
@@ -204,14 +376,20 @@ int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st) {
   VFX_REQUIRE(!d.bias || d.bias_mod > 0, "conv_gemm: bias_mod must be > 0");
   if ((d.res_enc && d.residual) || (d.raw_enc && d.out_raw))
     VFX_REQUIRE(d.enc_slope > 0.f, "conv_gemm_tc: enc_slope must be positive");
-  const int al = 16 / (int)prec_esz(precision);     // 16-byte cp.async chunks of operand rows
+  const int esz = (int)prec_esz(precision);
+  const int al = 16 / esz;                          // 16-byte cp.async chunks of operand rows
   if (d.Cin % al || d.a_sW % al || d.a_sH % al || d.a_sB % al || ((uintptr_t)d.a & 15) || ((uintptr_t)d.w & 15))
     return VFX_ERR_UNSUPPORTED;
   for (int t = 0; t < d.ntaps; ++t) if (d.w_off[t] % al) return VFX_ERR_UNSUPPORTED;
-  if (ceil_div((long long)d.B * d.Hq * d.Wq, BM) >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;
-  if (precision == VFX_PREC_TF32) return launch_kind<0>(d, st);
-  if (precision == VFX_PREC_BF16) return launch_kind<1>(d, st);
-  return launch_kind<2>(d, st);
+  const long long M = (long long)d.B * d.Hq * d.Wq;
+  if (M + BM - 1 >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;       // rows and tile row ends (m0 + 127) stay inside int
+  // the ConvT phase groups and the concat buffers start rows at arbitrary columns: vector epilogue only when aligned
+  const int vec = vec_ok(d.out_raw, 4, d.o_sB, d.o_sH, d.o_sW, d.o_col) &&
+                  vec_ok(d.out_act, esz, d.oa_sB, d.oa_sH, d.oa_sW, d.oa_col) &&
+                  vec_ok(d.residual, 4, d.r_sB, d.r_sH, d.r_sW, d.r_col);
+  if (precision == VFX_PREC_TF32) return launch_kind<0>(d, vec, st);
+  if (precision == VFX_PREC_BF16) return launch_kind<1>(d, vec, st);
+  return launch_kind<2>(d, vec, st);
 }
 
 }  // namespace vfx

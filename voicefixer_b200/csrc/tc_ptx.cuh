@@ -1,5 +1,6 @@
 // PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu): cp.async operand staging with zero fill,
-// the generic -> async proxy fence, wgmma fences / groups and the shared-memory matrix descriptor.
+// the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups and the shared-memory
+// matrix descriptor.
 #pragma once
 #include "vfx_common.cuh"
 
@@ -17,9 +18,41 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 // wgmma reads shared memory through the async proxy: make this thread's (generic-proxy) cp.async data visible to it
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// mbarrier stage hand-off (arrive: release, try_wait: acquire, both at CTA scope)
+__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  while (!done)
+    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+}
+// named barriers over a subset of the CTA's warps (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ bool named_sync_or(int id, int nthreads, bool v) {
+  uint32_t r;
+  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %1, 0;\n\tbar.red.or.pred q, %2, %3, p;\n\tselp.u32 %0, 1, 0, q;\n\t}"
+               : "=r"(r) : "r"((uint32_t)v), "r"(id), "r"(nthreads) : "memory");
+  return r != 0;
+}
+// per-warpgroup register budget of a warp-specialised kernel
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// register dependence on a wgmma accumulator: the compiler may not move its reads or writes across this point
+template <int N> __device__ __forceinline__ void wgmma_fence_operand(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
 
 // K-major operand tile with 128-byte rows in the 128-byte swizzle (16-byte chunk c of row r stored at chunk c ^ (r & 7)),
 // 1024-byte aligned.  Descriptor: [0,14) start >> 4, [16,30) leading offset >> 4 (unused for this layout: 1),
