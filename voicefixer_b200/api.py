@@ -3,7 +3,10 @@
 Same class names, method signatures, checkpoint paths and error types; the bodies run the
 hand-written sm_90a kernels through the C-ABI engine.  The `cuda` argument is accepted for
 signature compatibility: the computation always runs on the GPU (there is no CPU path)."""
+import numbers
 import os
+from collections import deque
+
 import numpy as np
 import torch
 
@@ -157,6 +160,263 @@ def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
     return _pack(lengths, max_items)
 
 
+_STREAM_SHORT = "restore_stream: fewer than 1025 samples in total; the front end reflect-pads 1024"
+
+
+class StreamSchedule:
+    """The window rule of VoiceFixer.restore_stream and StreamPool, in samples at 44.1 kHz.  Each chunk of `chunk`
+    samples is restored inside the window [pos - ctx, pos + chunk + ctx), clipped to the stream, as soon as that window has
+    arrived; at the end of the stream the last windows are flushed without (full) look-ahead.  Only the chunk itself is
+    kept from each window."""
+
+    def __init__(self, chunk, ctx):
+        self.chunk, self.ctx = int(chunk), int(ctx)
+        # the longest window due() returns: chunk + 2 ctx for a full window; a flush window shorter than 1025 samples is
+        # widened to 1025 + ctx; with ctx = 0 a flush window may take in a tail of up to 1024 samples after its chunk
+        if self.ctx == 0:
+            self.capacity = max(self.chunk + 1024, 1025)
+        else:
+            self.capacity = max(self.chunk + 2 * self.ctx, 1025 + self.ctx)
+
+    def due(self, pos, avail, ended):
+        """([(lo, hi, keep_lo, keep_hi), ...], new pos): the windows that are due once samples [0, avail) of the stream
+        have arrived (and nothing more will, if `ended`) and every sample before `pos` has been scheduled.  Window
+        [lo, hi) is restored whole and its samples [keep_lo, keep_hi) are emitted; the new pos follows the last of them.
+        Raises RuntimeError, restore_stream's message, when an ended stream leaves a flush window that cannot reach 1025
+        samples (the front end reflect-pads 1024)."""
+        chunk, ctx = self.chunk, self.ctx
+        windows = []
+        while avail >= pos + chunk + ctx:                                # a full chunk plus its look-ahead has arrived
+            windows.append((max(0, pos - ctx), pos + chunk + ctx, pos, pos + chunk))
+            pos += chunk
+        while ended and pos < avail:                                     # flush: the last windows have no (full) look-ahead
+            hi = min(avail, pos + chunk + ctx)
+            keep_hi = min(avail, pos + chunk)
+            if avail - keep_hi <= 1024 and avail - keep_hi > 0 and ctx == 0:  # never leave a tail the front end cannot pad
+                keep_hi = hi = avail
+            lo = max(0, pos - ctx)
+            if hi - lo <= 1024:                                          # reflect padding needs > 1024 samples (base.py:78)
+                lo = max(0, hi - 1025 - ctx)
+                if hi - lo <= 1024:
+                    raise RuntimeError(_STREAM_SHORT)
+            windows.append((lo, hi, pos, keep_hi))
+            pos = keep_hi
+        return windows, pos
+
+
+class _Stream:
+    """One stream of a StreamPool: its recent input at its own rate and where its schedule stands."""
+
+    def __init__(self, rate):
+        self.rate = rate
+        self._data = np.zeros(0, dtype=np.float32)  # buf = _data[_lo:_hi], grown by doubling: a push copies its block once
+        self._lo = self._hi = 0
+        self.base = 0                              # buf holds input samples [base, n) at `rate`
+        self.n = 0                                 # input samples received
+        self.pos = 0                               # next 44.1 kHz sample to schedule
+        self.pending = deque()                     # windows scheduled and not yet restored, oldest first
+        self.closed = False
+
+    @property
+    def buf(self):
+        return self._data[self._lo:self._hi]
+
+    def append(self, a):
+        if self._hi + a.shape[0] > self._data.shape[0]:
+            held = self.buf
+            self._data = np.empty(max(4096, 2 * (held.shape[0] + a.shape[0])), dtype=np.float32)
+            self._data[:held.shape[0]] = held
+            self._lo, self._hi = 0, held.shape[0]
+        self._data[self._hi:self._hi + a.shape[0]] = a
+        self._hi += a.shape[0]
+        self.n += a.shape[0]
+
+    def drop_before(self, first):
+        """Forgets the input before sample `first`."""
+        if first > self.base:
+            self._lo += first - self.base
+            self.base = first
+
+
+class StreamPool:
+    """Many live streams restored together (VoiceFixer.stream_pool), driven by one caller thread.
+
+    Every stream follows restore_stream's window rule (StreamSchedule) on its own 44.1 kHz samples.  A window is due as
+    soon as the input it needs has arrived; step() restores the due windows of all streams, oldest first, as one ragged
+    batch: the rows of a (B, window_len) input, B the smallest bucket (a power of two, or max_windows) that holds them,
+    and one replay of a restore graph captured for that bucket.  The concatenation of everything step() returns for a
+    stream is bit-identical to restore_stream on that stream's audio alone, however pushes, closes and steps interleave.
+
+    A stream at another rate than 44.1 kHz is kept at its own rate on the host; its 44.1 kHz samples [0, m) are available
+    once the input they read has arrived (resample.available), all of them after close().  Its windows are resampled on
+    the device (Engine.resample) into the step's input rows, bit-identical to wavio._resample on the whole stream."""
+
+    def __init__(self, engine, chunk_seconds=2.0, context_seconds=1.0, max_windows=None, device=None):
+        chunk = int(round(chunk_seconds * 44100))
+        ctx = int(round(context_seconds * 44100))
+        if chunk <= 0 or ctx < 0:
+            raise ValueError("chunk_seconds must be positive and context_seconds non-negative")
+        if chunk + ctx <= 1024:
+            raise ValueError(f"stream_pool: chunk_seconds + context_seconds is {chunk + ctx} samples, the length of a "
+                             "stream's first window; the front end reflect-pads 1024, so it needs at least 1025")
+        if max_windows is not None and (isinstance(max_windows, (bool, np.bool_))
+                                        or not isinstance(max_windows, numbers.Integral) or max_windows < 1):
+            raise ValueError(f"stream_pool: max_windows is {max_windows!r}; give a positive integer or None")
+        self._eng = engine
+        self._dev = device or f"cuda:{engine.device}"
+        self._cuda = torch.device(self._dev).type == "cuda"
+        self._sched = StreamSchedule(chunk, ctx)
+        self.window_len = L = self._sched.capacity
+        # a row of input and of output per window, and the resampler's output row (its staged input is smaller)
+        fit = engine.max_batch(L, extra_per_item=4 * 3 * L)
+        self.max_windows = fit if max_windows is None else min(int(max_windows), fit)
+        self.buckets = sorted({1 << k for k in range(self.max_windows.bit_length())} | {self.max_windows})
+        self._streams = {}
+        self._queue = deque()                      # (sid, window) of every stream, in the order they fell due
+        self._next_sid = 0
+        self._graphs = {}                          # bucket -> captured restore graph
+        self._bufs = None
+
+    # ------------------------------------------------------------------ the caller's side
+    def open(self, sample_rate=44100):
+        """Starts a stream whose blocks come at sample_rate Hz; returns its id."""
+        sid = self._next_sid
+        rate = resample.check_rate(sample_rate, f"stream_pool.open: stream {sid}")
+        self._next_sid += 1
+        self._streams[sid] = _Stream(rate)
+        return sid
+
+    def push(self, sid, block):
+        """Appends a 1-D block of any size, at the stream's own rate, to stream sid."""
+        s = self._open_stream(sid, "push")
+        a = np.asarray(block, dtype=np.float32)
+        if a.ndim != 1:
+            raise ValueError(f"stream_pool.push: stream {sid}: a block has shape {a.shape}; blocks are 1-D")
+        s.append(a)
+        self._schedule(sid, s, resample.available(s.n, s.rate), ended=False)
+
+    def close(self, sid):
+        """Marks the end of stream sid's input: its last windows fall due.  A stream of fewer than 1025 samples at
+        44.1 kHz raises restore_stream's RuntimeError, naming the stream, and is dropped; the other streams go on."""
+        s = self._open_stream(sid, "close")
+        try:
+            self._schedule(sid, s, resample.out_len(s.n, s.rate), ended=True)
+        except RuntimeError as e:
+            del self._streams[sid]
+            self._queue = deque(q for q in self._queue if q[0] != sid)
+            raise RuntimeError(f"stream_pool.close: stream {sid}: {e}") from None
+        s.closed = True
+
+    def step(self):
+        """Restores the due windows, oldest first, at most max_windows of them, in one graph replay; the rest wait for
+        the next step.  Returns {sid: [restored blocks, in order]} for the streams that had windows in this step.  A
+        stream that is closed and fully restored is forgotten afterwards."""
+        n = min(len(self._queue), self.max_windows)
+        batch = [self._queue.popleft() for _ in range(n)]
+        out = {}
+        if batch:
+            rows = self._run(batch)
+            for k, (sid, (lo, hi, keep_lo, keep_hi)) in enumerate(batch):
+                out.setdefault(sid, []).append(rows[k, keep_lo - lo:keep_hi - lo].copy())
+                self._streams[sid].pending.popleft()
+        for sid in [sid for sid, s in self._streams.items() if s.closed and not s.pending]:
+            del self._streams[sid]
+        for sid in out:
+            if sid in self._streams:
+                self._trim(self._streams[sid])
+        return out
+
+    @property
+    def streams(self):
+        """Ids of the streams the pool still holds: open ones, and closed ones with windows left to restore."""
+        return list(self._streams)
+
+    @property
+    def pending(self):
+        """Windows due and not yet restored, of all streams."""
+        return len(self._queue)
+
+    @property
+    def graph_count(self):
+        """Restore graphs captured so far (one per bucket used)."""
+        return len(self._graphs)
+
+    # ------------------------------------------------------------------ bookkeeping
+    def _open_stream(self, sid, what):
+        s = self._streams.get(sid)
+        if s is None:
+            raise ValueError(f"stream_pool.{what}: stream {sid!r} is not open in this pool (never opened, or closed and "
+                             "fully restored)")
+        if s.closed:
+            raise ValueError(f"stream_pool.{what}: stream {sid} is closed; its input has ended")
+        return s
+
+    def _schedule(self, sid, s, avail, ended):
+        windows, s.pos = self._sched.due(s.pos, avail, ended)
+        for w in windows:
+            s.pending.append(w)
+            self._queue.append((sid, w))
+        self._trim(s)
+
+    def _trim(self, s):
+        """Drops input that no window of s will read again: before its oldest pending window, and before the lowest
+        start a later window can have (a short flush window is widened by up to 1025 samples before pos - ctx)."""
+        keep = max(0, s.pos - self._sched.ctx - 1025)
+        if s.pending:
+            keep = min(keep, s.pending[0][0])
+        first, stop = resample.window(s.n, s.rate, keep, keep + 1)
+        if stop > first:
+            s.drop_before(first)
+
+    def bucket(self, n):
+        """The number of rows a step of n windows runs: the smallest bucket that holds them."""
+        return next(b for b in self.buckets if b >= n)
+
+    # ------------------------------------------------------------------ the launch
+    def _buffers(self):
+        """Input / output rows of the largest bucket, and one workspace that every bucket's graph shares (they replay
+        one at a time on one stream); each bucket's graph reads and writes row prefixes of them."""
+        if self._bufs is None:
+            B, L, dev = self.max_windows, self.window_len, self._dev
+            pin = (lambda t: t.pin_memory()) if self._cuda else (lambda t: t)
+            self._bufs = {"dev_in": torch.zeros((B, L), device=dev), "dev_out": torch.empty((B, L), device=dev),
+                          "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
+                          "host_in": pin(torch.zeros((B, L))), "host_out": pin(torch.empty((B, L))),
+                          "host_lens": pin(torch.empty(B, dtype=torch.int32)),
+                          "ws": torch.empty(self._eng.workspace_bytes(B, L), dtype=torch.uint8, device=dev)}
+        return self._bufs
+
+    def _run(self, batch):
+        """Restores the windows of batch [(sid, (lo, hi, keep_lo, keep_hi)), ...] and returns the output rows (host)."""
+        p = self._buffers()
+        n, B = len(batch), self.bucket(len(batch))
+        streams = [self._streams[sid] for sid, _ in batch]
+        lens = p["host_lens"]
+        lens[:B] = 1025                            # unused rows: any valid length; their output is never read
+        lens[:n] = torch.tensor([hi - lo for _, (lo, hi, _, _) in batch], dtype=torch.int32)
+        if any(s.rate != resample.RATE for s in streams):
+            x, lens_dev = self._eng.resample(*_stage([s.buf for s in streams], [s.rate for s in streams],
+                                                     [(k, w[0], w[1]) for k, (_, w) in enumerate(batch)], self._dev,
+                                                     extents=[(s.base, s.n) for s in streams]), self.window_len)
+            p["dev_in"][:n].copy_(x)
+            p["dev_lens"][n:B].copy_(lens[n:B], non_blocking=True)
+            p["dev_lens"][:n].copy_(lens_dev)
+        else:
+            hin = p["host_in"].numpy()
+            for k, (s, (_, (lo, hi, _, _))) in enumerate(zip(streams, batch)):
+                hin[k, :hi - lo] = s.buf[lo - s.base:hi - s.base]
+            p["dev_in"][:n].copy_(p["host_in"][:n], non_blocking=True)
+            p["dev_lens"][:B].copy_(lens[:B], non_blocking=True)
+        if B not in self._graphs:                  # captured once the lengths are staged: its warm-up runs read them
+            self._graphs[B] = self._eng.make_graph(p["dev_in"][:B], p["dev_out"][:B], mode=0, lens=p["dev_lens"][:B],
+                                                   ws=p["ws"])
+        self._graphs[B].replay()
+        p["host_out"][:n].copy_(p["dev_out"][:n], non_blocking=True)
+        if self._cuda:
+            torch.cuda.current_stream().synchronize()
+        return p["host_out"].numpy()
+
+
 class _ModelShim:
     """Stands in for `VoiceFixer._model` (the reference nn.Module): callers poke
     `.parameters()`, `.to()`, `.eval()`, `.train()` and `.vocoder` (test/streamlit.py:40-42)."""
@@ -308,15 +568,17 @@ def _drop_masks(drop_masks_fn, B, T):
     return masks
 
 
-def _stage(items, rates, segs, dev):
+def _stage(items, rates, segs, dev, extents=None):
     """The device resampler's input for output ranges segs = [(recording, a, b), ...] of the 44.1 kHz streams: each
     range's input window (resample.window), concatenated on the host and uploaded as one staging buffer, and the items
-    of Engine.resample."""
+    of Engine.resample.  extents (live streams, whose older input is dropped): one (base, n) per item, items[i] then
+    holding input samples [base, base + len(items[i])) of a recording of which n samples have arrived so far; without
+    it each item is a whole recording."""
     windows, table, off = [], [], 0
     for i, a, b in segs:
-        n = items[i].shape[0]
+        base, n = extents[i] if extents is not None else (0, items[i].shape[0])
         first, stop = resample.window(n, rates[i], a, b)
-        windows.append(items[i][first:stop])
+        windows.append(items[i][first - base:stop - base])
         table.append((rates[i], n, off, first, stop - first, a, b - a))
         off += stop - first
     return torch.from_numpy(np.concatenate(windows)).to(dev), table
@@ -607,6 +869,7 @@ class VoiceFixer:
             raise ValueError("chunk_seconds must be positive and context_seconds non-negative")
         eng = self._engine
         dev = f"cuda:{eng.device}"
+        sched = StreamSchedule(chunk, ctx)
         buf = np.zeros(0, dtype=np.float32)       # samples [base, base + len(buf)) of the stream
         base = 0                                  # stream index of buf[0]
         pos = 0                                   # next sample to emit
@@ -619,26 +882,24 @@ class VoiceFixer:
         for block in blocks:
             block = np.asarray(block, dtype=np.float32).reshape(-1)
             buf = np.concatenate([buf, block])
-            while base + len(buf) >= pos + chunk + ctx:                  # a full chunk plus its look-ahead has arrived
-                lo = max(0, pos - ctx)
-                yield run(lo, pos + chunk + ctx, pos, pos + chunk)
-                pos += chunk
-                drop = max(0, pos - ctx) - base                          # audio older than the next window's left context
-                if drop > 0:
-                    buf, base = buf[drop:], base + drop
-        end = base + len(buf)
-        while pos < end:                                                 # flush: the last windows have no (full) look-ahead
-            hi = min(end, pos + chunk + ctx)
-            keep_hi = min(end, pos + chunk)
-            if end - keep_hi <= 1024 and end - keep_hi > 0 and ctx == 0:  # never leave a tail the front end cannot pad
-                keep_hi = hi = end
-            lo = max(0, pos - ctx)
-            if hi - lo <= 1024:                                          # reflect padding needs > 1024 samples (base.py:78)
-                lo = max(0, hi - 1025 - ctx)
-                if hi - lo <= 1024:
-                    raise RuntimeError("restore_stream: fewer than 1025 samples in total; the front end reflect-pads 1024")
-            yield run(lo, hi, pos, keep_hi)
-            pos = keep_hi
+            windows, pos = sched.due(pos, base + len(buf), ended=False)
+            for w in windows:
+                yield run(*w)
+            drop = max(0, pos - ctx) - base                              # audio older than the next window's left context
+            if drop > 0:
+                buf, base = buf[drop:], base + drop
+        windows, pos = sched.due(pos, base + len(buf), ended=True)
+        for w in windows:
+            yield run(*w)
+
+    def stream_pool(self, chunk_seconds=2.0, context_seconds=1.0, max_windows=None):
+        """Extension: restore_stream for many live streams at once (StreamPool).  open() a stream per caller, push() its
+        blocks as they arrive, close() it at its end, and call step() to restore every window that is due, of every
+        stream, in one ragged CUDA-graph replay.  Each stream's output is bit-identical to restore_stream on that
+        stream's audio alone with the same chunk_seconds / context_seconds.  max_windows: the most windows one step
+        restores (default: as many as fit the device memory that is free, at most 64)."""
+        _check_cuda(False)
+        return StreamPool(self._engine, chunk_seconds, context_seconds, max_windows)
 
     def restore(self, input, output, cuda=False, mode=0, your_vocoder_func=None):
         wav_10k = self._load_wav(input, sample_rate=44100)               # base.py:141-146

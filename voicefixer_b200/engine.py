@@ -301,15 +301,22 @@ class Engine(_WorkspaceQueries):
                                         _stream()), "vfx_restore")
         return out
 
-    def make_graph(self, wav, out, mode=0, lens=None):
+    def make_graph(self, wav, out, mode=0, lens=None, ws=None):
         """Captures the whole restore() launch sequence (~360 kernels) for the given device buffers into a
         CUDA graph; returns an object whose .replay() re-runs it (inputs are read from `wav`, results land in
         `out`).  Shapes, buffers and the workspace are frozen into the graph.  With `lens` (ragged batch) the graph
-        reads the lengths from that buffer at every replay: refill it, like `wav`, before replay()."""
+        reads the lengths from that buffer at every replay: refill it, like `wav`, before replay().
+
+        ws (optional): a uint8 device workspace of at least workspace_bytes(*wav.shape) bytes for the graph to use, e.g.
+        one that several graphs share because they never replay at the same time; without it the graph gets its own."""
         assert wav.is_cuda and out.is_cuda and wav.shape == out.shape
-        # the graph bakes raw device pointers in: it gets its OWN workspace, and the returned object keeps every
-        # buffer it touches alive (a later, larger call may replace the engine's shared workspace)
-        ws = torch.empty(self.workspace_bytes(*wav.shape), dtype=torch.uint8, device=wav.device)
+        # the graph bakes raw device pointers in: it gets its OWN workspace unless given one, and the returned object keeps
+        # every buffer it touches alive (a later, larger call may replace the engine's shared workspace)
+        need = self.workspace_bytes(*wav.shape)
+        if ws is None:
+            ws = torch.empty(need, dtype=torch.uint8, device=wav.device)
+        elif not (ws.is_cuda and ws.dtype == torch.uint8 and ws.numel() >= need):
+            raise ValueError(f"make_graph: ws must be a uint8 CUDA tensor of at least {need} bytes")
         side = torch.cuda.Stream(device=wav.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                                # warm-up: one-time attribute / table setup

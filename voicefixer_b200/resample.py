@@ -55,6 +55,17 @@ def out_len(n_in, rate):
     return -(-int(n_in) * up // down)
 
 
+def available(n_in, rate):
+    """Samples at 44.1 kHz that the first n_in input samples of a recording still arriving determine: the prefix [0, m)
+    whose window(n, rate, 0, m) ends at or before n_in for every n >= n_in, i.e. every output whose last input,
+    (j + rem) * down // up, has arrived.  That is out_len(n_in, rate) - rem (at least 0), and n_in for a copy; once the
+    recording has ended, all out_len(n_in, rate) samples are determined."""
+    up, down = ratio(rate)
+    if up == down == 1:
+        return int(n_in)
+    return max(0, out_len(n_in, rate) - taps(rate)[1])
+
+
 def window(n_in, rate, a, b):
     """(first, stop): the inputs [first, stop) that output samples [a, b) read, clipped to [0, n_in).  Empty (first ==
     stop) when b <= a or no input contributes."""
@@ -82,11 +93,14 @@ def rates(sample_rate, n, what):
             raise ValueError(f"{what}: sample_rate has {len(rs)} entries for {n} recordings; give one rate, or one per recording")
     else:
         rs = [sample_rate] * n
-    for i, r in enumerate(rs):
-        if isinstance(r, (bool, np.bool_)) or not isinstance(r, numbers.Integral) or not 0 < r <= MAX_RATE:
-            raise ValueError(f"{what}: recording {i} has sample_rate {r!r}; a sample rate is a positive integer number of "
-                             f"Hz (at most {MAX_RATE})")
-    return [int(r) for r in rs]
+    return [check_rate(r, f"{what}: recording {i}") for i, r in enumerate(rs)]
+
+
+def check_rate(r, who):
+    """r as an int if it is a valid sample rate; else raises ValueError `<who> has sample_rate ...`."""
+    if isinstance(r, (bool, np.bool_)) or not isinstance(r, numbers.Integral) or not 0 < r <= MAX_RATE:
+        raise ValueError(f"{who} has sample_rate {r!r}; a sample rate is a positive integer number of Hz (at most {MAX_RATE})")
+    return int(r)
 
 
 def staging_bound(L, rate):
