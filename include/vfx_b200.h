@@ -70,6 +70,9 @@ int vfx_engine_set_tensor(vfx_engine* e, const char* name, const void* dev_ptr, 
 int vfx_engine_set_option(vfx_engine* e, const char* key, int value);
 /* Number of CUDA kernels this library has launched in this process (bench.py's gpu_launches). */
 unsigned long long vfx_launch_count(void);
+/* How many of them were tensor-core convolutions whose operands were staged by TMA (launches without per-item extents
+ * whose operands a tensor map can express, DESIGN.md §4.1); the others were staged with cp.async. */
+unsigned long long vfx_conv_tma_launch_count(void);
 /* With option "profile" = 1 every launch group is bracketed by CUDA events on the call's stream;
  * this synchronises, writes one line per tag "tag count total_ms flops bytes" and clears the log. */
 int vfx_profile_report(vfx_engine* e, char* buf, size_t cap);

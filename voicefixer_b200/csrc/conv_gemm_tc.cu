@@ -5,11 +5,18 @@
 //
 // Persistent, warp-specialised kernel: grid = min(tiles, SMs), each CTA walks a static stride over the 128 x BN output
 // tiles in N-fastest order (the N tiles of one M tile run together, so their A rows come from HBM about once).
-//  - Producer warpgroup (56 registers): for every K slice (tap, 128-byte channel slice) it stages 16-byte chunks of the
-//    shifted input rows and of the tap's weight rows with cp.async into a ring of 128-byte-swizzled K-major tiles;
-//    chunks outside the input (convolution padding), beyond Cin or beyond N are zero-filled by the copy itself, so any
-//    tap offset, stride and edge is handled without a separate padded tensor.  Stages are handed over through full /
-//    empty mbarriers; it fills the ring for the next tile while the consumers run the epilogue.
+//  - Producer: for every K slice (tap, 128-byte channel slice) the shifted input rows and the tap's weight rows go into
+//    a ring of 128-byte-swizzled K-major tiles; whatever lies outside the input (convolution padding), beyond Cin or
+//    beyond N arrives as zeros, so any tap offset, stride and edge is handled without a separate padded tensor.  Stages
+//    are handed over through full / empty mbarriers; the ring is filled for the next tile while the consumers run the
+//    epilogue.  Two forms (TMA below):
+//      TMA: one thread issues two tensor-map loads per slice, a box of the [B][H][W][Cin] input at the tile's origin plus
+//      the tap's offset and a box of the weights; the out-of-bounds fill of the maps supplies the zeros and the loads
+//      themselves complete the stage's full barrier.  A box is a rectangle of one tensor, so an M tile is a rectangle of
+//      the output grid (TmaPlan) and not 128 consecutive rows of the flattened one.
+//      cp.async: the producer warpgroup (56 registers) stages 16-byte chunks with zero-fill copies from a per-tile row
+//      table.  It serves the launches a tensor map cannot express: ragged batches, whose zeros depend on the item, and
+//      operands whose strides or weight offsets the maps do not take (tma_plan).
 //  - Two consumer warpgroups (224 registers), 64 rows each: one m64nBN wgmma group in flight per warpgroup, into one of
 //    two partial accumulators, while the previous slice's partial is added to the fp32 accumulator.
 //  - Staged epilogue: the tile goes through a shared fp32 buffer and is processed row by row (bias, fp32 residual,
@@ -20,10 +27,11 @@
 // Ragged batches (seq_in / seq_out): each item's extent on the sequence axis acts as that item's own edge, so every row
 // inside it is computed from the same operands as with the item alone; a tile none of whose rows is stored is skipped.
 //
-// What still stands between this kernel and the roof: the producer recomputes and issues every 16-byte chunk with
-// cp.async (no TMA), the A halo of the taps is re-read from L2 for every tap, and the per-slice sum costs BN / 2 FADDs
-// per slice in the consumers.
+// What still stands between this kernel and the roof: the A halo of the taps is re-read from L2 for every tap, every
+// CTA reads its own copy of the weights from L2, the ring is 4 stages deep at BN = 128 (the fp32 epilogue buffer takes
+// the rest of shared memory), and the per-slice sum costs BN / 2 FADDs per slice in the consumers.
 #include <atomic>
+#include <cuda.h>      // CUtensorMap and the types of its encoder; the encoder itself is looked up at run time
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -44,17 +52,32 @@ template <> struct OpT<2> { using T = __half; static constexpr int ESZ = 2; };
 // epilogue offsets of one tile row (ok == 0: the row is not stored)
 struct OutRow { long long raw, act, res; int ok; };
 
-template <int BN> struct Cfg {
+// What a TMA launch carries beside the descriptor.  An M tile is the box of tw x th x tb output-grid positions
+// (qw, qh, b) at a multiple of the box: a whole number of lines, or a piece of one line, of one item, or whole items,
+// so that its input rows are one box of the input tensor.  Tile row r is position (r % tw, r / tw % th, r / (tw th));
+// rows from tw th tb on do not exist (their shared memory is not written and their results are not stored).
+struct TmaPlan {
+  CUtensorMap a;           // input  (Cin, W, H, B),    box (128 bytes, tw, th, tb)
+  CUtensorMap w;           // weights (Cin, N, groups), box (128 bytes, BN, 1): tap t is group wtap[t]
+  int tw, th, tb;
+  int ntw, nth, mtiles;    // boxes per line, per item's lines, in all
+  int wtap[9];
+};
+
+template <int BN, bool TMA> struct Cfg {
   static constexpr int STAGE = A_BYTES + BN * 128;
   static constexpr int EPI_LD = BN + 8;            // fp32 words per epilogue row; +8 keeps the fragment stores conflict-free
   static constexpr int EPI = BM * EPI_LD * 4;
-  static constexpr int ROWS = BM * 24 + BM * (int)sizeof(OutRow);   // producer and epilogue row tables
+  static constexpr int PROWS = TMA ? 0 : BM * 24;  // the cp.async producer's row table
+  static constexpr int ROWS = PROWS + BM * (int)sizeof(OutRow);     // + the epilogue's
   static constexpr int FIXED = 1024 + EPI + ROWS;  // + 1024: alignment of the ring
   static constexpr int FIT = (SMEM_MAX - FIXED) / (STAGE + 16);
   static constexpr int STAGES = FIT < 8 ? FIT : 8;                  // 4 at BN = 128, 7 at 64, 8 at 32
-  // The producer signals slice k full after issuing slice k + AHEAD (cp.async.wait_group AHEAD).  It must wait for an
-  // empty slot before issuing, and the consumers free slot k - 1 only once slice k is full, so AHEAD <= STAGES - 2:
+  // cp.async: the producer signals slice k full after issuing slice k + AHEAD (cp.async.wait_group AHEAD).  It must wait
+  // for an empty slot before issuing, and the consumers free slot k - 1 only once slice k is full, so AHEAD <= STAGES - 2:
   // with more, the producer waits for a slot the consumers can only free after a signal it has not sent yet.
+  // TMA has no such rule: a slice's full barrier is completed by its loads, whatever the issuing thread does next, so
+  // that thread may block on the empty barrier of the oldest stage with every other stage in flight.
   static constexpr int AHEAD = STAGES - 2;
   static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
   static_assert(STAGES >= 3 && SMEM <= SMEM_MAX, "conv_gemm_tc: shared-memory plan");
@@ -67,6 +90,16 @@ __device__ __forceinline__ bool grid_row(const vfx_conv_desc& d, int M, int m, i
   const int r = m / d.Wq;
   qh = r % d.Hq; b = r / d.Hq;
   return true;
+}
+// row r of M tile mt -> item b and grid position (qh, qw); false where the tile has no such row
+template <bool TMA>
+__device__ __forceinline__ bool tile_row(const vfx_conv_desc& d, const TmaPlan& tp, int M, int mt, int r, int& b, int& qh, int& qw) {
+  if (!TMA) return grid_row(d, M, mt * BM + r, b, qh, qw);
+  const int j = r / tp.tw, u = mt / tp.ntw;
+  qw = mt % tp.ntw * tp.tw + r % tp.tw;
+  qh = u % tp.nth * tp.th + j % tp.th;
+  b = u / tp.nth * tp.tb + j / tp.th;
+  return j / tp.th < tp.tb && qw < d.Wq && qh < d.Hq && b < d.B;
 }
 // whether grid position (b, qh, qw) is stored: inside the output and, in a ragged batch, inside its item's extent.
 // The producer and the consumers both decide a tile's skip from this function alone, so they walk the same tiles.
@@ -88,28 +121,34 @@ __device__ __forceinline__ float act_out(const vfx_conv_desc& d, float v, int n)
   return apply_act(va, d.act, d.act_param);
 }
 
-// SEQ: the descriptor carries per-item extents (seq_in / seq_out); without them the kernel is compiled without the checks.
+// TMA: the operands arrive through the tensor maps of `tp` and the M tiles are its boxes; otherwise through cp.async
+// with 128 consecutive rows of the flattened output grid per M tile, `tp` unused, and the per-item extents
+// (seq_in / seq_out) honoured where the descriptor carries them.
 // vec: every output / residual pointer, stride and column offset allows 4-column vector accesses.
-template <int BN, int KIND, bool SEQ>
-__global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d, const int nkc,
+template <int BN, int KIND, bool TMA>
+__global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d,
+                                                                 const __grid_constant__ TmaPlan tp, const int nkc,
                                                                  const int vec) {
   using T = typename OpT<KIND>::T;
-  using C = Cfg<BN>;
+  using C = Cfg<BN, TMA>;
+  constexpr bool SEQ = !TMA;
   constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
   constexpr int S = C::STAGES, STAGE = C::STAGE, AHEAD = C::AHEAD;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* const gbase = smem_raw + (sbase - smem_u32(smem_raw));
   float* const epi = reinterpret_cast<float*>(gbase + S * STAGE);
-  int4* const prow = reinterpret_cast<int4*>(gbase + S * STAGE + C::EPI);
+  int4* const prow = reinterpret_cast<int4*>(gbase + S * STAGE + C::EPI);        // (cp.async producer only)
   long long* const pbase = reinterpret_cast<long long*>(prow + BM);
-  OutRow* const crow = reinterpret_cast<OutRow*>(pbase + BM);
+  OutRow* const crow = reinterpret_cast<OutRow*>(gbase + S * STAGE + C::EPI + C::PROWS);
   const uint32_t full0 = sbase + S * STAGE + C::EPI + C::ROWS, empty0 = full0 + 8 * S;
 
   const int tid = threadIdx.x;
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
-      mbar_init(full0 + 8 * s, 128);    // every producer thread, after its own copies of the stage have landed
+      // full: the issuing thread's expect_tx plus the bytes of the stage's two loads (TMA), or every producer thread
+      // after its own copies of the stage have landed
+      mbar_init(full0 + 8 * s, TMA ? 1 : 128);
       mbar_init(empty0 + 8 * s, 8);     // every consumer warp, after its wgmma group has read the stage
     }
   }
@@ -118,13 +157,34 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
   // derived after each role's setmaxnreg, so that nothing stays live across it
 #define VFX_TILE_WALK                                                                                              \
   const int M = d.B * d.Hq * d.Wq;                 /* < 2^31, and so is the tile count (conv_gemm_tc) */           \
-  const int ntn = (d.N + BN - 1) / BN, ntiles = (M + BM - 1) / BM * ntn, niter = d.ntaps * nkc;                    \
+  const int ntn = (d.N + BN - 1) / BN, ntiles = (TMA ? tp.mtiles : (M + BM - 1) / BM) * ntn, niter = d.ntaps * nkc; \
   const bool skips = SEQ && d.seq_out;
 
   if (tid < 128) {
     // ================================================================ producer
     setmaxnreg_dec<PROD_REGS>();
     VFX_TILE_WALK
+    if constexpr (TMA) {
+      if (tid != 0) return;
+      const uint32_t bytes = (uint32_t)(tp.tw * tp.th * tp.tb * 128 + BN * 128);   // of one stage: whole boxes, zeros included
+      uint32_t k = 0;                                 // K slices issued by this CTA
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int mt = t / ntn, u = mt / tp.ntw;
+        const int n0 = t % ntn * BN;
+        const int w0 = mt % tp.ntw * tp.tw, h0 = u % tp.nth * tp.th, b0 = u / tp.nth * tp.tb;
+        for (int it = 0; it < niter; ++it, ++k) {
+          const int s = k % S;
+          if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+          const int tap = it / nkc;
+          const int c = (it - tap * nkc) * BK;
+          const uint32_t sa = sbase + s * STAGE, full = full0 + 8 * s;
+          mbar_expect_tx(full, bytes);
+          tma_load_4d(sa, &tp.a, full, c, w0 + d.dw[tap], h0 + d.dh[tap], b0);
+          tma_load_3d(sa + A_BYTES, &tp.w, full, c, n0, tp.wtap[tap]);
+        }
+      }
+      return;
+    }
     // this thread's staging work: chunk `chunk` of A rows lrow + 16 i and of B rows lrow + 16 i
     const int chunk = tid & 7, lrow = tid >> 3;
     uint32_t k = 0;                                   // K slices issued by this CTA
@@ -222,11 +282,11 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
 
   uint32_t k = 0;                                     // K slices consumed by this CTA
   for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-    const int m0 = t / ntn * BM;
+    const int mt = t / ntn;
     const int n0 = t % ntn * BN;
     if (skips) {
       int b, qh, qw;
-      const bool live = grid_row(d, M, m0 + (ct & 127), b, qh, qw) && row_stored<SEQ>(d, b, qh, qw);
+      const bool live = tile_row<TMA>(d, tp, M, mt, ct & 127, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw);
       if (!named_sync_or(2, 256, live)) continue;
     }
 #pragma unroll
@@ -267,7 +327,7 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
     if (ct < BM) {
       OutRow o{0, 0, 0, 0};
       int b, qh, qw;
-      if (grid_row(d, M, m0 + ct, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw)) {
+      if (tile_row<TMA>(d, tp, M, mt, ct, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw)) {
         const int oh = qh * d.sh + d.rh, ow = qw * d.sw + d.rw;
         o.raw = (long long)b * d.o_sB + (long long)oh * d.o_sH + (long long)ow * d.o_sW + d.o_col;
         o.act = (long long)b * d.oa_sB + (long long)oh * d.oa_sH + (long long)ow * d.oa_sW + d.oa_col;
@@ -327,37 +387,124 @@ int sm_count(int dev) {
   return n;
 }
 
-template <int BN, int KIND, bool SEQ>
-int launch(const vfx_conv_desc& d, int vec, cudaStream_t st) {
-  constexpr int smem = Cfg<BN>::SMEM;
+// cuTensorMapEncodeTiled, through the runtime (the library calls nothing else of the driver API)
+using EncodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiled tensor_map_encoder() {
+  static const EncodeTiled fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      p = nullptr;
+    return reinterpret_cast<EncodeTiled>(p);
+  }();
+  return fn;
+}
+
+// The tile boxes and the two tensor maps of a launch without per-item extents.  Returns 1 with `tp` filled, 0 where a
+// tensor map cannot express the operands (the launch then takes the cp.async producer), or an error.
+// Input: dimensions (Cin, W, H, B) with the descriptor's strides; the out-of-bounds fill of a box at the tile's origin
+// plus the tap's offset is the zero padding on every side, at any dilation (coordinates are 32-bit and may lie wholly
+// outside), the Cin tail of the last channel slice and the rows of a partial tile.
+// Weights: the taps' [N][Cin] matrices start at arbitrary offsets (the ConvTranspose phase groups use some taps of a
+// larger array), so the third dimension counts in units of the greatest common divisor of the offsets' differences,
+// from the lowest offset.  Rows n >= N of a box are then zeros, not the next matrix.
+int tma_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
+  const long long esz = (long long)prec_esz(precision), LIM = 1LL << 40;          // tensor-map strides are below 2^40 bytes
+  if (d.W <= 0 || d.H <= 0) return 0;
+  // ---- tiles: a piece of a line, else whole lines of an item, else whole items
+  tp.tw = d.Wq < BM ? d.Wq : BM;
+  tp.th = tp.tw < d.Wq ? 1 : (d.Hq < BM / tp.tw ? d.Hq : BM / tp.tw);
+  tp.tb = tp.th < d.Hq || tp.tw < d.Wq ? 1 : (d.B < BM / (tp.tw * tp.th) ? d.B : BM / (tp.tw * tp.th));
+  tp.ntw = ceil_div(d.Wq, tp.tw);
+  tp.nth = ceil_div(d.Hq, tp.th);
+  const long long mtiles = (long long)tp.ntw * tp.nth * ceil_div(d.B, tp.tb);
+  if (mtiles >= (1LL << 31) / BM) return 0;
+  tp.mtiles = (int)mtiles;
+  // ---- input map; the stride of a dimension of size 1 is never used: it takes the dense one, whatever the descriptor says
+  const cuuint64_t adim[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.B};
+  const long long asrc[3] = {d.a_sW, d.a_sH, d.a_sB};
+  cuuint64_t astr[3];
+  long long dense = d.Cin * esz;
+  for (int i = 0; i < 3; ++i) {
+    const long long s = adim[i + 1] > 1 ? asrc[i] * esz : dense;
+    if (s <= 0 || s >= LIM || s % 16) return 0;
+    astr[i] = (cuuint64_t)s;
+    dense = s < LIM / (long long)adim[i + 1] ? s * (long long)adim[i + 1] : LIM;
+  }
+  // ---- weight map
+  long long lo = d.w_off[0], g = 0;
+  for (int t = 1; t < d.ntaps; ++t) lo = d.w_off[t] < lo ? d.w_off[t] : lo;
+  for (int t = 0; t < d.ntaps; ++t)
+    for (long long a = d.w_off[t] - lo; a;) { const long long r = g % a; g = a; a = r; }
+  const long long mat = (long long)d.N * d.Cin;
+  if (g == 0) g = mat;                              // one matrix
+  if (lo < 0 || g < mat || g * esz >= LIM) return 0;   // matrices that overlap are left to cp.async
+  long long groups = 1;
+  for (int t = 0; t < d.ntaps; ++t) {
+    tp.wtap[t] = (int)((d.w_off[t] - lo) / g);
+    groups = tp.wtap[t] + 1 > groups ? tp.wtap[t] + 1 : groups;
+  }
+  const cuuint64_t wdim[3] = {(cuuint64_t)d.Cin, (cuuint64_t)d.N, (cuuint64_t)groups};
+  const cuuint64_t wstr[2] = {(cuuint64_t)(d.Cin * esz), (cuuint64_t)(g * esz)};
+  // ---- encode
+  const EncodeTiled encode = tensor_map_encoder();
+  VFX_REQUIRE(encode, "conv_gemm_tc: this CUDA driver has no cuTensorMapEncodeTiled");
+  const CUtensorMapDataType dt = precision == VFX_PREC_TF32   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                              : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const cuuint32_t bk = (cuuint32_t)(128 / esz), ones[4] = {1, 1, 1, 1};
+  const cuuint32_t abox[4] = {bk, (cuuint32_t)tp.tw, (cuuint32_t)tp.th, (cuuint32_t)tp.tb}, wbox[3] = {bk, (cuuint32_t)bn, 1};
+  CUresult r = encode(&tp.a, dt, 4, const_cast<void*>(d.a), adim, astr, abox, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  VFX_REQUIRE(r == CUDA_SUCCESS, "conv_gemm_tc: input tensor map refused (CUresult %d)", (int)r);
+  r = encode(&tp.w, dt, 3, const_cast<char*>(static_cast<const char*>(d.w)) + lo * esz, wdim, wstr, wbox, ones,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  VFX_REQUIRE(r == CUDA_SUCCESS, "conv_gemm_tc: weight tensor map refused (CUresult %d)", (int)r);
+  return 1;
+}
+
+template <int BN, int KIND, bool TMA>
+int launch(const vfx_conv_desc& d, const TmaPlan& tp, int vec, cudaStream_t st) {
+  constexpr int smem = Cfg<BN, TMA>::SMEM;
   static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
   int dev = 0;
   VFX_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, SEQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     if (dev < 64) attr_set |= 1ull << dev;
   }
   const int sms = sm_count(dev);
   VFX_REQUIRE(sms > 0, "conv_gemm_tc: cannot read the SM count of device %d", dev);
   const int nkc = ceil_div(d.Cin, 128 / OpT<KIND>::ESZ);
-  const long long tiles = ((long long)d.B * d.Hq * d.Wq + BM - 1) / BM * ceil_div(d.N, BN);
+  const long long mtiles = TMA ? tp.mtiles : ((long long)d.B * d.Hq * d.Wq + BM - 1) / BM;
+  const long long tiles = mtiles * ceil_div(d.N, BN);
   const int grid = (int)(tiles < sms ? tiles : sms);
   if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
-  conv_gemm_wgmma_kernel<BN, KIND, SEQ><<<grid, NT, smem, st>>>(d, nkc, vec);
+  conv_gemm_wgmma_kernel<BN, KIND, TMA><<<grid, NT, smem, st>>>(d, tp, nkc, vec);
   VFX_LAUNCH_CHECK();
+  if (TMA) ++g_conv_tma_launches;
   return VFX_OK;
 }
 
-template <int KIND, bool SEQ>
-int launch_n(const vfx_conv_desc& d, int vec, cudaStream_t st) {
-  if (d.N <= 32) return launch<32, KIND, SEQ>(d, vec, st);
-  if (d.N <= 64) return launch<64, KIND, SEQ>(d, vec, st);
-  return launch<128, KIND, SEQ>(d, vec, st);
+// Launches without per-item extents go through TMA where tma_plan can express them.  The cp.async instantiation reads
+// the extents only where the descriptor has them, so it also runs the others.
+template <int BN, int KIND>
+int launch_bn(int precision, const vfx_conv_desc& d, int vec, cudaStream_t st) {
+  TmaPlan tp{};
+  int tma = 0;
+  if (!d.seq_in && !d.seq_out && (tma = tma_plan(precision, d, BN, tp)) < 0) return tma;
+  return tma ? launch<BN, KIND, true>(d, tp, vec, st) : launch<BN, KIND, false>(d, tp, vec, st);
 }
 
 template <int KIND>
-int launch_kind(const vfx_conv_desc& d, int vec, cudaStream_t st) {
-  return (d.seq_in || d.seq_out) ? launch_n<KIND, true>(d, vec, st) : launch_n<KIND, false>(d, vec, st);
+int launch_kind(int precision, const vfx_conv_desc& d, int vec, cudaStream_t st) {
+  if (d.N <= 32) return launch_bn<32, KIND>(precision, d, vec, st);
+  if (d.N <= 64) return launch_bn<64, KIND>(precision, d, vec, st);
+  return launch_bn<128, KIND>(precision, d, vec, st);
 }
 
 // 4 consecutive columns of every output row start 4 * esz-aligned (16 B for fp32)
@@ -387,9 +534,9 @@ int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st) {
   const int vec = vec_ok(d.out_raw, 4, d.o_sB, d.o_sH, d.o_sW, d.o_col) &&
                   vec_ok(d.out_act, esz, d.oa_sB, d.oa_sH, d.oa_sW, d.oa_col) &&
                   vec_ok(d.residual, 4, d.r_sB, d.r_sH, d.r_sW, d.r_col);
-  if (precision == VFX_PREC_TF32) return launch_kind<0>(d, vec, st);
-  if (precision == VFX_PREC_BF16) return launch_kind<1>(d, vec, st);
-  return launch_kind<2>(d, vec, st);
+  if (precision == VFX_PREC_TF32) return launch_kind<0>(precision, d, vec, st);
+  if (precision == VFX_PREC_BF16) return launch_kind<1>(precision, d, vec, st);
+  return launch_kind<2>(precision, d, vec, st);
 }
 
 }  // namespace vfx

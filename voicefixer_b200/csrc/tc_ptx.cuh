@@ -1,6 +1,6 @@
-// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu): cp.async operand staging with zero fill,
-// the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups and the shared-memory
-// matrix descriptor.
+// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu): TMA tile loads, cp.async operand staging with zero
+// fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups and the
+// shared-memory matrix descriptor.
 #pragma once
 #include "vfx_common.cuh"
 
@@ -30,6 +30,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!done)
     asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
                  : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+}
+// TMA operand staging: one thread arms the stage's full barrier with the bytes to come, then issues the tile loads.  Each
+// load writes its whole box (elements outside the tensor as zeros) through the async proxy, in the swizzle of the tensor
+// map, and completes that many bytes on the barrier; wgmma reads through the same proxy, so no fence lies between them.
+// `map` is the address of a CUtensorMap in a __grid_constant__ kernel parameter; coordinates are innermost first.
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+               ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* map, uint32_t bar, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+               ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 // named barriers over a subset of the CTA's warps (id 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int nthreads) {

@@ -23,6 +23,7 @@ void set_error(const char* fmt, ...);
   } while (0)
 
 extern unsigned long long g_launches;   // kernels launched by this library (bench.py's gpu_launches)
+extern unsigned long long g_conv_tma_launches;   // those of them that were conv_gemm_tc launches fed by TMA
 #define VFX_LAUNCH_CHECK()                                                            \
   do { ++vfx::g_launches; VFX_CUDA_CHECK(cudaGetLastError()); } while (0)
 
