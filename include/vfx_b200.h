@@ -63,10 +63,8 @@ int vfx_engine_set_tensor(vfx_engine* e, const char* name, const void* dev_ptr, 
 /* Engine options: "use_tc" (BF16 / FP16 / TF32; 1 = wgmma kernel [default], 0 = SIMT cross-check on the same operands),
  * "profile" (0/1/2, see vfx_profile_report; 2 = one tag per shape / dilation),
  * "tf32_stream" (TF32: vocoder residual streams as one encoded tensor, vfx_conv_desc.res_enc / raw_enc, default 1),
- * "fuse_pair" (BF16 / FP16: width-64 ResStack pairs as one fused kernel, default 1),
- * "fuse_pair3" (TF32: width-64 ResStack pairs as one fused kernel on the encoded stream, default 1),
- * "fuse_pair2" (1 [default] = BF16 / FP16 width-128 ResStack pairs fused, 2 = also TF32 width 64 when "fuse_pair3" is 0,
- *  0 = off). */
+ * "fuse_pairs" (1 [default] = every ResStack pair vfx_resstack_pair supports runs as one fused kernel, 0 = every pair as
+ *  its two convolutions; the switch that compares the fused kernel against the two-launch path). */
 int vfx_engine_set_option(vfx_engine* e, const char* key, int value);
 /* Number of CUDA kernels this library has launched in this process (bench.py's gpu_launches). */
 unsigned long long vfx_launch_count(void);
@@ -278,13 +276,17 @@ int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream)
 /* Fused ResStack pair on the wgmma tensor cores:
  *   x' = x + conv2_{k3,d=1}( lrelu_0.01( conv1_{k3,dilation}( a ) + b1 ) ) + b2
  * ResStack.forward voicefixer/vocoder/model/modules.py:592-595 (layers :550-576).
- * impl: 0, 1 or 3 = one kernel, the intermediate h kept in shared memory (no scratch needed); 2 = the two convolutions per
- * block of rows with h in `scratch` (required for impl 2: vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned).
+ * form: VFX_PAIR_FUSED = one kernel on one SM per block of rows, the intermediate h kept in shared memory (no scratch);
+ * VFX_PAIR_BLOCKED = the two convolutions of vfx_conv_gemm per block of rows with h in `scratch` (required:
+ * vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned), the reference the fused form is tested against.  Any other
+ * form returns VFX_ERR_INVALID.
  *   VFX_PREC_BF16 / VFX_PREC_FP16, C = 64 or 128: a = lrelu_0.01(x) in the operand format [B][L][C]; x fp32 is read as the residual
  *     and, if write_raw, overwritten with x' (or written to x_out); out_act (optional, operand format, must not alias a) receives act(x').
  *   VFX_PREC_TF32, C = 64, stream_enc = 1: a == x == the encoded stream S (vfx_conv_desc.raw_enc), fp32 [B][L][C];
  *     the result goes to x_out (required, aliasing neither input) as S' (stream_enc_out = 1) or as plain x' (0).
- * w1 / w2: [3][C][C] in the operand format, tap-major.  Other shapes return VFX_ERR_UNSUPPORTED. */
+ * w1 / w2: [3][C][C] in the operand format, tap-major.  Other precisions (VFX_PREC_FP32) and shapes return
+ * VFX_ERR_UNSUPPORTED. */
+enum vfx_pair_form { VFX_PAIR_FUSED = 0, VFX_PAIR_BLOCKED = 1 };
 typedef struct vfx_pair_desc {
   const void* a;
   float* x;
@@ -293,14 +295,15 @@ typedef struct vfx_pair_desc {
   int B, L, C;
   int write_raw;
   void* out_act; int act; float act_param;
-  int precision;            /* vfx_precision: VFX_PREC_BF16 (0 is read as BF16 for compatibility), VFX_PREC_FP16 or VFX_PREC_TF32 */
-  int impl;                 /* see above */
+  int precision;            /* vfx_precision: VFX_PREC_BF16, VFX_PREC_FP16 or VFX_PREC_TF32 */
+  int form;                 /* vfx_pair_form; 0 (a zeroed descriptor) is the fused kernel */
   float* x_out;             /* NULL = in place over x (16-bit modes only) */
   int stream_enc, stream_enc_out;
-  void* scratch;            /* impl 2: device scratch of vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned: holds h */
+  void* scratch;            /* VFX_PAIR_BLOCKED: device scratch of vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned: holds h */
   size_t scratch_bytes;
   const int* lens;          /* optional per-item length (<= L; L stays the item stride): rows >= lens[b] read as zero and are not
-                             * written, as if item b had length lens[b].  NULL = every item has length L.  impl 2 refuses it. */
+                             * written, as if item b had length lens[b].  NULL = every item has length L.  VFX_PAIR_BLOCKED
+                             * refuses it with VFX_ERR_UNSUPPORTED. */
 } vfx_pair_desc;
 size_t vfx_resstack_pair_scratch_bytes(void);
 int vfx_resstack_pair(const vfx_pair_desc* d, void* stream);

@@ -157,9 +157,9 @@ def test_accumulation_is_unbiased(shape, prec, record_property):
 _SCRATCH = {}
 
 
-def _pair(prec, impl, a, x, w1, b1, w2, b2, dil, write_raw=1, out_act=None, act="lrelu", act_param=0.01, x_out=None,
+def _pair(prec, form, a, x, w1, b1, w2, b2, dil, write_raw=1, out_act=None, act="lrelu", act_param=0.01, x_out=None,
           stream_enc=0, stream_enc_out=0):
-    """vfx_resstack_pair; weights [3][C][C] (tap, out, in)"""
+    """vfx_resstack_pair in form "fused" or "blocked"; weights [3][C][C] (tap, out, in)"""
     from voicefixer_b200 import _lib
     lib = _lib.load()
     B, L, C = x.shape
@@ -169,10 +169,10 @@ def _pair(prec, impl, a, x, w1, b1, w2, b2, dil, write_raw=1, out_act=None, act=
     d.B, d.L, d.C, d.write_raw = B, L, C, write_raw
     d.out_act = None if out_act is None else out_act.data_ptr()
     d.act, d.act_param = _lib.ACT[act], act_param
-    d.precision, d.impl = _lib.PREC[prec], impl
+    d.precision, d.form = _lib.PREC[prec], _lib.PAIR_FORM[form]
     d.x_out = None if x_out is None else x_out.data_ptr()
     d.stream_enc, d.stream_enc_out = stream_enc, stream_enc_out
-    if impl == 2:
+    if form == "blocked":
         n = int(lib.vfx_resstack_pair_scratch_bytes())
         if "buf" not in _SCRATCH:
             _SCRATCH["buf"] = torch.empty(n, dtype=torch.uint8, device=DEV)
@@ -229,14 +229,14 @@ def _act64(z, act, p):
 @pytest.mark.parametrize("dil", [1, 3, 243, 2187])
 @pytest.mark.parametrize("L", [1, 125, 126, 127, 252, 253, 1000, 20000])
 def test_pair128_fused(L, dil, B, prec, record_property):
-    """Width 128, the one-kernel form (impl 0): tile edges at 126 rows, dilations up to beyond L, in place.  Measured
-    on the H100: the update within 1.2e-7 .. 1.5e-7 relative RMS of float64."""
+    """Width 128, the fused form: tile edges at 126 rows, dilations up to beyond L, in place.  Measured on the H100:
+    the update within 1.2e-7 .. 1.5e-7 relative RMS of float64."""
     C = 128
     a, x, w1, b1, w2, b2 = _pair_operands(B, L, C, prec, seed=L * 7 + dil * 3 + B)
     ref = _pair_ref(a, x, w1, b1, w2, b2, dil, prec)
     xin = x.clone()
     act = torch.full((B, L, C), SENT, dtype=DT[prec], device=DEV)
-    _pair(prec, 0, a, xin, w1, b1, w2, b2, dil, out_act=act)
+    _pair(prec, "fused", a, xin, w1, b1, w2, b2, dil, out_act=act)
     x64 = x.to(F64)
     err = _rel(xin.to(F64) - x64, ref - x64)              # the update itself, not masked by the residual
     record_property("raw_rel_rms", err)
@@ -260,8 +260,8 @@ def test_pair128_output_variants(prec, write_raw, act, dest, record_property):
     xout = torch.full_like(x, SENT) if dest == "x_out" else None
     out_act = None if act is None else torch.full((B, L, C), SENT, dtype=DT[prec], device=DEV)
     p = {"lrelu": 0.01, "lrelu_xsinx": 0.2}.get(act, 0.0)
-    _pair(prec, 0, a, xin, w1, b1, w2, b2, dil, write_raw=write_raw, out_act=out_act, act=act or "none", act_param=p,
-          x_out=xout)
+    _pair(prec, "fused", a, xin, w1, b1, w2, b2, dil, write_raw=write_raw, out_act=out_act, act=act or "none",
+          act_param=p, x_out=xout)
     x64 = x.to(F64)
     if write_raw:
         got = xout if dest == "x_out" else xin
@@ -290,8 +290,9 @@ def _dec(s, slope=0.01):
 @pytest.mark.parametrize("C", [64, 128])
 @pytest.mark.parametrize("prec", ["bf16", "fp16"])
 def test_pair_fused_and_blocked_are_bit_identical(prec, C):
-    """impl 0 (one kernel, h in shared memory) and impl 2 (two conv-GEMM launches, h in the scratch) use the same
-    instruction shape, the same K order and the same epilogue expression order: their results are the same bits."""
+    """The fused form (one kernel, h in shared memory) and the blocked form (two conv-GEMM launches, h in the scratch)
+    use the same instruction shape, the same K order and the same epilogue expression order: their results are the same
+    bits."""
     B, L, dil = 2, 3000, 9
     x = _rnd(B, L, C, seed=61)
     a = F.leaky_relu(x, 0.01).to(DT[prec])
@@ -299,10 +300,10 @@ def test_pair_fused_and_blocked_are_bit_identical(prec, C):
     w2, _ = _op(_rnd(3, C, C, seed=63, scale=0.08), prec)
     b1, b2 = _rnd(C, seed=64, scale=0.1), _rnd(C, seed=65, scale=0.1)
     outs = []
-    for impl in (0, 2):
+    for form in ("fused", "blocked"):
         xin = x.clone()
         act = torch.full((B, L, C), SENT, dtype=DT[prec], device=DEV)
-        _pair(prec, impl, a, xin, w1, b1, w2, b2, dil, out_act=act)
+        _pair(prec, form, a, xin, w1, b1, w2, b2, dil, out_act=act)
         outs.append((xin, act))
     assert torch.equal(outs[0][0], outs[1][0])
     assert torch.equal(outs[0][1].view(torch.int16), outs[1][1].view(torch.int16))
@@ -310,7 +311,7 @@ def test_pair_fused_and_blocked_are_bit_identical(prec, C):
 
 @pytest.mark.parametrize("enc_out", [1, 0])
 def test_pair_tf32_fused_and_blocked_are_bit_identical(enc_out):
-    """tf32 on the encoded stream: impl 3 (one kernel) and impl 2 (blocked) give the same bits (the blocked form
+    """tf32 on the encoded stream: the fused and the blocked form give the same bits (the blocked form
     decodes the residual with 1 / 0.01f, which is 100.0f exactly as the fused one)."""
     from voicefixer_b200.weights import round_tf32
     B, L, C, dil = 2, 5000, 64, 27
@@ -318,9 +319,9 @@ def test_pair_tf32_fused_and_blocked_are_bit_identical(enc_out):
     w1, w2 = round_tf32(_rnd(3, C, C, seed=72, scale=0.08)), round_tf32(_rnd(3, C, C, seed=73, scale=0.08))
     b1, b2 = _rnd(C, seed=74, scale=0.1), _rnd(C, seed=75, scale=0.1)
     outs = []
-    for impl in (3, 2):
+    for form in ("fused", "blocked"):
         out = torch.full_like(S, SENT)
-        _pair("tf32", impl, S, S, w1, b1, w2, b2, dil, x_out=out, stream_enc=1, stream_enc_out=enc_out)
+        _pair("tf32", form, S, S, w1, b1, w2, b2, dil, x_out=out, stream_enc=1, stream_enc_out=enc_out)
         outs.append(out)
     assert torch.equal(outs[0].view(torch.int32), outs[1].view(torch.int32))
 

@@ -1,6 +1,8 @@
-"""GPU tests of the ResStack pair entry point (vfx_resstack_pair: conv1 -> h in the caller's scratch -> conv2 + residual,
-on the tensor-core convolution) through the C ABI, against the same arithmetic spelled out with torch ops: bf16 operands (a, h, weights), fp32
-accumulation, fp32 residual stream.  Reference op: ResStack.forward voicefixer/vocoder/model/modules.py:592-595.
+"""GPU tests of the ResStack pair entry point (vfx_resstack_pair) through the C ABI: the fused kernel (h kept in shared
+memory) and, where a test asks for it, the blocked form (conv1 -> h in the caller's scratch -> conv2 + residual, on the
+tensor-core convolution), against the same arithmetic spelled out with torch ops: 16-bit (or tf32-rounded) operands
+(a, h, weights), fp32 accumulation, fp32 residual stream.  Reference op: ResStack.forward
+voicefixer/vocoder/model/modules.py:592-595.
 
 Tolerances: fp32 output 1e-4 relative RMS (bf16 x bf16 products are exact in fp32; a rare bf16 rounding tie of the
 intermediate h may flip against torch's), activated bf16 output 4e-3 (one bf16 rounding)."""
@@ -119,7 +121,7 @@ def test_pair_rejects_other_widths():
 
 
 # ---------------------------------------------------------------------------- width 128 and the scratch
-def test_pair2_needs_scratch():
+def test_blocked_pair_needs_scratch():
     from voicefixer_b200 import _lib
     from voicefixer_b200._lib import VfxError
     lib = _lib.load()
@@ -130,7 +132,8 @@ def test_pair2_needs_scratch():
     act = torch.zeros_like(a)
     d = _lib.PairDesc()
     d.a, d.x, d.w1, d.b1, d.dilation, d.w2, d.b2 = a.data_ptr(), x.data_ptr(), w.data_ptr(), b.data_ptr(), 1, w.data_ptr(), b.data_ptr()
-    d.B, d.L, d.C, d.write_raw, d.out_act, d.act, d.act_param, d.precision, d.impl = 1, 300, 128, 1, act.data_ptr(), 1, 0.01, 1, 2
+    d.B, d.L, d.C, d.write_raw, d.out_act, d.act, d.act_param, d.precision = 1, 300, 128, 1, act.data_ptr(), 1, 0.01, 1
+    d.form = _lib.PAIR_FORM["blocked"]
     with pytest.raises(VfxError, match="scratch"):
         _lib.check(lib.vfx_resstack_pair(ctypes.byref(d), None), "pair2")
 
@@ -162,7 +165,7 @@ def test_pair2_16bit_matches_two_convolutions(C, L, dil, B, prec):
     act = torch.zeros(B, L, C, device=DEV, dtype=dt)
     d = _desc(_lib, a=a.data_ptr(), x=xin.data_ptr(), w1=w1p.data_ptr(), b1=b1.data_ptr(), dilation=dil, w2=w2p.data_ptr(),
               b2=b2.data_ptr(), B=B, L=L, C=C, write_raw=1, out_act=act.data_ptr(), act=_lib.ACT["lrelu"], act_param=0.01,
-              precision=_lib.PREC[prec], impl=2)
+              precision=_lib.PREC[prec], form=_lib.PAIR_FORM["blocked"])
     _lib.check(lib.vfx_resstack_pair(ctypes.byref(d), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "pair2")
     torch.cuda.synchronize()
     assert rel_rms((xin - x).cpu(), (ref - x).cpu()) < 1e-4
@@ -179,15 +182,14 @@ def _dec(s, slope=0.01):
     return torch.where(y > 0, y, y / slope)
 
 
-@pytest.mark.parametrize("impl", [3, 2])
+@pytest.mark.parametrize("form", ["fused", "blocked"])
 @pytest.mark.parametrize("L,dil,B,enc_out", [(1000, 1, 2, 1), (5000, 81, 1, 1), (3000, 9, 2, 0), (20000, 729, 2, 1),
                                              (125, 1, 1, 1), (127, 3, 2, 0), (4000, 27, 1, 1), (9000, 2187, 1, 1),
                                              (40000, 243, 3, 1), (378, 9, 1, 1)])
-def test_pair_tf32_encoded_stream(L, dil, B, enc_out, impl):
+def test_pair_tf32_encoded_stream(L, dil, B, enc_out, form):
     """tf32, C = 64: the encoded stream S is operand and residual carrier; the result goes to the other buffer as S' (or as
-    plain x' for the last pair of a stack).  impl 3 and 2 are the values callers of the sm_100a build pass; both must be
-    accepted: 3 runs the fused kernel, 2 the two convolutions per row block through the scratch.  Reference: tf32-rounded
-    operands and intermediate, fp32 accumulation."""
+    plain x' for the last pair of a stack), by the fused kernel and by the blocked form (the two convolutions per row
+    block through the scratch).  Reference: tf32-rounded operands and intermediate, fp32 accumulation."""
     from voicefixer_b200 import _lib
     from voicefixer_b200.weights import round_tf32
     lib = _lib.load()
@@ -204,8 +206,8 @@ def test_pair_tf32_encoded_stream(L, dil, B, enc_out, impl):
     out = torch.zeros_like(S)
     w1p, w2p = w1.permute(2, 0, 1).contiguous(), w2.permute(2, 0, 1).contiguous()
     d = _desc(_lib, a=S.data_ptr(), x=S.data_ptr(), w1=w1p.data_ptr(), b1=b1.data_ptr(), dilation=dil, w2=w2p.data_ptr(),
-              b2=b2.data_ptr(), B=B, L=L, C=C, write_raw=1, precision=_lib.PREC["tf32"], impl=impl, x_out=out.data_ptr(),
-              stream_enc=1, stream_enc_out=enc_out)
+              b2=b2.data_ptr(), B=B, L=L, C=C, write_raw=1, precision=_lib.PREC["tf32"], form=_lib.PAIR_FORM[form],
+              x_out=out.data_ptr(), stream_enc=1, stream_enc_out=enc_out)
     keep = S.clone()
     _lib.check(lib.vfx_resstack_pair(ctypes.byref(d), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "pair2")
     torch.cuda.synchronize()

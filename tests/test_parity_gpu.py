@@ -273,34 +273,20 @@ def test_tf32_encoded_stream_engine_path(states, oracle_10s):
 
 
 @pytest.mark.parametrize("prec", ["tf32", "fp16", "bf16"])
-def test_two_cta_pair_pipeline_engine_path(states, oracle_10s, prec):
-    """fuse_pair2: the width-128 ResStack pairs of the 16-bit modes (and, with 2, the tf32 width-64 pairs) as fused kernels:
-    same tolerance as the mode's plain path, and within rounding noise of it."""
+def test_fused_pairs_engine_path(states, oracle_10s, prec):
+    """fuse_pairs: every ResStack pair the fused kernel supports (tf32: C = 64 on the encoded stream; 16-bit: C = 64 and
+    128) as one kernel (1, the default) or as its two convolution launches (0).  The fused kernel adds the same slices in
+    the same order as the convolution: the two runs give the same bits, and both meet the mode's tolerance."""
     from voicefixer_b200.engine import Engine
     wav, ref = oracle_10s
     eng = Engine(states[0], states[1], precision=prec)
-    eng.set_option("fuse_pair3", 0)                       # tf32 width 64 would otherwise be fused already
-    eng.set_option("fuse_pair2", 0)
+    eng.set_option("fuse_pairs", 0)
     y0 = eng.restore(wav[None]).cpu().numpy()
-    eng.set_option("fuse_pair2", 2)
+    eng.set_option("fuse_pairs", 1)
     y1 = eng.restore(wav[None]).cpu().numpy()
-    assert rel_rms(y1, ref) < FULL_TOL[prec][0] and float(np.mean(np.abs(y1 - ref))) < FULL_TOL[prec][1]
-    assert rel_rms(y1, y0) < FULL_TOL[prec][0]
-
-
-def test_tf32_fused_pair_engine_path(states, oracle_10s):
-    """fuse_pair3 (default on): the width-64 ResStack pairs of the tf32 mode as one fused kernel each (h kept in shared
-    memory): same arithmetic as the two-launch path -- the outputs agree to rounding noise of the
-    accumulation order, far inside the mode's tolerance."""
-    from voicefixer_b200.engine import Engine
-    wav, ref = oracle_10s
-    eng = Engine(states[0], states[1], precision="tf32")
-    eng.set_option("fuse_pair3", 0)
-    y0 = eng.restore(wav[None]).cpu().numpy()
-    eng.set_option("fuse_pair3", 1)
-    y1 = eng.restore(wav[None]).cpu().numpy()
-    assert rel_rms(y1, ref) < FULL_TOL["tf32"][0] and float(np.mean(np.abs(y1 - ref))) < FULL_TOL["tf32"][1]
-    assert rel_rms(y1, y0) < 5e-4
+    for y in (y0, y1):
+        assert rel_rms(y, ref) < FULL_TOL[prec][0] and float(np.mean(np.abs(y - ref))) < FULL_TOL[prec][1]
+    assert np.array_equal(y1, y0), f"max |fused - unfused| {np.max(np.abs(y1 - y0)):.3e}, rel-rms {rel_rms(y1, y0):.3e}"
 
 
 # ---------------------------------------------------------------------------- fp16 tensor-core path

@@ -214,14 +214,14 @@ def test_conv_gemm_seq_extents(case, impl, prec):
         assert err < tol, f"item {b}: relative RMS {err:.2e} against float64"
 
 
-def _pair(prec, a, x, w1, b1, w2, b2, dil, lens=None, impl=0, x_out=None, enc=False):
+def _pair(prec, a, x, w1, b1, w2, b2, dil, lens=None, form="fused", x_out=None, enc=False):
     from voicefixer_b200 import _lib
     B, L, C = x.shape
     d = _lib.PairDesc()
     d.a, d.x = a.data_ptr(), x.data_ptr()
     d.w1, d.b1, d.dilation, d.w2, d.b2 = w1.data_ptr(), b1.data_ptr(), dil, w2.data_ptr(), b2.data_ptr()
     d.B, d.L, d.C, d.write_raw = B, L, C, 1
-    d.precision, d.impl = _lib.PREC[prec], impl
+    d.precision, d.form = _lib.PREC[prec], _lib.PAIR_FORM[form]
     d.x_out = None if x_out is None else x_out.data_ptr()
     d.stream_enc, d.stream_enc_out = (1, 1) if enc else (0, 0)
     d.lens = None if lens is None else lens.data_ptr()
@@ -232,7 +232,7 @@ def _pair(prec, a, x, w1, b1, w2, b2, dil, lens=None, impl=0, x_out=None, enc=Fa
 
 @pytest.mark.parametrize("prec,C", [("bf16", 64), ("bf16", 128), ("fp16", 64), ("fp16", 128), ("tf32", 64)])
 @pytest.mark.parametrize("dil", [1, 27, 243])
-def test_pair_lens_equal_items_alone(prec, C, dil):
+def test_fused_pair_lens_equal_items_alone(prec, C, dil):
     from voicefixer_b200.weights import round_tf32
     g = torch.Generator().manual_seed(20 + C + dil)
     lens_l = [400, 1, 127, 250, 5]
@@ -263,8 +263,8 @@ def test_pair_lens_equal_items_alone(prec, C, dil):
         rest = out[b, n:]
         assert torch.equal(rest, torch.full_like(rest, SENT) if enc else before[b, n:]), \
             f"item {b}: rows past its length were written"
-    # the blocked form (impl 2) refuses per-item lengths
-    assert _pair(prec, a, xin, w1, b1, w2, b2, dil, lens=lens, impl=2, x_out=out if enc else None, enc=enc) == -5
+    # the blocked form refuses per-item lengths
+    assert _pair(prec, a, xin, w1, b1, w2, b2, dil, lens=lens, form="blocked", x_out=out if enc else None, enc=enc) == -5
 
 
 def _gru(gi, whh_t, bhh, lens=None):

@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(HERE, "libvfx_b200.so")
 VFX_OK = 0
 PREC = {"fp32": 0, "bf16": 1, "tf32": 2, "fp16": 3}
 ACT = {"none": 0, "lrelu": 1, "elu": 2, "lrelu_xsinx": 3, "sigmoid": 4}
+PAIR_FORM = {"fused": 0, "blocked": 1}
 
 _c = ctypes
 _vp, _i, _f, _sz, _ll = _c.c_void_p, _c.c_int, _c.c_float, _c.c_size_t, _c.c_longlong
@@ -38,7 +39,7 @@ class PairDesc(ctypes.Structure):
     """struct vfx_pair_desc (include/vfx_b200.h)."""
     _fields_ = [("a", _vp), ("x", _vp), ("w1", _vp), ("b1", _vp), ("dilation", _i), ("w2", _vp), ("b2", _vp),
                 ("B", _i), ("L", _i), ("C", _i), ("write_raw", _i), ("out_act", _vp), ("act", _i), ("act_param", _f),
-                ("precision", _i), ("impl", _i), ("x_out", _vp), ("stream_enc", _i), ("stream_enc_out", _i),
+                ("precision", _i), ("form", _i), ("x_out", _vp), ("stream_enc", _i), ("stream_enc_out", _i),
                 ("scratch", _vp), ("scratch_bytes", _sz), ("lens", _vp)]
 
 

@@ -47,9 +47,7 @@ struct vfx_engine {
   std::vector<std::string> missing;
   int parts = 0;    // VFX_PART_* bits of the weight sets found complete by vfx_engine_finalize
   int tf32_stream = 1;  // TF32: vocoder residual streams are kept as ONE encoded fp32 tensor (operand + residual carrier)
-  int fuse_pair = 1;  // BF16 / FP16: ResStack pairs of width 64 run as ONE fused kernel (resstack_pair.cu)
-  int fuse_pair3 = 1; // TF32 width 64: the same fused kernel on the encoded stream
-  int fuse_pair2 = 1; // fused pairs of width 128 (BF16 / FP16); 2 = also TF32 width 64 when fuse_pair3 is 0
+  int fuse_pairs = 1;   // ResStack pairs that pair_supported() accepts run as ONE fused kernel (resstack_pair.cu)
   int profile = 0;
   std::vector<vfx::ProfRec> prof;
   std::string prof_report;
@@ -526,6 +524,78 @@ int analysis_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop
 }
 
 // ------------------------------------------------------------------ vocoder
+// The inputs and outputs of fused pair i of stack j (last: i == 7, last_stack: j == 3).  A pair reads its operand with a
+// halo that neighbouring tiles would overwrite in place, so the operand ping-pongs from cur to nxt: the tf32 encoded stream
+// between X and A0 (fused at C = 64 only, the last stack, whose 8 pairs end in X), the 16-bit operand between A0 and Hh.
+void pair_io(vfx_pair_desc& pd, bool enc, bool last, bool last_stack, void* cur, void* nxt, float* X, void* U) {
+  pd.a = cur;
+  if (enc) {
+    pd.x = (float*)cur; pd.x_out = (float*)nxt; pd.write_raw = 1;
+    pd.stream_enc = 1; pd.stream_enc_out = last ? 0 : 1;    // the last pair hands plain x' to the final convolution
+    return;
+  }
+  pd.x = X;
+  pd.write_raw = (!last || last_stack) ? 1 : 0;             // the next up-sampler consumes the operand only
+  if (!last) { pd.out_act = nxt; pd.act = VFX_ACT_LRELU; pd.act_param = 0.01f; }
+  else if (!last_stack) { pd.out_act = U; pd.act = VFX_ACT_LRELU_XSINX; pd.act_param = 0.2f; }
+}
+
+// ResStack j: 8 x (x + conv_k3_d1(lrelu(conv_k3_d3^i(lrelu(x))))), modules.py:550-576,592-595, width C, L rows (ext: the
+// items' lengths), x (or, enc, the encoded stream) in X.  A pair that pair_supported() accepts is one fused kernel (h stays
+// on chip), the others two convolutions with h in Hh.  The last stack ends with x' in X, the others with the next operand in U.
+int resstack(Ctx& c, int j, int B, long long L, int C, const int* ext, bool enc, float* X, void* A0, void* Hh, void* U) {
+  const int prec = c.prec();
+  const bool fused = c.e->use_tc && c.e->fuse_pairs && pair_supported(prec, C, enc);
+  void* cur = enc ? (void*)X : A0; void* nxt = enc ? A0 : Hh;
+  const std::string rs = "voc.rs" + std::to_string(j);
+  for (int i = 0, dil = 1; i < 8; ++i, dil *= 3) {
+    const std::string p = rs + ".l" + std::to_string(i);
+    const std::string per_dil = c.e->profile > 1 ? ".d" + std::to_string(dil) : "";   // profile 2: a tag per dilation
+    const void* w1 = getw(c, p + ".c1.w", (size_t)3 * C * C, prec); const float* b1 = getf(c, p + ".c1.b", C);
+    const void* w2 = getw(c, p + ".c2.w", (size_t)3 * C * C, prec); const float* b2 = getf(c, p + ".c2.b", C);
+    if (fused) {
+      vfx_pair_desc pd;
+      memset(&pd, 0, sizeof(pd));
+      pd.precision = prec; pd.dilation = dil; pd.B = B; pd.L = (int)L; pd.C = C; pd.lens = ext;
+      pd.w1 = w1; pd.b1 = b1; pd.w2 = w2; pd.b2 = b2;
+      pair_io(pd, enc, i == 7, j == 3, cur, nxt, X, U);
+      if (!c.dry && c.rc == VFX_OK) {
+        const double els = (double)B * L * C;
+        // algorithmic bytes of a pair (SURVEY 8d): x in + x' out, fp32
+        ProfScope ps(c, (rs + ".pair" + per_dil).c_str(), 2.0 * 2.0 * 3.0 * C * els, 8.0 * els);
+        VFX_TRY(resstack_pair(pd, c.st));
+      }
+      std::swap(cur, nxt);
+    } else {
+      vfx_conv_desc d1 = conv_base(enc ? (const void*)X : (const void*)A0, B, 1, (int)L, C, w1, C);
+      d1.ntaps = 3;
+      for (int k = 0; k < 3; ++k) { d1.dw[k] = (k - 1) * dil; d1.w_off[k] = (long long)k * C * C; }
+      set_seq(d1, ext, ext, 1);
+      d1.bias = b1;
+      set_act(d1, Hh, C, 0, VFX_ACT_LRELU, 0.01f);
+      VFX_TRY(run_conv(c, prec, d1, (rs + ".c1" + per_dil).c_str()));
+      vfx_conv_desc d2 = conv_base(Hh, B, 1, (int)L, C, w2, C);
+      d2.ntaps = 3;
+      for (int k = 0; k < 3; ++k) { d2.dw[k] = k - 1; d2.w_off[k] = (long long)k * C * C; }
+      set_seq(d2, ext, ext, 1);
+      d2.bias = b2;
+      set_res(d2, X, C, 0);
+      if (enc) {
+        d2.res_enc = 1; d2.enc_slope = 0.01f;
+        if (i < 7) { set_raw(d2, X, C, 0); d2.raw_enc = 1; }              // S' in place
+        else if (j == 3) set_raw(d2, X, C, 0);                           // last stack: plain x' for the final conv
+        else set_act(d2, U, C, 0, VFX_ACT_LRELU_XSINX, 0.2f);            // next UpsampleNet's operand only
+      } else {
+        set_raw(d2, X, C, 0);
+        if (i < 7) set_act(d2, A0, C, 0, VFX_ACT_LRELU, 0.01f);
+        else if (j < 3) set_act(d2, U, C, 0, VFX_ACT_LRELU_XSINX, 0.2f);  // act + next UpsampleNet's x+sin x
+      }
+      VFX_TRY(run_conv(c, prec, d2, (rs + ".c2").c_str()));
+    }
+  }
+  return VFX_OK;     // a missing weight stays in c.rc: the dry pass goes on listing the others
+}
+
 // vocoder Generator.forward voicefixer/vocoder/model/generator.py:127-145 on cond [B][Tc][128]
 // (operand precision), then the fused post conv / tanh / trim.
 int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, int trim_len, float scale) {
@@ -586,10 +656,8 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
     // ragged batch: items' lengths at this up-sampler's input (= rows of its reshaped output view) and output rate
     const int* ext_in = c.ext_at(j == 0 ? EXT_COND : EXT_UP0 + j - 1);
     const int* ext_out = c.ext_at(EXT_UP0 + j);
-    char up_tag[32], c1_tag[32], c2_tag[32];
+    char up_tag[32];
     snprintf(up_tag, sizeof(up_tag), "voc.up%d", j);
-    snprintf(c1_tag, sizeof(c1_tag), "voc.rs%d.c1", j);
-    snprintf(c2_tag, sizeof(c2_tag), "voc.rs%d.c2", j);
     // ---- UpsampleNet: ConvTranspose1d(k=2u, s=u, p, op) as two phase-group GEMMs (modules.py:451-459)
     snprintf(name, sizeof(name), "voc.up%d", j);
     {
@@ -615,80 +683,7 @@ int vocoder_generator(Ctx& c, const void* cond, int B, int Tc, float* wav_out, i
         VFX_TRY(run_conv(c, prec, d, up_tag));
       }
     }
-    // ---- ResStack: 8 x (x + conv_k3_d1(lrelu(conv_k3_d3^i(lrelu(x))))), modules.py:550-576,592-595
-    // 16-bit modes, width 64 / 128: each pair is ONE fused kernel (h stays on chip); the activated operand copy ping-pongs
-    // between A0 and Hh because a pair reads it with a halo that neighbouring tiles would overwrite in place.
-    const bool is16 = prec == VFX_PREC_BF16 || prec == VFX_PREC_FP16;          // 2-byte operand modes share every kernel
-    const bool fuse_pairs = is16 && c.e->use_tc &&
-                            ((c.e->fuse_pair && Co == 64) || (c.e->fuse_pair2 && Co == 128));
-    // tf32, width 64: the encoded stream ping-pongs between X and the (otherwise unused) operand buffer; 8 pairs end in X
-    const bool fuse_tf32 = enc && (c.e->fuse_pair3 || c.e->fuse_pair2 >= 2) && Co == 64 && j == 3;
-    void* a_cur = A0; void* a_nxt = Hh;
-    float* s_cur = X; float* s_nxt = (float*)A0;
-    int dil = 1;
-    for (int i = 0; i < 8; ++i, dil *= 3) {
-      snprintf(name, sizeof(name), "voc.rs%d.l%d", j, i);
-      const std::string p(name);
-      if (fuse_tf32 || fuse_pairs) {
-        vfx_pair_desc pd;
-        memset(&pd, 0, sizeof(pd));
-        pd.precision = prec; pd.dilation = dil; pd.B = B; pd.L = (int)Lout; pd.C = Co; pd.lens = ext_out;
-        pd.w1 = getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec); pd.b1 = getf(c, p + ".c1.b", Co);
-        pd.w2 = getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec); pd.b2 = getf(c, p + ".c2.b", Co);
-        if (fuse_tf32) {
-          pd.a = s_cur; pd.x = s_cur; pd.x_out = s_nxt; pd.write_raw = 1;
-          pd.stream_enc = 1; pd.stream_enc_out = i < 7 ? 1 : 0;   // the last pair hands plain x' to the final convolution
-        } else {
-          pd.a = a_cur; pd.x = X;
-          pd.write_raw = (i < 7 || j == 3) ? 1 : 0;               // the next up-sampler consumes the operand only
-          if (i < 7) { pd.out_act = a_nxt; pd.act = VFX_ACT_LRELU; pd.act_param = 0.01f; }
-          else if (j < 3) { pd.out_act = U; pd.act = VFX_ACT_LRELU_XSINX; pd.act_param = 0.2f; }
-        }
-        if (!c.dry && c.rc == VFX_OK) {
-          char pt[48], ptd[64];
-          snprintf(pt, sizeof(pt), "voc.rs%d.pair", j);
-          snprintf(ptd, sizeof(ptd), "%s.d%d", pt, dil);
-          const double els = (double)B * Lout * Co;
-          // algorithmic bytes of a pair (SURVEY 8d): x in + x' out, fp32
-          ProfScope ps(c, c.e->profile > 1 ? ptd : pt, 2.0 * 2.0 * 3.0 * Co * els, 8.0 * els);
-          VFX_TRY(resstack_pair(pd, c.st));
-        }
-        if (fuse_tf32) { float* t = s_cur; s_cur = s_nxt; s_nxt = t; }
-        else { void* t = a_cur; a_cur = a_nxt; a_nxt = t; }
-        continue;
-      }
-      {
-        vfx_conv_desc d = conv_base(enc ? (const void*)X : (const void*)A0, B, 1, (int)Lout, Co,
-                                    getw(c, p + ".c1.w", (size_t)3 * Co * Co, prec), Co);
-        d.ntaps = 3;
-        for (int k = 0; k < 3; ++k) { d.dw[k] = (k - 1) * dil; d.w_off[k] = (long long)k * Co * Co; }
-        set_seq(d, ext_out, ext_out, 1);
-        d.bias = getf(c, p + ".c1.b", Co);
-        set_act(d, Hh, Co, 0, VFX_ACT_LRELU, 0.01f);
-        char c1d[48];
-        snprintf(c1d, sizeof(c1d), "%s.d%d", c1_tag, dil);
-        VFX_TRY(run_conv(c, prec, d, c.e->profile > 1 ? c1d : c1_tag));
-      }
-      {
-        vfx_conv_desc d = conv_base(Hh, B, 1, (int)Lout, Co, getw(c, p + ".c2.w", (size_t)3 * Co * Co, prec), Co);
-        d.ntaps = 3;
-        for (int k = 0; k < 3; ++k) { d.dw[k] = k - 1; d.w_off[k] = (long long)k * Co * Co; }
-        set_seq(d, ext_out, ext_out, 1);
-        d.bias = getf(c, p + ".c2.b", Co);
-        set_res(d, X, Co, 0);
-        if (enc) {
-          d.res_enc = 1; d.enc_slope = 0.01f;
-          if (i < 7) { set_raw(d, X, Co, 0); d.raw_enc = 1; }               // S' in place
-          else if (j == 3) set_raw(d, X, Co, 0);                            // last stack: plain x' for the final conv
-          else set_act(d, U, Co, 0, VFX_ACT_LRELU_XSINX, 0.2f);             // next UpsampleNet's operand only
-        } else {
-          set_raw(d, X, Co, 0);
-          if (i < 7) set_act(d, A0, Co, 0, VFX_ACT_LRELU, 0.01f);
-          else if (j < 3) set_act(d, U, Co, 0, VFX_ACT_LRELU_XSINX, 0.2f);   // act + next UpsampleNet's x+sin x
-        }
-        VFX_TRY(run_conv(c, prec, d, c2_tag));
-      }
-    }
+    VFX_TRY(resstack(c, j, B, Lout, Co, ext_out, enc, X, A0, Hh, U));
     Lin = Lout;
   }
   // ---- LeakyReLU(0.2) + ReflectionPad1d(3) + Conv1d(64,1,7) + Tanh + _trim_center
@@ -994,9 +989,7 @@ int vfx_engine_set_option(vfx_engine* e, const char* key, int value) {
   VFX_REQUIRE(e && key, "set_option: null argument");
   if (!strcmp(key, "use_tc")) { e->use_tc = value; return VFX_OK; }
   if (!strcmp(key, "profile")) { e->profile = value; return VFX_OK; }
-  if (!strcmp(key, "fuse_pair")) { e->fuse_pair = value; return VFX_OK; }
-  if (!strcmp(key, "fuse_pair2")) { e->fuse_pair2 = value; return VFX_OK; }
-  if (!strcmp(key, "fuse_pair3")) { e->fuse_pair3 = value; return VFX_OK; }
+  if (!strcmp(key, "fuse_pairs")) { e->fuse_pairs = value; return VFX_OK; }
   if (!strcmp(key, "tf32_stream")) { e->tf32_stream = value; return VFX_OK; }
   set_error("set_option: unknown key '%s'", key);
   return VFX_ERR_INVALID;
@@ -1246,8 +1239,8 @@ int vfx_resstack_pair(const vfx_pair_desc* d, void* stream) {
   VFX_REQUIRE(d, "resstack_pair: null descriptor");
   const int r = resstack_pair(*d, (cudaStream_t)stream);
   if (r == VFX_ERR_UNSUPPORTED)
-    set_error("resstack_pair: unsupported shape (impl 0..3; bf16 / fp16: C = 64 or 128; tf32: C = 64 with stream_enc and x_out; "
-              "16-byte aligned tensors)");
+    set_error("resstack_pair: unsupported (bf16 / fp16: C = 64 or 128; tf32: C = 64 with stream_enc and x_out; "
+              "16-byte aligned tensors; the blocked form takes no lens)");
   return r;
 }
 

@@ -1,7 +1,7 @@
 // ResStack pair x' = x + conv2_{k3,d=1}(lrelu_0.01(conv1_{k3,dilation}(a) + b1)) + b2 (include/vfx_b200.h,
 // vfx_resstack_pair), ResStack.forward voicefixer/vocoder/model/modules.py:592-595.
 //
-// Fused form (impl 0 / 1 / 3; the engine's fused pairs): one CTA per 126 output rows of one item, two warpgroups.
+// Fused form (VFX_PAIR_FUSED; the engine's fused pairs): one CTA per 126 output rows of one item, two warpgroups.
 // conv1 computes h for the 128 rows [r0 - 1, r0 + 127) with wgmma (a staged by cp.async into 128-byte-swizzled tiles,
 // W1 streamed through the same 3-stage ring); its epilogue writes lrelu(h + b1) in the operand format into shared
 // memory three times, copy t shifted up by t rows, so that conv2's tap t reads copy t as an ordinary K-major A tile
@@ -12,7 +12,7 @@
 //
 // Ragged batches (vfx_pair_desc.lens): item b is computed as if its length were lens[b]; tiles starting beyond it exit.
 //
-// Blocked form (impl 2): the two convolutions of conv_gemm_tc.cu per block of rows, h in the caller's scratch.
+// Blocked form (VFX_PAIR_BLOCKED, the tests' reference): conv_gemm_tc.cu's two convolutions per row block, h in a scratch.
 #include <string.h>
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
@@ -234,16 +234,19 @@ static int pair_blocked(const vfx_pair_desc& d, int prec, cudaStream_t st) {
   return VFX_OK;
 }
 
+bool pair_supported(int prec, int C, bool stream_enc) {
+  return prec == VFX_PREC_TF32 ? C == 64 && stream_enc
+                               : (prec == VFX_PREC_BF16 || prec == VFX_PREC_FP16) && (C == 64 || C == 128) && !stream_enc;
+}
+
 int resstack_pair(const vfx_pair_desc& d, cudaStream_t st) {
-  const int prec = d.precision == VFX_PREC_FP32 ? VFX_PREC_BF16 : d.precision;    // 0 is read as BF16
-  const bool tf32 = prec == VFX_PREC_TF32;
-  const bool shape_ok = tf32 ? (d.C == 64 && d.stream_enc && d.x_out)
-                             : ((prec == VFX_PREC_BF16 || prec == VFX_PREC_FP16) && (d.C == 64 || d.C == 128) && !d.stream_enc);
-  if (!shape_ok || d.impl < 0 || d.impl > 3) return VFX_ERR_UNSUPPORTED;
+  VFX_REQUIRE(d.form == VFX_PAIR_FUSED || d.form == VFX_PAIR_BLOCKED, "resstack_pair: form %d is not a vfx_pair_form", d.form);
+  const int prec = d.precision;
+  if (!pair_supported(prec, d.C, d.stream_enc != 0) || (d.stream_enc && !d.x_out)) return VFX_ERR_UNSUPPORTED;
   VFX_REQUIRE(d.a && d.x && d.w1 && d.w2 && d.b1 && d.b2 && d.B > 0 && d.L > 0 && d.dilation > 0, "resstack_pair: bad arguments");
-  if (d.impl == 2) return d.lens ? VFX_ERR_UNSUPPORTED : pair_blocked(d, prec, st);
+  if (d.form == VFX_PAIR_BLOCKED) return d.lens ? VFX_ERR_UNSUPPORTED : pair_blocked(d, prec, st);
   if (((uintptr_t)d.a & 15) || ((uintptr_t)d.w1 & 15) || ((uintptr_t)d.w2 & 15)) return VFX_ERR_UNSUPPORTED;
-  if (tf32) return launch_fused<64, 0>(d, st);
+  if (prec == VFX_PREC_TF32) return launch_fused<64, 0>(d, st);
   if (prec == VFX_PREC_BF16) return d.C == 64 ? launch_fused<64, 1>(d, st) : launch_fused<128, 1>(d, st);
   return d.C == 64 ? launch_fused<64, 2>(d, st) : launch_fused<128, 2>(d, st);
 }

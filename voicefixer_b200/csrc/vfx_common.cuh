@@ -95,8 +95,10 @@ __device__ __forceinline__ float apply_act(float v, int act, float p) {
 
 // ------------------------------------------------------------------ kernels (host launchers)
 int conv_gemm_simt(int precision, const vfx_conv_desc& d, cudaStream_t st);
-int resstack_pair(const vfx_pair_desc& d, cudaStream_t st);        // ResStack pair as two conv_gemm_tc launches per row block
+int resstack_pair(const vfx_pair_desc& d, cudaStream_t st);        // ResStack pair, fused or blocked form (vfx_pair_desc.form)
 size_t resstack_pair_scratch_bytes();
+// the pairs resstack_pair runs: bf16 / fp16 at C = 64 or 128 without stream encoding, tf32 at C = 64 on the encoded stream
+bool pair_supported(int prec, int C, bool stream_enc);
 int conv_gemm_tc(int precision, const vfx_conv_desc& d, cudaStream_t st);   // wgmma: bf16 / fp16 (f16 kinds) or tf32
 
 // y = act(scale[b][c]*x + shift[b][c]); x fp32 [B][P][C] (row pitch ldx), y operand type.
