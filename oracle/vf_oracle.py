@@ -17,7 +17,28 @@ All functions take flat state dicts in the reference checkpoint layout:
                                   "f_helper.stft.conv_real.weight", ...)
   voc: keys of ckpt["generator"] ("condnet.0.bias", "...parametrizations.weight.original0/1"
                                   or old-style "...weight_g/weight_v")
+
+Arithmetic follows the dtype and device of the state dicts: given float64 copies of the checkpoints (on any device),
+every function computes in float64 there, on the float32 samples it is given.  Constants the reference defines in
+float32 (the vocoder's mel weights and min_level, the Slaney basis, the checkpoint's STFT kernels) keep their float32
+values, converted exactly.  With float32 state dicts the results are the fp32 oracle's, bit for bit.
+
+Operand rounding (`operand_rounding`): a model of the engine's tensor-core precisions.  Inside the context, the
+operands of every dense contraction the engine runs on the tensor cores are rounded to tf32 / fp16 / bf16 where the
+engine rounds them (csrc/engine.cu, weights.py); accumulation stays in the state dicts' dtype.  Rounded:
+  - every Conv1d / Conv2d / ConvTranspose input and weight of the UNet and the vocoder (the operand buffers A0 / Hh /
+    U / opA / opH / opX and the conditions, cast by their producers' epilogues), including the shortcut convs' raw x;
+  - the denoiser's Linear inputs act(bn(x)) and weights;
+  - the GRU input projections: bn(x) and layer 0's output y0 (dn_operand), and the w_ih weights;
+  - in eval mode, UNet ConvBlockRes.conv1 with bn2 folded into it: the engine rounds round(w1 * bn2.scale) and adds
+    bn2.shift in fp32 (weights._conv_block's conv1f), so the model does the same.
+Not rounded: the STFT front end (an fp32 FFT), the GRU recurrence, the UNet head after_conv2 (unet.head.w is fp32),
+the vocoder post conv generator.16 (voc.post.w is fp32 and reads plain x'), BatchNorm statistics, residual adds,
+the denoiser mask and the log.  Tensors the engine keeps in fp32 between contractions pass through
+`OperandRounding.stored` (identity here), so that a test can model a wiring fault that would store one in the
+operand format.
 """
+import contextlib
 import math
 import numpy as np
 import torch
@@ -30,6 +51,74 @@ N_MEL = 128
 SEG_LEN = SR * 30                      # voicefixer/base.py:116
 UPSAMPLE_SCALES = (7, 7, 3, 3)         # voicefixer/vocoder/config.py:20
 MEL_W_A, MEL_W_B = 18.8927416350036, 0.0269863588184314   # vocoder/config.py:301,310
+BN_EPS = 1e-5                          # nn.BatchNorm2d default, every BatchNorm of the analysis model
+
+
+# --------------------------------------------------------------------------- operand rounding
+def round_tf32(x):
+    """Nearest tf32 value, ties away from zero (PTX cvt.rna.tf32.f32), in x's dtype (float32 or float64)."""
+    if x.dtype == torch.float64:
+        i = x.contiguous().view(torch.int64)
+        return ((i + (1 << 41)) & ~((1 << 42) - 1)).view(torch.float64)
+    i = x.contiguous().view(torch.int32)
+    return ((i + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def trunc_tf32(x):
+    """Truncation to tf32: what the tensor core does to an fp32 operand that was not rounded."""
+    if x.dtype == torch.float64:
+        i = x.contiguous().view(torch.int64)
+        return (i & ~((1 << 42) - 1)).view(torch.float64)
+    i = x.contiguous().view(torch.int32)
+    return (i & ~0x1FFF).view(torch.float32)
+
+
+def _via(dtype):
+    return lambda x: x.to(dtype).to(x.dtype)
+
+
+ROUNDINGS = {"tf32": round_tf32, "tf32-trunc": trunc_tf32, "fp16": _via(torch.float16), "bf16": _via(torch.bfloat16)}
+
+
+class OperandRounding:
+    """The operand format of one engine precision: `operand` rounds a contraction's input or weight, `stored` is
+    applied to the tensors the engine keeps in fp32 between contractions ("vocoder.residual": the ResStack stream x
+    after the up-sampler and after each pair; "unet.block": each ConvBlockRes output).  Subclass to model faults."""
+
+    def __init__(self, fmt):
+        if fmt not in ROUNDINGS:
+            raise ValueError(f"unknown operand format '{fmt}' (one of {sorted(ROUNDINGS)})")
+        self.fmt = fmt
+        self.round = ROUNDINGS[fmt]
+
+    def operand(self, x):
+        return self.round(x)
+
+    def stored(self, x, where):
+        return x
+
+
+_rounding = None
+
+
+@contextlib.contextmanager
+def operand_rounding(model):
+    """Runs the oracle with the operand rounding `model` (an OperandRounding or a format name) inside the block."""
+    global _rounding
+    saved = _rounding
+    _rounding = OperandRounding(model) if isinstance(model, str) else model
+    try:
+        yield _rounding
+    finally:
+        _rounding = saved
+
+
+def _op(x):
+    return x if _rounding is None else _rounding.operand(x)
+
+
+def _stored(x, where):
+    return x if _rounding is None else _rounding.stored(x, where)
 
 
 # --------------------------------------------------------------------------- front end
@@ -38,9 +127,10 @@ def stft_mag(wav, ana):
     torchlibrosa.stft.STFT.forward as built at tools/modules/fDomainHelper.py:23-31 (DFT-matrix
     conv1d, stride 441, reflect pad 1024) and spectrogram_phase fDomainHelper.py:81-86 with
     eps=1e-8 (wav_to_spectrogram_phase :88)."""
-    x = wav.float()[:, None, :]
+    kr = ana["f_helper.stft.conv_real.weight"]
+    x = wav.to(dtype=kr.dtype, device=kr.device)[:, None, :]
     x = F.pad(x, (N_FFT // 2, N_FFT // 2), mode="reflect")
-    real = F.conv1d(x, ana["f_helper.stft.conv_real.weight"], stride=HOP)
+    real = F.conv1d(x, kr, stride=HOP)
     imag = F.conv1d(x, ana["f_helper.stft.conv_imag.weight"], stride=HOP)
     real = real[:, None].transpose(2, 3)
     imag = imag[:, None].transpose(2, 3)
@@ -64,9 +154,9 @@ def _bn1(x, ana, prefix, train):
     (N,H,W).  restorer/model.py:69-99 (BatchNorm2d(1) members)."""
     w, b = ana[prefix + ".weight"], ana[prefix + ".bias"]
     if train:
-        return F.batch_norm(x, None, None, w, b, True, 0.0, 1e-5)
+        return F.batch_norm(x, None, None, w, b, True, 0.0, BN_EPS)
     return F.batch_norm(x, ana[prefix + ".running_mean"], ana[prefix + ".running_var"], w, b,
-                        False, 0.0, 1e-5)
+                        False, 0.0, BN_EPS)
 
 
 def gru_layer_dir(x, w_ih, w_hh, b_ih, b_hh, reverse):
@@ -74,7 +164,7 @@ def gru_layer_dir(x, w_ih, w_hh, b_ih, b_hh, reverse):
     Gate order r,z,n; n = tanh(W_in x + b_in + r*(W_hn h + b_hn)); h' = (1-z)*n + z*h."""
     B, T, _ = x.shape
     H = w_hh.shape[1]
-    gi = x @ w_ih.t() + b_ih
+    gi = _op(x) @ _op(w_ih).t() + b_ih
     h = x.new_zeros(B, H)
     out = x.new_zeros(B, T, H)
     steps = range(T - 1, -1, -1) if reverse else range(T)
@@ -111,42 +201,57 @@ def denoiser(mel, ana, train=False, drop_masks=None):
     SURVEY 8c hygiene note: torch RNG-stream parity is not attainable)."""
     p = "generator.denoiser."
     x = _bn1(mel, ana, p + "0", train)
-    x = F.relu(F.linear(x, ana[p + "1.weight"], ana[p + "1.bias"]))
+    x = F.relu(_linear(x, ana, p + "1"))
     x = _bn1(x, ana, p + "3", train)
-    x = F.linear(x, ana[p + "4.weight"], ana[p + "4.bias"])
+    x = _linear(x, ana, p + "4")
     if train and drop_masks is not None:
-        x = x * drop_masks[0].to(x.dtype) * 2.0
+        x = x * drop_masks[0].to(x) * 2.0
     x = F.relu(x)
     x = bn_gru(x, ana, p + "7", train)
     x = bn_gru(x, ana, p + "8", train)
     x = F.relu(_bn1(x, ana, p + "9", train))
-    x = F.linear(x, ana[p + "11.weight"], ana[p + "11.bias"])
+    x = _linear(x, ana, p + "11")
     if train and drop_masks is not None:
-        x = x * drop_masks[1].to(x.dtype) * 2.0
+        x = x * drop_masks[1].to(x) * 2.0
     x = F.relu(_bn1(x, ana, p + "13", train))
-    x = F.linear(x, ana[p + "15.weight"], ana[p + "15.bias"])
+    x = _linear(x, ana, p + "15")
     return torch.sigmoid(x)
+
+
+def _linear(x, ana, p):
+    return F.linear(_op(x), _op(ana[p + ".weight"]), ana[p + ".bias"])
 
 
 # --------------------------------------------------------------------------- UNet
 def _bn2d(x, ana, prefix, train):
     w, b = ana[prefix + ".weight"], ana[prefix + ".bias"]
     if train:
-        return F.batch_norm(x, None, None, w, b, True, 0.0, 1e-5)
+        return F.batch_norm(x, None, None, w, b, True, 0.0, BN_EPS)
     return F.batch_norm(x, ana[prefix + ".running_mean"], ana[prefix + ".running_var"], w, b,
-                        False, 0.0, 1e-5)
+                        False, 0.0, BN_EPS)
+
+
+def _conv1_bn2(a, ana, p, train):
+    """bn2(conv1(a)).  Under operand rounding in eval mode, the engine's form: bn2 folded into conv1, the folded
+    weight rounded, the shift added after the contraction (weights._conv_block, engine.cu conv_block)."""
+    w1 = ana[p + ".conv1.weight"]
+    if _rounding is None or train:
+        return _bn2d(F.conv2d(_op(a), _op(w1), padding=1), ana, p + ".bn2", train)
+    q = p + ".bn2"
+    scale = ana[q + ".weight"] / torch.sqrt(ana[q + ".running_var"] + BN_EPS)
+    shift = ana[q + ".bias"] - ana[q + ".running_mean"] * scale
+    return F.conv2d(_op(a), _op(w1 * scale[:, None, None, None]), shift, padding=1)
 
 
 def conv_block_res(x, ana, p, train):
     """ConvBlockRes.forward restorer/modules.py:68-76 (pre-activation, lrelu 0.01)."""
     origin = x
-    x = F.conv2d(F.leaky_relu(_bn2d(x, ana, p + ".bn1", train), 0.01), ana[p + ".conv1.weight"],
-                 padding=1)
-    x = F.conv2d(F.leaky_relu(_bn2d(x, ana, p + ".bn2", train), 0.01), ana[p + ".conv2.weight"],
-                 padding=1)
+    x = _conv1_bn2(F.leaky_relu(_bn2d(x, ana, p + ".bn1", train), 0.01), ana, p, train)
+    x = F.conv2d(_op(F.leaky_relu(x, 0.01)), _op(ana[p + ".conv2.weight"]), padding=1)
     if (p + ".shortcut.weight") in ana:
-        return F.conv2d(origin, ana[p + ".shortcut.weight"], ana[p + ".shortcut.bias"]) + x
-    return origin + x
+        return _stored(F.conv2d(_op(origin), _op(ana[p + ".shortcut.weight"]), ana[p + ".shortcut.bias"]) + x,
+                       "unet.block")
+    return _stored(origin + x, "unet.block")
 
 
 def encoder_block(x, ana, p, train):
@@ -159,7 +264,7 @@ def encoder_block(x, ana, p, train):
 def decoder_block(x, skip, ana, p, train):
     """DecoderBlockRes.forward restorer/modules.py:149-157 (relu(bn1) -> ConvT 3x3 s2 ->
     prune last time row -> cat -> 4 ConvBlockRes)."""
-    x = F.conv_transpose2d(F.relu(_bn2d(x, ana, p + ".bn1", train)), ana[p + ".conv1.weight"],
+    x = F.conv_transpose2d(_op(F.relu(_bn2d(x, ana, p + ".bn1", train))), _op(ana[p + ".conv1.weight"]),
                            stride=2)
     x = x[:, :, 0:-1, :]
     x = torch.cat((x, skip), 1)
@@ -183,7 +288,7 @@ def unet(x, ana, train=False):
     for i in range(1, 7):
         x = decoder_block(x, skips[6 - i], ana, f"{u}decoder_block{i}", train)
     x = conv_block_res(x, ana, u + "after_conv_block1", train)
-    x = F.conv2d(x, ana[u + "after_conv2.weight"], ana[u + "after_conv2.bias"])
+    x = F.conv2d(x, ana[u + "after_conv2.weight"], ana[u + "after_conv2.bias"])      # fp32 in the engine too
     x = F.pad(x, (0, 1))
     return x[:, :, 0:origin_len, :]
 
@@ -230,24 +335,25 @@ def vocoder_normalize(mel):
     """Vocoder.forward vocoder/base.py:51-54 + tr_amp_to_db/tr_normalize/tr_pre
     vocoder/model/util.py:8-36,69-80.  mel (B,1,T,128) linear -> cond (B,128,T + T%2 + 4)."""
     assert mel.size()[-1] == 128
-    mel = mel / mel_weight()[None, None, None, :].type_as(mel)
-    min_level = torch.exp(torch.tensor(-100.0) / 20 * torch.log(torch.tensor(10.0)))
+    mel = mel / mel_weight()[None, None, None, :].to(mel)
+    min_level = torch.exp(torch.tensor(-100.0) / 20 * torch.log(torch.tensor(10.0))).to(mel)
     S = 20 * torch.log10(torch.maximum(min_level, torch.abs(mel))) - 20.0
     S = torch.clip(8.0 * ((S + 115.0) / 115.0) - 4.0, -4.0, 4.0)
     c = S[:, 0].transpose(1, 2)
     pad_tail = c.size(-1) % 2 + 4
-    return torch.cat([c, torch.zeros(c.size(0), N_MEL, pad_tail) - 4.0], -1)
+    return torch.cat([c, torch.zeros(c.size(0), N_MEL, pad_tail, dtype=c.dtype, device=c.device) - 4.0], -1)
 
 
 def res_stack(x, voc, p):
     """ResStack.forward modules.py:592-595 over the Sequentials built at :550-576."""
+    x = _stored(x, "vocoder.residual")
     for i in range(8):
         d = 3 ** i
-        h = F.conv1d(F.leaky_relu(x, 0.01), _wn(voc, f"{p}.layers.{i}.1"), voc[f"{p}.layers.{i}.1.bias"],
+        h = F.conv1d(_op(F.leaky_relu(x, 0.01)), _op(_wn(voc, f"{p}.layers.{i}.1")), voc[f"{p}.layers.{i}.1.bias"],
                      dilation=d, padding=d)
-        h = F.conv1d(F.leaky_relu(h, 0.01), _wn(voc, f"{p}.layers.{i}.3"), voc[f"{p}.layers.{i}.3.bias"],
+        h = F.conv1d(_op(F.leaky_relu(h, 0.01)), _op(_wn(voc, f"{p}.layers.{i}.3")), voc[f"{p}.layers.{i}.3.bias"],
                      padding=1)
-        x = x + h
+        x = _stored(x + h, "vocoder.residual")
     return x
 
 
@@ -256,7 +362,7 @@ def upsample_net(x, voc, p, u):
     weight-normed ConvTranspose1d(k=2u, s=u, p=u//2+u%2, output_padding=u%2).  The skip_conv
     result is discarded by the reference (SURVEY D7) and is not computed here."""
     x = x + torch.sin(x)
-    return F.conv_transpose1d(x, _wn(voc, p + ".layer"), voc[p + ".layer.bias"], stride=u,
+    return F.conv_transpose1d(_op(x), _op(_wn(voc, p + ".layer")), voc[p + ".layer.bias"], stride=u,
                               padding=u // 2 + u % 2, output_padding=u % 2)
 
 
@@ -264,13 +370,14 @@ def vocoder_generator(cond, voc):
     """vocoder Generator.forward generator.py:127-145 (condnet :33-54, generator :73-100)."""
     x = cond
     for i in (0, 2, 4, 6, 8):
-        x = F.elu(F.conv1d(x, _wn(voc, f"condnet.{i}"), voc[f"condnet.{i}.bias"], padding=1))
-    x = F.conv1d(F.pad(x, (3, 3), mode="reflect"), _wn(voc, "generator.1"), voc["generator.1.bias"])
+        x = F.elu(F.conv1d(_op(x), _op(_wn(voc, f"condnet.{i}")), voc[f"condnet.{i}.bias"], padding=1))
+    x = F.conv1d(_op(F.pad(x, (3, 3), mode="reflect")), _op(_wn(voc, "generator.1")), voc["generator.1.bias"])
     x = F.leaky_relu(x, 0.2)
     for j, u in enumerate(UPSAMPLE_SCALES):
         x = upsample_net(x, voc, f"generator.{3 + 3 * j}", u)
         x = res_stack(x, voc, f"generator.{4 + 3 * j}")
         x = F.leaky_relu(x, 0.2)
+    # fp32 in the engine too: voc.post.w is fp32 and reads plain x'
     x = F.conv1d(F.pad(x, (3, 3), mode="reflect"), _wn(voc, "generator.16"), voc["generator.16.bias"])
     return torch.tanh(x)
 
@@ -292,17 +399,20 @@ def trim_center(est, ref_len):
     return est[..., :min(n, ref_len)]
 
 
-def remove_higher_frequency(wav, ratio=0.95):
+def remove_higher_frequency(wav, ratio=0.95, dtype=np.float32, return_cut=False):
     """VoiceFixer.remove_higher_frequency base.py:87-104 (mode 1) with librosa 0.10.1
     (Dockerfile:9) defaults restated: stft(n_fft=2048, hop=512, hann periodic, center=True,
-    pad_mode='constant'), istft(length=None -> 512*(frames-1), window-sumsquare normalised)."""
-    wav = np.asarray(wav, dtype=np.float32)
+    pad_mode='constant'), istft(length=None -> 512*(frames-1), window-sumsquare normalised).
+    dtype: np.float32 (the reference's arithmetic) or np.float64.  return_cut: also return the first
+    zeroed bin."""
+    wav = np.asarray(wav, dtype=dtype)
+    cdt = np.result_type(dtype, np.complex64)
     n_fft, hop = 2048, 512
-    win = (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(n_fft) / n_fft)).astype(np.float32)
+    win = (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(n_fft) / n_fft)).astype(dtype)
     x = np.pad(wav, (n_fft // 2, n_fft // 2), mode="constant")
     nfr = 1 + (len(x) - n_fft) // hop
     idx = np.arange(n_fft)[None, :] + hop * np.arange(nfr)[:, None]
-    stft = np.fft.rfft(x[idx] * win[None, :], axis=1).T.astype(np.complex64)     # (1025, T)
+    stft = np.fft.rfft(x[idx] * win[None, :], axis=1).T.astype(cdt)     # (1025, T)
     real, img = np.real(stft), np.imag(stft)
     mag = (real ** 2 + img ** 2) ** 0.5
     cos, sin = real / (mag + 1e-8), img / (mag + 1e-8)
@@ -317,38 +427,46 @@ def remove_higher_frequency(wav, ratio=0.95):
         i += 1
     spec[i:, ...] = 0
     stft = spec * cos + 1j * spec * sin
-    frames = np.fft.irfft(stft.T, n=n_fft, axis=1).astype(np.float32) * win[None, :]
+    frames = np.fft.irfft(stft.T, n=n_fft, axis=1).astype(dtype) * win[None, :]
     out_len = n_fft + hop * (nfr - 1)
-    y = np.zeros(out_len, dtype=np.float32)
-    wss = np.zeros(out_len, dtype=np.float32)
+    y = np.zeros(out_len, dtype=dtype)
+    wss = np.zeros(out_len, dtype=dtype)
     wsq = win ** 2
     for t in range(nfr):
         y[t * hop:t * hop + n_fft] += frames[t]
         wss[t * hop:t * hop + n_fft] += wsq
     nz = wss > np.finfo(np.float32).tiny
     y[nz] /= wss[nz]
-    return y[n_fft // 2: n_fft // 2 + hop * (nfr - 1)]
+    y = y[n_fft // 2: n_fft // 2 + hop * (nfr - 1)]
+    return (y, i) if return_cut else y
+
+
+def _np_dtype(t):
+    return torch.empty(0, dtype=t.dtype).numpy().dtype
 
 
 def restore_inmem(wav, ana, voc, mode=0, drop_masks_fn=None):
-    """VoiceFixer.restore_inmem base.py:106-139: np (L,) -> np (1, N) float32.  30 s segments,
-    independent, concatenated (SURVEY D4).  mode 2 = train-mode BN (+ dropout if masks given)."""
-    wav = np.asarray(wav, dtype=np.float32)
+    """VoiceFixer.restore_inmem base.py:106-139: np (L,) -> np (1, N) in the state dicts' dtype (float32 for the
+    checkpoints as stored).  30 s segments, independent, concatenated (SURVEY D4).  mode 2 = train-mode BN (+ dropout
+    if masks given).  The samples are read as float32, as the reference reads them."""
+    like = ana["mel.fb"]
+    dt = _np_dtype(like)
+    wav = np.asarray(np.asarray(wav, dtype=np.float32), dtype=dt)
     train = (mode == 2)
     res = []
     break_point = SEG_LEN
     while break_point < wav.shape[0] + SEG_LEN:
         segment = wav[break_point - SEG_LEN: break_point]
         if mode == 1:
-            segment = remove_higher_frequency(segment)
-        _, mel = frontend(torch.from_numpy(np.ascontiguousarray(segment))[None], ana)
+            segment = remove_higher_frequency(segment, dtype=dt)
+        _, mel = frontend(torch.from_numpy(np.ascontiguousarray(segment))[None].to(like.device), ana)
         masks = drop_masks_fn(mel.shape[2]) if (train and drop_masks_fn) else None
         out_mel = analysis(mel, ana, train, masks)
         out = vocoder_forward(from_log(out_mel), voc)
         out = trim_center(out, segment.shape[-1])
         res.append(out)
         break_point += SEG_LEN
-    return torch.cat(res, -1).squeeze(0).numpy()
+    return torch.cat(res, -1).squeeze(0).cpu().numpy()
 
 
 # --------------------------------------------------------------------------- oracle() front end
@@ -372,28 +490,35 @@ def slaney_htk_mel_basis():
     return weights.astype(np.float32)
 
 
-def oracle_cond(wav):
+def oracle_cond(wav, dtype=torch.float32):
     """Vocoder.oracle front end vocoder/base.py:61-73: peak-normalise, |librosa.stft|
     (n_fft 2048, hop 441, hann, center, pad_mode='constant' per librosa 0.10.1), Slaney mel,
     dB-20, normalise, pre() -> cond (1,128,T+T%2+4).  librosa's stft multiplies the float32 frames by
-    get_window's float64 window without a cast: the windowed frames are float64."""
-    wav = np.asarray(wav, dtype=np.float32)
+    get_window's float64 window without a cast: the windowed frames are float64.
+    dtype: torch.float32 (the reference's arithmetic and result) or torch.float64 (float64 throughout, on the
+    float32 samples and the float32 Slaney basis)."""
+    f64 = dtype == torch.float64
+    wav = np.asarray(np.asarray(wav, dtype=np.float32), dtype=np.float64 if f64 else np.float32)
     wav = wav / np.max(np.abs(wav))
     win = 0.5 - 0.5 * np.cos(2 * np.pi * np.arange(N_FFT) / N_FFT)
     x = np.pad(wav, (N_FFT // 2, N_FFT // 2), mode="constant")
     nfr = 1 + (len(x) - N_FFT) // HOP
     idx = np.arange(N_FFT)[None, :] + HOP * np.arange(nfr)[:, None]
-    stft = np.abs(np.fft.rfft(x[idx] * win[None, :], axis=1).T.astype(np.complex64))
-    mel = np.dot(slaney_htk_mel_basis(), stft)
+    stft = np.fft.rfft(x[idx] * win[None, :], axis=1).T
+    stft = np.abs(stft if f64 else stft.astype(np.complex64))
+    basis = slaney_htk_mel_basis()
+    mel = np.dot(basis.astype(np.float64) if f64 else basis, stft)
     min_level = np.exp(-100 / 20 * np.log(10))
     S = 20 * np.log10(np.maximum(min_level, np.abs(mel))) - 20
     S = np.clip(8.0 * ((S + 115.0) / 115.0) - 4.0, -4.0, 4.0)
-    c = torch.FloatTensor(np.transpose(S, (1, 0))).unsqueeze(0).transpose(1, 2)
+    c = torch.from_numpy(np.ascontiguousarray(np.transpose(S, (1, 0)))).to(dtype).unsqueeze(0).transpose(1, 2)
     pad_tail = c.size(-1) % 2 + 4
-    return torch.cat([c, torch.zeros(1, N_MEL, pad_tail) - 4.0], -1)
+    return torch.cat([c, torch.zeros(1, N_MEL, pad_tail, dtype=dtype) - 4.0], -1)
 
 
 def oracle_wave(wav, voc):
     """Vocoder.oracle vocoder/base.py:58-77 up to (not including) the file write:
-    returns float wav_re * 2**15 as np (1, 1, S)."""
-    return (vocoder_generator(oracle_cond(wav), voc) * 2 ** 15).numpy()
+    returns float wav_re * 2**15 as np (1, 1, S), in the dtype and on the device of voc."""
+    like = voc["condnet.0.bias"]
+    cond = oracle_cond(wav, like.dtype).to(like.device)
+    return (vocoder_generator(cond, voc) * 2 ** 15).cpu().numpy()
