@@ -5,6 +5,10 @@ brings from L2 into shared memory (per K slice one A box of 128 rows x 128 bytes
 holds fewer, and one BN x 128-byte weight box; whole boxes, zero fill included), and the FLOP the tensor cores execute per slice (2 * 128 * BN * channels per
 slice, padding included).  With a GPU: the kernel time by CUDA events, and from it the L2 -> shared-memory rate, the
 executed TFLOP/s and the time one CTA spends per slice (time * CTAs / slices; the CTAs are min(tiles, SMs)).
+Each shape is timed twice: with a light epilogue (raw output only) and with the restore step's (bias, an fp32 residual,
+raw output and the activated operand for the next layer); the difference, per tile and CTA, is what the epilogue costs.
+The ResStack C = 128 shape is also timed as the tf32 step runs its second convolution: the encoded stream read as the
+residual and overwritten in place.
 Shapes: the four ResStack widths, the UNet's 32- and 64-channel 3x3 on 127 bins, one up-sampler phase group.
 usage: python tools/bench_conv_feed.py [--dry] [--prec tf32|bf16|fp16] [--B 8] [--iters 5]"""
 import argparse, os, sys
@@ -67,13 +71,29 @@ for name, H, W, Cin, N, taps, mats in SHAPES:
     w = (torch.randn(nmat, N, Cin, device="cuda:0") * 0.05).to(odt)
     w_off = [i * N * Cin for i in mats] if mats else None
     raw = torch.empty(args.B, H, W, N, device="cuda:0")
-    run = lambda: conv_gemm(a, w, taps, N=N, w_off=w_off, precision=args.prec, impl=1, out_raw=raw)
-    run()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(args.iters):
+    bias = torch.randn(N, device="cuda:0") * 0.1
+    res = torch.randn(args.B, H, W, N, device="cuda:0")
+    act = torch.empty(args.B, H, W, N, device="cuda:0", dtype=odt)
+    runs = [("light", lambda: conv_gemm(a, w, taps, N=N, w_off=w_off, precision=args.prec, impl=1, out_raw=raw)),
+            ("step", lambda: conv_gemm(a, w, taps, N=N, w_off=w_off, precision=args.prec, impl=1, out_raw=raw, bias=bias,
+                                       residual=res, want_act=True, out_act=act, act="lrelu", act_param=0.01))]
+    if name == "resstack C=128":
+        enc = res.clone()
+        runs.append(("step, encoded stream in place",
+                     lambda: conv_gemm(a, w, taps, N=N, w_off=w_off, precision=args.prec, impl=1, out_raw=enc, bias=bias,
+                                       residual=enc, res_enc=1, raw_enc=1, enc_slope=0.01, want_act=True, out_act=act,
+                                       act="lrelu", act_param=0.01)))
+    light = None
+    for label, run in runs:
         run()
-    e1.record(); torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / args.iters
-    print(f"    {ms:8.3f} ms  L2->smem {m['bytes'] / ms / 1e9:6.2f} TB/s  executed {m['flop'] / ms / 1e9:6.1f} TFLOP/s  "
-          f"{ms * 1e3 * m['ctas'] / (m['tiles'] * m['slices']):6.3f} us per slice per CTA", flush=True)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.iters):
+            run()
+        e1.record(); torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / args.iters
+        per_slice = ms * 1e3 * m['ctas'] / (m['tiles'] * m['slices'])
+        extra = "" if light is None else f"  epilogue {(per_slice - light) * m['slices']:6.2f} us per tile per CTA over light"
+        light = per_slice if light is None else light
+        print(f"    {label:30s} {ms:8.3f} ms  L2->smem {m['bytes'] / ms / 1e9:6.2f} TB/s  executed {m['flop'] / ms / 1e9:6.1f} TFLOP/s  "
+              f"{per_slice:6.3f} us per slice per CTA{extra}", flush=True)

@@ -21,7 +21,8 @@
 //    two partial accumulators, while the previous slice's partial is added to the fp32 accumulator.
 //  - Staged epilogue: the tile goes through a shared fp32 buffer and is processed row by row (bias, fp32 residual,
 //    eval-BN affine, activation, operand for the next layer), with 16-byte accesses where the host found every pointer,
-//    stride and column offset aligned.
+//    stride and column offset aligned.  A thread's column parameters are read once per tile and all its residual rows
+//    are loaded before its first store, so a tile waits on global memory once, not once per row.
 // kind tf32 reads fp32 operands and ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the
 // encoded stream of vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.
 // Ragged batches (seq_in / seq_out): each item's extent on the sequence axis acts as that item's own edge, so every row
@@ -29,7 +30,9 @@
 //
 // What still stands between this kernel and the roof: the A halo of the taps is re-read from L2 for every tap, every
 // CTA reads its own copy of the weights from L2, the ring is 4 stages deep at BN = 128 (the fp32 epilogue buffer takes
-// the rest of shared memory), and the per-slice sum costs BN / 2 FADDs per slice in the consumers.
+// the rest of shared memory), the per-slice sum costs BN / 2 FADDs per slice in the consumers, and the epilogue runs
+// after the K loop with the tensor cores idle: its residual loads are issued together but only once the K loop is done,
+// and its stores do not overlap the next tile's wgmma.
 #include <atomic>
 #include <cuda.h>      // CUtensorMap and the types of its encoder; the encoder itself is looked up at run time
 #include "tc_ptx.cuh"
@@ -108,16 +111,17 @@ template <bool SEQ> __device__ __forceinline__ bool row_stored(const vfx_conv_de
   return oh < d.OH && ow < d.OW && (!SEQ || !d.seq_out || (d.seq_axis ? ow : oh) < d.seq_out[b]);
 }
 
-// one output element, in the order every path keeps: bias, then the residual (rv, decoded when encoded), then the raw
-// output (encoded when asked), then the BN affine and the activation of the operand
-__device__ __forceinline__ float add_in(const vfx_conv_desc& d, float v, int n, float rv) {
-  if (d.bias) v += d.bias[n % d.bias_mod];
+// one output element, in the order every path keeps: bias (bv = bias[n % bias_mod]), then the residual (rv, decoded
+// when encoded), then the raw output (encoded when asked), then the BN affine (sc, sf = act_scale[n], act_shift[n]) and
+// the activation of the operand
+__device__ __forceinline__ float add_in(const vfx_conv_desc& d, float v, float bv, float rv) {
+  if (d.bias) v += bv;
   if (d.residual) v += d.res_enc ? stream_dec(rv, 1.0f / d.enc_slope) : rv;
   return v;
 }
 __device__ __forceinline__ float raw_out(const vfx_conv_desc& d, float v) { return d.raw_enc ? stream_enc(v, d.enc_slope) : v; }
-__device__ __forceinline__ float act_out(const vfx_conv_desc& d, float v, int n) {
-  const float va = d.act_scale ? fmaf(v, d.act_scale[n], d.act_shift[n]) : v;
+__device__ __forceinline__ float act_out(const vfx_conv_desc& d, float v, float sc, float sf) {
+  const float va = d.act_scale ? fmaf(v, sc, sf) : v;
   return apply_act(va, d.act, d.act_param);
 }
 
@@ -338,37 +342,80 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
     }
     named_sync(2, 256);
 
-    // row by row: BN / 4 threads per row, 4 consecutive columns each
-    constexpr int TPR = BN / 4, RPP = 256 / TPR;
-    const int c4 = (ct % TPR) * 4, n = n0 + c4;
+    // row by row: BN / 4 threads per row, 4 consecutive columns each, rows r0 + RPP i
+    constexpr int TPR = BN / 4, RPP = 256 / TPR, RPT = BM / RPP;
+    const int c4 = (ct % TPR) * 4, n = n0 + c4, r0 = ct / TPR;
     if (n >= d.N) continue;
-    const bool full = vec && n + 4 <= d.N;
-    for (int r = ct / TPR; r < BM; r += RPP) {
+    const int ncol = d.N - n < 4 ? d.N - n : 4;
+    const bool full = vec && ncol == 4;
+    // The thread's columns are the same in every row: their parameters are read once per tile.
+    float bv[4], sc[4], sf[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int ne = e < ncol ? n + e : n;            // columns from N on are not stored
+      bv[e] = d.bias ? d.bias[ne % d.bias_mod] : 0.f;
+      sc[e] = d.act_scale ? d.act_scale[ne] : 1.f;
+      sf[e] = d.act_scale ? d.act_shift[ne] : 0.f;
+    }
+    if (d.residual) {
+      // All of the thread's residual rows are loaded before any is used and before its first store, so the tile waits
+      // for memory once and not once per row (the compiler cannot move a load above a store it may alias: the tf32
+      // ResStack writes the encoded stream in place over its residual).  That is safe because each residual element is
+      // read by the thread that writes the same element of out_raw, and by no other: the residual's element (row, n) is
+      // the output's (row, n) or lies outside it.  Bias and residual are then added into the staged tile, so that the
+      // unrolled part stays small; the row pass below is a loop (unrolled with its stores, it overflows the
+      // instruction cache).
+      float4 rv[RPT];
+#pragma unroll
+      for (int i = 0; i < RPT; ++i) {
+        const OutRow& o = crow[r0 + RPP * i];
+        rv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (o.ok) {
+          const float* p = d.residual + o.res + n;
+          if (full) {
+            rv[i] = *reinterpret_cast<const float4*>(p);
+          } else {
+            rv[i].x = p[0];
+            if (ncol > 1) rv[i].y = p[1];
+            if (ncol > 2) rv[i].z = p[2];
+            if (ncol > 3) rv[i].w = p[3];
+          }
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < RPT; ++i) {
+        const int r = r0 + RPP * i;
+        if (!crow[r].ok) continue;
+        float4* q = reinterpret_cast<float4*>(epi + r * C::EPI_LD + c4);
+        const float4 v = *q;
+        *q = make_float4(add_in(d, v.x, bv[0], rv[i].x), add_in(d, v.y, bv[1], rv[i].y), add_in(d, v.z, bv[2], rv[i].z),
+                         add_in(d, v.w, bv[3], rv[i].w));
+      }
+    }
+    for (int r = r0; r < BM; r += RPP) {
       const OutRow o = crow[r];
       if (!o.ok) continue;
-      const float* src = epi + r * C::EPI_LD + c4;
+      float4 v = *reinterpret_cast<const float4*>(epi + r * C::EPI_LD + c4);
+      if (!d.residual)
+        v = make_float4(add_in(d, v.x, bv[0], 0.f), add_in(d, v.y, bv[1], 0.f), add_in(d, v.z, bv[2], 0.f), add_in(d, v.w, bv[3], 0.f));
       if (full) {
-        float4 v = *reinterpret_cast<const float4*>(src);
-        if (d.residual) {
-          const float4 rv = *reinterpret_cast<const float4*>(d.residual + o.res + n);
-          v = make_float4(add_in(d, v.x, n, rv.x), add_in(d, v.y, n + 1, rv.y), add_in(d, v.z, n + 2, rv.z), add_in(d, v.w, n + 3, rv.w));
-        } else {
-          v = make_float4(add_in(d, v.x, n, 0.f), add_in(d, v.y, n + 1, 0.f), add_in(d, v.z, n + 2, 0.f), add_in(d, v.w, n + 3, 0.f));
-        }
         if (d.out_raw)
           *reinterpret_cast<float4*>(d.out_raw + o.raw + n) = make_float4(raw_out(d, v.x), raw_out(d, v.y), raw_out(d, v.z), raw_out(d, v.w));
         if (out_act) {
-          const float y0 = act_out(d, v.x, n), y1 = act_out(d, v.y, n + 1), y2 = act_out(d, v.z, n + 2), y3 = act_out(d, v.w, n + 3);
+          const float y0 = act_out(d, v.x, sc[0], sf[0]), y1 = act_out(d, v.y, sc[1], sf[1]);
+          const float y2 = act_out(d, v.z, sc[2], sf[2]), y3 = act_out(d, v.w, sc[3], sf[3]);
           if (ESZ == 4)
             *reinterpret_cast<float4*>(out_act + o.act + n) = make_float4(round_tf32(y0), round_tf32(y1), round_tf32(y2), round_tf32(y3));
           else
             *reinterpret_cast<uint2*>(out_act + o.act + n) = make_uint2(pack16<KIND == 2>(y0, y1), pack16<KIND == 2>(y2, y3));
         }
       } else {
-        for (int e = 0; e < 4 && n + e < d.N; ++e) {
-          const float v = add_in(d, src[e], n + e, d.residual ? d.residual[o.res + n + e] : 0.f);
-          if (d.out_raw) d.out_raw[o.raw + n + e] = raw_out(d, v);
-          if (out_act) out_act[o.act + n + e] = from_f<T>(act_out(d, v, n + e));
+        const float ve[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          if (e >= ncol) break;
+          if (d.out_raw) d.out_raw[o.raw + n + e] = raw_out(d, ve[e]);
+          if (out_act) out_act[o.act + n + e] = from_f<T>(act_out(d, ve[e], sc[e], sf[e]));
         }
       }
     }

@@ -146,6 +146,23 @@ __global__ void __launch_bounds__(256) pair_fused_kernel(const __grid_constant__
   run(NITER);
   float* dst = d.x_out ? d.x_out : d.x;
   T* out_act = reinterpret_cast<T*>(d.out_act);
+  // acc + b2 and every residual element of the thread are loaded before the first store, so the stores (which may
+  // overwrite x in place) do not serialise the loads; each element is read and written by this thread alone.
+  float xr[C / 2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int i = wg * 64 + w * 16 + (l >> 2) + 8 * h, g = r0 + i;
+    const bool live = i < P_ROWS && g < L;
+    const long long row = item + (long long)g * C;
+#pragma unroll
+    for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = 8 * j + 2 * (l & 3) + e;
+        acc[4 * j + 2 * h + e] += d.b2[n];
+        xr[4 * j + 2 * h + e] = live ? d.x[row + n] : 0.f;
+      }
+  }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int i = wg * 64 + w * 16 + (l >> 2) + 8 * h, g = r0 + i;
@@ -156,8 +173,8 @@ __global__ void __launch_bounds__(256) pair_fused_kernel(const __grid_constant__
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int n = 8 * j + 2 * (l & 3) + e;
-        const float r = d.x[row + n];
-        const float v = acc[4 * j + 2 * h + e] + d.b2[n] + (d.stream_enc ? stream_dec(r, 100.0f) : r);
+        const float r = xr[4 * j + 2 * h + e];
+        const float v = acc[4 * j + 2 * h + e] + (d.stream_enc ? stream_dec(r, 100.0f) : r);
         if (d.write_raw) dst[row + n] = (d.stream_enc && d.stream_enc_out) ? stream_enc(v, 0.01f) : v;
         if (out_act) out_act[row + n] = from_f<T>(apply_act(v, d.act, d.act_param));
       }
