@@ -276,7 +276,9 @@ int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream)
 /* Fused ResStack pair on the wgmma tensor cores:
  *   x' = x + conv2_{k3,d=1}( lrelu_0.01( conv1_{k3,dilation}( a ) + b1 ) ) + b2
  * ResStack.forward voicefixer/vocoder/model/modules.py:592-595 (layers :550-576).
- * form: VFX_PAIR_FUSED = one kernel on one SM per block of rows, the intermediate h kept in shared memory (no scratch);
+ * form: VFX_PAIR_FUSED = one persistent kernel (a CTA per SM walking blocks of rows), the intermediate h kept in shared
+ * memory (no scratch); it needs a, w1, w2 16-byte aligned, x / x_out 8-byte aligned and out_act aligned to two elements
+ * (VFX_ERR_UNSUPPORTED otherwise);
  * VFX_PAIR_BLOCKED = the two convolutions of vfx_conv_gemm per block of rows with h in `scratch` (required:
  * vfx_resstack_pair_scratch_bytes() bytes, 128-byte aligned), the reference the fused form is tested against.  Any other
  * form returns VFX_ERR_INVALID.

@@ -33,8 +33,6 @@
 // the rest of shared memory), the per-slice sum costs BN / 2 FADDs per slice in the consumers, and the epilogue runs
 // after the K loop with the tensor cores idle: its residual loads are issued together but only once the K loop is done,
 // and its stores do not overlap the next tile's wgmma.
-#include <atomic>
-#include <cuda.h>      // CUtensorMap and the types of its encoder; the encoder itself is looked up at run time
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -420,34 +418,6 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       }
     }
   }
-}
-
-int sm_count(int dev) {
-  static std::atomic<int> sms[64];                    // per device, queried once (host threads may drive several devices)
-  if (dev < 64) {
-    const int n = sms[dev].load(std::memory_order_relaxed);
-    if (n) return n;
-  }
-  int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 0;
-  if (dev < 64) sms[dev].store(n, std::memory_order_relaxed);
-  return n;
-}
-
-// cuTensorMapEncodeTiled, through the runtime (the library calls nothing else of the driver API)
-using EncodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiled tensor_map_encoder() {
-  static const EncodeTiled fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    return reinterpret_cast<EncodeTiled>(p);
-  }();
-  return fn;
 }
 
 // The tile boxes and the two tensor maps of a launch without per-item extents.  Returns 1 with `tp` filled, 0 where a

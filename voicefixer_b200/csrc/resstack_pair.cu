@@ -1,16 +1,33 @@
 // ResStack pair x' = x + conv2_{k3,d=1}(lrelu_0.01(conv1_{k3,dilation}(a) + b1)) + b2 (include/vfx_b200.h,
 // vfx_resstack_pair), ResStack.forward voicefixer/vocoder/model/modules.py:592-595.
 //
-// Fused form (VFX_PAIR_FUSED; the engine's fused pairs): one CTA per 126 output rows of one item, two warpgroups.
-// conv1 computes h for the 128 rows [r0 - 1, r0 + 127) with wgmma (a staged by cp.async into 128-byte-swizzled tiles,
-// W1 streamed through the same 3-stage ring); its epilogue writes lrelu(h + b1) in the operand format into shared
-// memory three times, copy t shifted up by t rows, so that conv2's tap t reads copy t as an ordinary K-major A tile
-// (rows outside [0, L) are zero: conv2's padding).  conv2 streams W2 through the ring, accumulates in registers and its
-// epilogue adds b2 and the residual and writes x' / act(x').  h never leaves the SM: HBM traffic is a (with a halo),
-// the residual and the outputs.  Shared memory: 3 copies of h (48 KB bf16 C = 64, 96 KB tf32 C = 64 or 16-bit C = 128)
-// + 3 stages of (16 KB of a + C x 128 B of weights).
-//
-// Ragged batches (vfx_pair_desc.lens): item b is computed as if its length were lens[b]; tiles starting beyond it exit.
+// Fused form (VFX_PAIR_FUSED; the engine's fused pairs): a persistent, warp-specialised kernel.  grid = min(tiles, SMs);
+// a tile is 126 output rows of one item, and each CTA walks a static stride over the (item, row block) tiles with the
+// row block fastest, so that neighbouring CTAs work on neighbouring rows and the dilation halo comes from L2.
+//  - Producer warpgroup: per tile, conv1's 3 x NKS K slices (the 128 a rows [r0 - 1, r0 + 127) shifted by the tap, and
+//    the tap's W1 rows), then conv2's 3 x NKS slices (W2 rows only), into a ring of 128-byte-swizzled K-major tiles handed
+//    over through full / empty mbarriers.  It runs ahead into the next tile's conv1 while the consumers finish conv2 and
+//    the epilogue of this one.  Two forms:
+//      TMA (launches without lens): one thread issues a box of the (C, L, B) operand map at row r0 - 1 + (tap - 1) *
+//      dilation and a box of the [3][C][C] weight map per slice; the out-of-bounds fill is conv1's zero padding.
+//      cp.async (ragged batches): the warpgroup stages 16-byte chunks with zero fill beyond the item's own length.
+//  - Two consumer warpgroups, 64 rows each: conv1 with one wgmma group in flight into one of two partials while the
+//    previous slice's partial is added to the fp32 accumulator (conv_gemm_tc.cu's K loop); its epilogue writes lrelu(h +
+//    b1) in the operand format into shared memory three times, copy t shifted up by t rows, so that conv2's tap t reads
+//    copy t as an ordinary K-major A tile (rows outside [0, L) are zero: conv2's padding).  The h copies are one buffer:
+//    a named barrier keeps the next tile's h writes behind this tile's last conv2 wgmma.  conv2 runs the same K loop
+//    from the h copies and its epilogue adds b2 and the residual and writes x' / act(x').
+//  - Nothing global in the epilogues' critical path: b1 and b2 are staged in shared memory once per CTA.  In tf32 the
+//    residual (the encoded stream, a == x) is rows 1 ... 126 of conv1's centre-tap A tiles, which are kept out of the
+//    ring for that, read into registers in the h epilogue and then released to the producer (one mbarrier).  In the
+//    16-bit modes x is a separate fp32 tensor: at C = 64 the residual is loaded into registers before conv2's K loop,
+//    at C = 128 (no registers to spare beside the accumulator and two partials) it is prefetched into L2 then and
+//    loaded after the K loop.
+// h never leaves the SM: HBM traffic is a (with a halo), the residual (16-bit modes) and the outputs.  Shared memory:
+// the h copies (3 x 128 rows x C x e: 48 KB bf16 / fp16 C = 64, 96 KB tf32 C = 64 or 16-bit C = 128), the tf32 centre
+// tiles (32 KB), the ring (16 KB of a + C x 128 B of weights per stage: 4 stages tf32, 7 16-bit C = 64, 4 C = 128).
+// Every sum is in the order of the blocked form: per K slice 4 wgmma into a zeroed partial, partials added in (tap,
+// channel slice) order with round-to-nearest fp32 adds, then (acc + b) + residual.
 //
 // Blocked form (VFX_PAIR_BLOCKED, the tests' reference): conv_gemm_tc.cu's two convolutions per row block, h in a scratch.
 #include <string.h>
@@ -27,174 +44,378 @@ template <> struct PairT<0> { using T = tf32_t; static constexpr int ESZ = 4; };
 template <> struct PairT<1> { using T = __nv_bfloat16; static constexpr int ESZ = 2; };
 template <> struct PairT<2> { using T = __half; static constexpr int ESZ = 2; };
 
-constexpr int P_ROWS = 126, P_STAGES = 3, P_A_BYTES = 128 * 128;
+constexpr int P_ROWS = 126, P_NT = 384, P_A_BYTES = 128 * 128;   // warpgroup 0 produces, warpgroups 1 and 2 consume
+constexpr int P_SMEM_MAX = 227 * 1024;
+constexpr int P_PROD_REGS = 56, P_CONS_REGS = 224;               // 128 x 56 + 256 x 224 <= 384 x 168
 
-template <int C, int KIND> constexpr int pair_nks() { return C * PairT<KIND>::ESZ / 128; }
-template <int C, int KIND> constexpr int pair_smem() {
-  return P_STAGES * (P_A_BYTES + C * 128) + 3 * pair_nks<C, KIND>() * 16384 + 1024;
-}
+template <int C, int KIND> struct PairCfg {
+  static constexpr int ESZ = PairT<KIND>::ESZ, NKS = C * ESZ / 128, NITER = 3 * NKS;   // K slices per convolution
+  static constexpr int STAGE = P_A_BYTES + C * 128;
+  static constexpr int H = 3 * NKS * 16384;                       // the three h copies
+  static constexpr int CTR = KIND == 0 ? NKS * 16384 : 0;         // tf32: conv1's centre-tap A tiles (the residual)
+  static constexpr int FIXED = 1024 + H + CTR + 2 * C * 4 + 8;    // + ring alignment, b1 / b2, the centre's barrier
+  static constexpr int FIT = (P_SMEM_MAX - FIXED) / (STAGE + 16);
+  static constexpr int STAGES = FIT < 8 ? FIT : 8;
+  // cp.async: slice k is signalled full after slice k + AHEAD is issued (conv_gemm_tc.cu's Cfg::AHEAD)
+  static constexpr int AHEAD = STAGES - 2;
+  static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
+  static_assert(STAGES >= 3 && SMEM <= P_SMEM_MAX, "resstack_pair: shared-memory plan");
+};
 
-// element n of row j of an h copy (K-major, 128-byte slices of 16 KB, 128-byte swizzle)
+// What a TMA launch carries beside the descriptor: the operand (C, L, B), box (128 bytes, 128 rows, 1), and the two
+// weight arrays (C, C, 3), box (128 bytes, C rows, 1)
+struct PairMaps { CUtensorMap a, w1, w2; };
+
+// element n of row j of an h copy (K-major, 128-byte slices of 16 KB, 128-byte swizzle); also the layout of conv1's
+// centre-tap A tiles
 template <int ESZ> __device__ __forceinline__ uint32_t h_offset(int j, int n) {
   const int kb = n * ESZ;
   return (uint32_t)((kb >> 7) * 16384 + j * 128 + ((((kb & 127) >> 4) ^ (j & 7)) << 4) + (kb & 15));
 }
 
-template <int C, int KIND>
-__global__ void __launch_bounds__(256) pair_fused_kernel(const __grid_constant__ vfx_pair_desc d) {
+// tile t -> item b, its first output row r0 and the item's length L; false where the tile holds no row of its item (a
+// ragged batch's rows at or beyond lens[b]).  The producer and the consumers skip tiles by this function alone.
+__device__ __forceinline__ bool pair_tile(const vfx_pair_desc& d, int nrb, int t, int& b, int& r0, int& L) {
+  b = t / nrb;
+  r0 = (t - b * nrb) * P_ROWS;
+  L = d.lens ? d.lens[b] : d.L;
+  return r0 < L;
+}
+
+template <int C, int KIND, bool TMA>
+__global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_constant__ vfx_pair_desc d,
+                                                             const __grid_constant__ PairMaps m, const int niter) {
   using T = typename PairT<KIND>::T;
-  constexpr int ESZ = PairT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ, NKS = pair_nks<C, KIND>();
-  constexpr int STAGE = P_A_BYTES + C * 128, NITER = 3 * NKS;
+  using G = PairCfg<C, KIND>;
+  constexpr int ESZ = G::ESZ, AL = 16 / ESZ, BK = 128 / ESZ, NKS = G::NKS, NITER = G::NITER;
+  constexpr int S = G::STAGES, STAGE = G::STAGE, AHEAD = G::AHEAD;
+  constexpr bool EARLY = KIND != 0 && C == 64;    // 16-bit C = 64: the residual goes to registers before conv2
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t hbase = sbase + P_STAGES * STAGE;
-  uint8_t* const hgen = smem_raw + (hbase - smem_u32(smem_raw));
+  uint8_t* const gbase = smem_raw + (sbase - smem_u32(smem_raw));
+  const uint32_t hbase = sbase + S * STAGE, cbase = hbase + G::H;
+  uint8_t* const hgen = gbase + S * STAGE;
+  const uint8_t* const cgen = hgen + G::H;
+  float* const bias = reinterpret_cast<float*>(hgen + G::H + G::CTR);          // b1[C], b2[C]
+  const uint32_t full0 = cbase + G::CTR + 2 * C * 4, empty0 = full0 + 8 * S, cempty = empty0 + 8 * S;
 
-  const int tid = threadIdx.x, chunk = tid & 7, lrow = tid >> 3, wg = tid >> 7, w = (tid >> 5) & 3, l = tid & 31;
-  const int b = blockIdx.y, r0 = blockIdx.x * P_ROWS;
-  const long long item = (long long)b * d.L * C;
-  const int L = d.lens ? d.lens[b] : d.L;         // this item's length (ragged batch): its rows beyond are padding
-  if (r0 >= L) return;
-  const char* __restrict__ A = reinterpret_cast<const char*>(d.a) + item * ESZ;
-  const char* __restrict__ W1 = reinterpret_cast<const char*>(d.w1);
-  const char* __restrict__ W2 = reinterpret_cast<const char*>(d.w2);
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full0 + 8 * s, TMA ? 1 : 128);      // the issuing thread's expect_tx + the bytes, or every producer thread
+      mbar_init(empty0 + 8 * s, 8);                 // every consumer warp, after its wgmma group has read the stage
+    }
+    mbar_init(cempty, 8);                           // every consumer warp, after it has read its residual rows
+  }
+  for (int i = tid; i < 2 * C; i += P_NT) bias[i] = i < C ? d.b1[i] : d.b2[i - C];
+  __syncthreads();
+  // derived after each role's setmaxnreg, so that nothing stays live across it
+#define VFX_PAIR_WALK const int nrb = (d.L + P_ROWS - 1) / P_ROWS, ntiles = d.B * nrb;
 
-  // phase 1 (it < NITER): a rows + W1; phase 2: W2 only (a comes from the h copies)
-  auto load = [&](int it, int s) {
-    const bool p2 = it >= NITER;
-    const int k = p2 ? it - NITER : it, tap = k / NKS, c = (k % NKS) * BK + chunk * AL;
-    const uint32_t sa = sbase + s * STAGE, sb = sa + P_A_BYTES;
-    if (!p2) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = lrow + 32 * i, g = r0 - 1 + r + (tap - 1) * d.dilation;
-        const bool ok = g >= 0 && g < L;
-        cp_async16(sa + sw128_offset(r, chunk), ok ? A + ((long long)g * C + c) * ESZ : A, ok);
+  if (tid < 128) {
+    // ================================================================ producer
+    setmaxnreg_dec<P_PROD_REGS>();
+    VFX_PAIR_WALK
+    uint32_t k = 0, u = 0;                          // K slices issued, tiles staged by this CTA
+    if constexpr (TMA) {
+      if (tid != 0) return;
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++u) {
+        int b, r0, L;
+        pair_tile(d, nrb, t, b, r0, L);
+        for (int it = 0; it < 2 * NITER; ++it, ++k) {
+          const int s = k % S;
+          if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+          const bool p2 = it >= NITER;
+          const int kk = p2 ? it - NITER : it, tap = kk / NKS, ks = kk - tap * NKS;
+          const uint32_t sa = sbase + s * STAGE, full = full0 + 8 * s;
+          if (!p2) {
+            const bool ctr = KIND == 0 && tap == 1;
+            if (ctr && ks == 0 && u > 0) mbar_wait(cempty, (u - 1) & 1);   // the last tile's residual has been read
+            mbar_expect_tx(full, P_A_BYTES + C * 128);
+            tma_load_3d(ctr ? cbase + ks * 16384 : sa, &m.a, full, ks * BK, r0 - 1 + (tap - 1) * d.dilation, b);
+          } else {
+            mbar_expect_tx(full, C * 128);
+          }
+          tma_load_3d(sa + P_A_BYTES, p2 ? &m.w2 : &m.w1, full, ks * BK, 0, tap);
+        }
       }
+      return;
     }
-    const char* Wt = p2 ? W2 : W1;
+    // this thread's staging work: chunk `chunk` of a rows lrow + 16 i and of weight rows lrow + 16 i
+    const int chunk = tid & 7, lrow = tid >> 3;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      int b, r0, L;
+      if (!pair_tile(d, nrb, t, b, r0, L)) continue;
+      const char* A = static_cast<const char*>(d.a) + (long long)b * d.L * C * ESZ;
+      for (int it = 0; it < 2 * NITER; ++it, ++k) {
+        const int s = k % S;
+        if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+        const bool p2 = it >= NITER;
+        const int kk = p2 ? it - NITER : it, tap = kk / NKS, ks = kk - tap * NKS, c = ks * BK + chunk * AL;
+        const uint32_t sa = sbase + s * STAGE;
+        if (!p2) {
+          const bool ctr = KIND == 0 && tap == 1;
+          if (ctr && ks == 0 && u > 0) mbar_wait(cempty, (u - 1) & 1);
+          const uint32_t dst = ctr ? cbase + ks * 16384 : sa;
 #pragma unroll
-    for (int i = 0; i < C / 32; ++i) {
-      const int n = lrow + 32 * i;
-      cp_async16(sb + sw128_offset(n, chunk), Wt + ((long long)tap * C * C + (long long)n * C + c) * ESZ, true);
-    }
-  };
-
-  float acc[C / 2];
-  auto run = [&](int it0) {            // NITER K slices starting at global iteration it0 (stage = it % P_STAGES)
+          for (int i = 0; i < 8; ++i) {
+            const int r = lrow + 16 * i, g = r0 - 1 + r + (tap - 1) * d.dilation;
+            const bool ok = g >= 0 && g < L;
+            cp_async16(dst + sw128_offset(r, chunk), ok ? A + ((long long)g * C + c) * ESZ : A, ok);
+          }
+        }
+        const char* W = static_cast<const char*>(p2 ? d.w2 : d.w1) + ((long long)tap * C * C + c) * ESZ;
 #pragma unroll
-    for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-    for (int s = 0; s < P_STAGES - 1; ++s) {
-      load(it0 + s, (it0 + s) % P_STAGES);
-      cp_async_commit();
-    }
-    for (int k = 0; k < NITER; ++k) {
-      const int it = it0 + k;
-      cp_async_wait<P_STAGES - 2>();
-      fence_proxy_async();
-      __syncthreads();
-      if (k + P_STAGES - 1 < NITER) load(it + P_STAGES - 1, (it + P_STAGES - 1) % P_STAGES);
-      cp_async_commit();
-      const uint32_t sa = sbase + (it % P_STAGES) * STAGE;
-      const uint32_t a_tile = it < NITER ? sa + wg * 64 * 128 : hbase + (uint32_t)k * 16384 + wg * 64 * 128;
-      const uint64_t da = sw128_desc(a_tile), db = sw128_desc(sa + P_A_BYTES);
-      float part[C / 2];
-#pragma unroll
-      for (int i = 0; i < C / 2; ++i) part[i] = 0.f;
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) Wgmma<C, KIND>::mma(part, da + 2 * kk, db + 2 * kk);
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < C / 2; ++i) acc[i] += part[i];     // round-to-nearest sum of the slices (conv_gemm_tc.cu)
+        for (int i = 0; i < C / 16; ++i) {
+          const int n = lrow + 16 * i;
+          cp_async16(sa + P_A_BYTES + sw128_offset(n, chunk), W + (long long)n * C * ESZ, true);
+        }
+        cp_async_commit();
+        if (k >= (uint32_t)AHEAD) {
+          cp_async_wait<AHEAD>();                   // this thread's chunks of slice k - AHEAD have landed
+          fence_proxy_async();                      // ... and are visible to the tensor core's (async-proxy) reads
+          mbar_arrive(full0 + 8 * ((k - AHEAD) % S));
+        }
+      }
+      ++u;
     }
     cp_async_wait<0>();
-    __syncthreads();
-  };
+    fence_proxy_async();
+    for (uint32_t j = k > (uint32_t)AHEAD ? k - AHEAD : 0; j < k; ++j) mbar_arrive(full0 + 8 * (j % S));
+    return;
+  }
 
-  // ---- conv1 -> h copies
-  run(0);
+  // ================================================================== consumers
+  setmaxnreg_inc<P_CONS_REGS>();
+  VFX_PAIR_WALK
+#undef VFX_PAIR_WALK
+  const int ct = tid - 128, cw = ct >> 7, w = (ct >> 5) & 3, l = tid & 31;
+  float* const dst = d.x_out ? d.x_out : d.x;
+  T* const out_act = reinterpret_cast<T*>(d.out_act);
+  const float* const b1 = bias;
+  const float* const b2 = bias + C;
+  float acc[C / 2], p0[C / 2], p1[C / 2], xr[C / 2];
+  // issue slice kk (slice it of the tile: conv1 for it < NITER, conv2 after) as 4 wgmma into p, zeroed
+  auto issue = [&](float (&p)[C / 2], uint32_t kk, int it) {
+    const uint32_t s = kk % S;
+    mbar_wait(full0 + 8 * s, (kk / S) & 1);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int i = wg * 64 + w * 16 + (l >> 2) + 8 * h, g = r0 - 1 + i;
-    const bool inside = g >= 0 && g < L;
+    for (int i = 0; i < C / 2; ++i) p[i] = 0.f;
+    const uint32_t sa = sbase + s * STAGE;
+    const uint32_t a_tile = it >= NITER ? hbase + (uint32_t)(it - NITER) * 16384
+                            : KIND == 0 && it / NKS == 1 ? cbase + (uint32_t)(it - NKS) * 16384 : sa;
+    const uint64_t da = sw128_desc(a_tile + cw * 64 * 128), db = sw128_desc(sa + P_A_BYTES);
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < C / 8; ++j) {
-      const int n = 8 * j + 2 * (l & 3);
-      float v0 = acc[4 * j + 2 * h] + d.b1[n], v1 = acc[4 * j + 2 * h + 1] + d.b1[n + 1];
-      v0 = inside ? (v0 > 0.f ? v0 : 0.01f * v0) : 0.f;
-      v1 = inside ? (v1 > 0.f ? v1 : 0.01f * v1) : 0.f;
+    for (int q = 0; q < 4; ++q) Wgmma<C, KIND>::mma(p, da + 2 * q, db + 2 * q);
+    wgmma_commit();
+  };
+  // slice kk's group has completed: free its stage and add it (round to nearest, in slice order)
+  auto retire = [&](float (&p)[C / 2], uint32_t kk) {
+    wgmma_fence_operand(p);
+    __syncwarp();
+    if (l == 0) mbar_arrive(empty0 + 8 * (kk % S));
 #pragma unroll
-      for (int t = 0; t < 3; ++t) {
-        const int jr = i - t;
-        if (jr < 0) continue;
-        uint8_t* dst = hgen + t * NKS * 16384 + h_offset<ESZ>(jr, n);
-        if (ESZ == 2) {
-          *reinterpret_cast<uint32_t*>(dst) = pack16<KIND == 2>(v0, v1);
-        } else {
-          *reinterpret_cast<float2*>(dst) = make_float2(round_tf32(v0), round_tf32(v1));
+    for (int i = 0; i < C / 2; ++i) acc[i] += p[i];
+    wgmma_fence_operand(acc);                       // the adds stay here, before the next slice is issued: p is reused
+  };
+  // one convolution: the niter (= NITER) slices from ring slice k0, tile slice it0; slice it goes to p[it & 1] and
+  // slice it - 1 is added while slice it is in flight.  The count is a kernel argument, as in conv_gemm_tc.cu: with
+  // the compile-time NITER, ptxas peels the loop and serialises its wgmma groups (C7514).
+  auto conv = [&](uint32_t k0, int it0) {
+#pragma unroll
+    for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+    issue(p0, k0, it0);
+    int it = 1;
+#pragma unroll 1
+    for (; it + 1 < niter; it += 2) {
+      issue(p1, k0 + it, it0 + it);
+      wgmma_wait<1>();
+      retire(p0, k0 + it - 1);
+      issue(p0, k0 + it + 1, it0 + it + 1);
+      wgmma_wait<1>();
+      retire(p1, k0 + it);
+    }
+    if (it < niter) {
+      issue(p1, k0 + it, it0 + it);
+      wgmma_wait<1>();
+      retire(p0, k0 + it - 1);
+      wgmma_wait<0>();
+      retire(p1, k0 + it);
+    } else {
+      wgmma_wait<0>();
+      retire(p0, k0 + it - 1);
+    }
+  };
+  // accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is row cw*64 + w*16 + l/4 + 8h,
+  // column 8j + 2(l%4) + e
+  const int row0 = cw * 64 + w * 16 + (l >> 2);
+
+  uint32_t k = 0;                                   // K slices consumed by this CTA
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    int b, r0, L;
+    if (!pair_tile(d, nrb, t, b, r0, L)) continue;
+    const long long item = (long long)b * d.L * C;
+    // the 16-bit modes' residual rows of this thread (x, fp32), all loaded before any is used
+    auto load_res = [&] {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = row0 + 8 * h, g = r0 + i;
+        const bool live = i < P_ROWS && g < L;
+        const float* xrow = d.x + item + (long long)g * C;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const float2 r = live ? *reinterpret_cast<const float2*>(xrow + 8 * j + 2 * (l & 3)) : make_float2(0.f, 0.f);
+          xr[4 * j + 2 * h] = r.x;
+          xr[4 * j + 2 * h + 1] = r.y;
+        }
+      }
+    };
+
+    // ---- conv1 -> h copies
+    conv(k, 0);
+    k += NITER;
+    named_sync(1, 256);                             // every consumer's conv2 of the last tile has read the h copies
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int i = row0 + 8 * h, g = r0 - 1 + i;
+      const bool inside = g >= 0 && g < L;
+#pragma unroll
+      for (int j = 0; j < C / 8; ++j) {
+        const int n = 8 * j + 2 * (l & 3);
+        float v0 = acc[4 * j + 2 * h] + b1[n], v1 = acc[4 * j + 2 * h + 1] + b1[n + 1];
+        v0 = inside ? (v0 > 0.f ? v0 : 0.01f * v0) : 0.f;
+        v1 = inside ? (v1 > 0.f ? v1 : 0.01f * v1) : 0.f;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const int jr = i - c;
+          if (jr < 0) continue;
+          uint8_t* p = hgen + c * NKS * 16384 + h_offset<ESZ>(jr, n);
+          if (ESZ == 2) {
+            *reinterpret_cast<uint32_t*>(p) = pack16<KIND == 2>(v0, v1);
+          } else {
+            *reinterpret_cast<float2*>(p) = make_float2(round_tf32(v0), round_tf32(v1));
+          }
+        }
+      }
+    }
+    if constexpr (KIND == 0) {
+      // output row i is row i + 1 of the centre-tap tiles (a == x): its residual, bit for bit as it lies in x
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = row0 + 8 * h;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const float2 r = i < P_ROWS ? *reinterpret_cast<const float2*>(cgen + h_offset<4>(i + 1, 8 * j + 2 * (l & 3)))
+                                      : make_float2(0.f, 0.f);
+          xr[4 * j + 2 * h] = r.x;
+          xr[4 * j + 2 * h + 1] = r.y;
+        }
+      }
+      __syncwarp();
+      if (l == 0) mbar_arrive(cempty);
+    } else if constexpr (EARLY) {
+      load_res();
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = row0 + 8 * h, g = r0 + i;
+        if (i < P_ROWS && g < L)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(d.x + item + (long long)g * C + 32 * (l & 3)));
+      }
+    }
+    fence_proxy_async();                            // the h copies are visible to conv2's wgmma
+    named_sync(1, 256);
+
+    // ---- conv2 from the h copies, residual, outputs
+    conv(k, NITER);
+    k += NITER;
+    if constexpr (KIND != 0 && !EARLY) load_res();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int i = row0 + 8 * h, g = r0 + i;
+      if (i >= P_ROWS || g >= L) continue;
+      const long long row = item + (long long)g * C;
+      // the thread's two adjacent columns n, n + 1 go out as one 8-byte (raw, tf32 operand) or 4-byte (16-bit) store
+#pragma unroll
+      for (int j = 0; j < C / 8; ++j) {
+        const int n = 8 * j + 2 * (l & 3);
+        float v[2], y[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float r = xr[4 * j + 2 * h + e];
+          v[e] = (acc[4 * j + 2 * h + e] + b2[n + e]) + (KIND == 0 ? stream_dec(r, 100.0f) : r);
+          y[e] = apply_act(v[e], d.act, d.act_param);
+          if (KIND == 0 && d.stream_enc_out) v[e] = stream_enc(v[e], 0.01f);
+        }
+        if (d.write_raw) *reinterpret_cast<float2*>(dst + row + n) = make_float2(v[0], v[1]);
+        if (out_act) {
+          if (ESZ == 4)
+            *reinterpret_cast<float2*>(out_act + row + n) = make_float2(round_tf32(y[0]), round_tf32(y[1]));
+          else
+            *reinterpret_cast<uint32_t*>(out_act + row + n) = pack16<KIND == 2>(y[0], y[1]);
         }
       }
     }
   }
-  fence_proxy_async();
-  __syncthreads();
-
-  // ---- conv2 from the h copies, residual, outputs
-  run(NITER);
-  float* dst = d.x_out ? d.x_out : d.x;
-  T* out_act = reinterpret_cast<T*>(d.out_act);
-  // acc + b2 and every residual element of the thread are loaded before the first store, so the stores (which may
-  // overwrite x in place) do not serialise the loads; each element is read and written by this thread alone.
-  float xr[C / 2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int i = wg * 64 + w * 16 + (l >> 2) + 8 * h, g = r0 + i;
-    const bool live = i < P_ROWS && g < L;
-    const long long row = item + (long long)g * C;
-#pragma unroll
-    for (int j = 0; j < C / 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = 8 * j + 2 * (l & 3) + e;
-        acc[4 * j + 2 * h + e] += d.b2[n];
-        xr[4 * j + 2 * h + e] = live ? d.x[row + n] : 0.f;
-      }
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int i = wg * 64 + w * 16 + (l >> 2) + 8 * h, g = r0 + i;
-    if (i >= P_ROWS || g >= L) continue;
-    const long long row = item + (long long)g * C;
-#pragma unroll
-    for (int j = 0; j < C / 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = 8 * j + 2 * (l & 3) + e;
-        const float r = xr[4 * j + 2 * h + e];
-        const float v = acc[4 * j + 2 * h + e] + (d.stream_enc ? stream_dec(r, 100.0f) : r);
-        if (d.write_raw) dst[row + n] = (d.stream_enc && d.stream_enc_out) ? stream_enc(v, 0.01f) : v;
-        if (out_act) out_act[row + n] = from_f<T>(apply_act(v, d.act, d.act_param));
-      }
-  }
 }
 
-template <int C, int KIND>
-int launch_fused(const vfx_pair_desc& d, cudaStream_t st) {
-  constexpr int smem = pair_smem<C, KIND>();
+// the launch's tensor maps (no lens: every item spans the whole tensor)
+int pair_maps(const vfx_pair_desc& d, PairMaps& m) {
+  const long long esz = (long long)prec_esz(d.precision), C = d.C;
+  const EncodeTiled encode = tensor_map_encoder();
+  VFX_REQUIRE(encode, "resstack_pair: this CUDA driver has no cuTensorMapEncodeTiled");
+  const CUtensorMapDataType dt = d.precision == VFX_PREC_TF32   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : d.precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const cuuint32_t bk = (cuuint32_t)(128 / esz), ones[3] = {1, 1, 1};
+  const cuuint64_t adim[3] = {(cuuint64_t)C, (cuuint64_t)d.L, (cuuint64_t)d.B};
+  const cuuint64_t astr[2] = {(cuuint64_t)(C * esz), (cuuint64_t)(d.L * C * esz)};
+  const cuuint32_t abox[3] = {bk, 128, 1};
+  const cuuint64_t wdim[3] = {(cuuint64_t)C, (cuuint64_t)C, 3};
+  const cuuint64_t wstr[2] = {(cuuint64_t)(C * esz), (cuuint64_t)(C * C * esz)};
+  const cuuint32_t wbox[3] = {bk, (cuuint32_t)C, 1};
+  CUresult r = encode(&m.a, dt, 3, const_cast<void*>(d.a), adim, astr, abox, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  VFX_REQUIRE(r == CUDA_SUCCESS, "resstack_pair: operand tensor map refused (CUresult %d)", (int)r);
+  const void* ws[2] = {d.w1, d.w2};
+  CUtensorMap* wm[2] = {&m.w1, &m.w2};
+  for (int i = 0; i < 2; ++i) {
+    r = encode(wm[i], dt, 3, const_cast<void*>(ws[i]), wdim, wstr, wbox, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    VFX_REQUIRE(r == CUDA_SUCCESS, "resstack_pair: weight tensor map refused (CUresult %d)", (int)r);
+  }
+  return VFX_OK;
+}
+
+template <int C, int KIND, bool TMA>
+int launch_pair(const vfx_pair_desc& d, const PairMaps& m, cudaStream_t st) {
+  constexpr int smem = PairCfg<C, KIND>::SMEM;
   static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
   int dev = 0;
   VFX_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(pair_fused_kernel<C, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    VFX_CUDA_CHECK(cudaFuncSetAttribute(pair_fused_kernel<C, KIND, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     if (dev < 64) attr_set |= 1ull << dev;
   }
-  dim3 grid(ceil_div(d.L, P_ROWS), d.B);
-  pair_fused_kernel<C, KIND><<<grid, 256, smem, st>>>(d);
+  const int sms = sm_count(dev);
+  VFX_REQUIRE(sms > 0, "resstack_pair: cannot read the SM count of device %d", dev);
+  const long long tiles = (long long)d.B * ceil_div(d.L, P_ROWS);
+  const int grid = (int)(tiles < sms ? tiles : sms);
+  if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
+  pair_fused_kernel<C, KIND, TMA><<<grid, P_NT, smem, st>>>(d, m, PairCfg<C, KIND>::NITER);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
+}
+
+// launches without per-item lengths are fed by TMA, ragged ones by cp.async
+template <int C, int KIND>
+int launch_fused(const vfx_pair_desc& d, cudaStream_t st) {
+  PairMaps m;
+  memset(&m, 0, sizeof(m));
+  if (d.lens) return launch_pair<C, KIND, false>(d, m, st);
+  const int r = pair_maps(d, m);
+  return r != VFX_OK ? r : launch_pair<C, KIND, true>(d, m, st);
 }
 
 }  // namespace
@@ -263,6 +484,9 @@ int resstack_pair(const vfx_pair_desc& d, cudaStream_t st) {
   VFX_REQUIRE(d.a && d.x && d.w1 && d.w2 && d.b1 && d.b2 && d.B > 0 && d.L > 0 && d.dilation > 0, "resstack_pair: bad arguments");
   if (d.form == VFX_PAIR_BLOCKED) return d.lens ? VFX_ERR_UNSUPPORTED : pair_blocked(d, prec, st);
   if (((uintptr_t)d.a & 15) || ((uintptr_t)d.w1 & 15) || ((uintptr_t)d.w2 & 15)) return VFX_ERR_UNSUPPORTED;
+  // the fused kernel reads and writes each thread's two adjacent columns with one access
+  if (((uintptr_t)d.x & 7) || ((uintptr_t)d.x_out & 7) || ((uintptr_t)d.out_act & (2 * prec_esz(prec) - 1)))
+    return VFX_ERR_UNSUPPORTED;
   if (prec == VFX_PREC_TF32) return launch_fused<64, 0>(d, st);
   if (prec == VFX_PREC_BF16) return d.C == 64 ? launch_fused<64, 1>(d, st) : launch_fused<128, 1>(d, st);
   return d.C == 64 ? launch_fused<64, 2>(d, st) : launch_fused<128, 2>(d, st);

@@ -1,7 +1,9 @@
-// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu): TMA tile loads, cp.async operand staging with zero
-// fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups and the
-// shared-memory matrix descriptor.
+// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu, resstack_pair.cu): TMA tile loads, cp.async operand
+// staging with zero fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups
+// and the shared-memory matrix descriptor; on the host, the SM count and the tensor-map encoder their launches use.
 #pragma once
+#include <atomic>
+#include <cuda.h>      // CUtensorMap and the types of its encoder; the encoder itself is looked up at run time
 #include "vfx_common.cuh"
 
 namespace vfx {
@@ -77,6 +79,35 @@ __device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {
   return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
+
+// ---- host: what a persistent launch sizes its grid by, and the encoder of its tensor maps
+inline int sm_count(int dev) {
+  static std::atomic<int> sms[64];                    // per device, queried once (host threads may drive several devices)
+  if (dev < 64) {
+    const int n = sms[dev].load(std::memory_order_relaxed);
+    if (n) return n;
+  }
+  int n = 0;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 0;
+  if (dev < 64) sms[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
+// cuTensorMapEncodeTiled, through the runtime (the library calls nothing else of the driver API)
+using EncodeTiled = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline EncodeTiled tensor_map_encoder() {
+  static const EncodeTiled fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      p = nullptr;
+    return reinterpret_cast<EncodeTiled>(p);
+  }();
+  return fn;
+}
 
 }  // namespace
 }  // namespace vfx
