@@ -83,7 +83,19 @@ ROUNDINGS = {"tf32": round_tf32, "tf32-trunc": trunc_tf32, "fp16": _via(torch.fl
 class OperandRounding:
     """The operand format of one engine precision: `operand` rounds a contraction's input or weight, `stored` is
     applied to the tensors the engine keeps in fp32 between contractions ("vocoder.residual": the ResStack stream x
-    after the up-sampler and after each pair; "unet.block": each ConvBlockRes output).  Subclass to model faults."""
+    after the up-sampler and after each pair; "unet.block": each ConvBlockRes output).  Subclass to model faults.
+
+    `where` names the rounding point of `operand`:
+      "denoiser.input" / "denoiser.weight"  the denoiser's Linear layers
+      "gru.input" / "gru.weight"            the GRU input projections: bn(x) or layer 0's output, and w_ih
+      "unet.bn_act"    act(bn(x)) read by a UNet conv: ConvBlockRes.conv1 and the decoders' ConvTranspose, and in
+                       train mode ConvBlockRes.conv2 (written by bn_act; in eval mode by the producing conv's epilogue)
+      "unet.act"       ConvBlockRes.conv2's input in eval mode (conv1's epilogue, bn2 folded)
+      "unet.shortcut"  the shortcut conv's raw x
+      "unet.weight"    every UNet conv weight (the folded conv1 weight in eval mode)
+      "vocoder.cond"   the conditions read by condnet.0 (voc_normalize, or the oracle front end)
+      "vocoder.act"    every other vocoder conv input
+      "vocoder.weight" every vocoder conv weight"""
 
     def __init__(self, fmt):
         if fmt not in ROUNDINGS:
@@ -91,7 +103,7 @@ class OperandRounding:
         self.fmt = fmt
         self.round = ROUNDINGS[fmt]
 
-    def operand(self, x):
+    def operand(self, x, where):
         return self.round(x)
 
     def stored(self, x, where):
@@ -113,8 +125,8 @@ def operand_rounding(model):
         _rounding = saved
 
 
-def _op(x):
-    return x if _rounding is None else _rounding.operand(x)
+def _op(x, where):
+    return x if _rounding is None else _rounding.operand(x, where)
 
 
 def _stored(x, where):
@@ -164,7 +176,7 @@ def gru_layer_dir(x, w_ih, w_hh, b_ih, b_hh, reverse):
     Gate order r,z,n; n = tanh(W_in x + b_in + r*(W_hn h + b_hn)); h' = (1-z)*n + z*h."""
     B, T, _ = x.shape
     H = w_hh.shape[1]
-    gi = _op(x) @ _op(w_ih).t() + b_ih
+    gi = _op(x, "gru.input") @ _op(w_ih, "gru.weight").t() + b_ih
     h = x.new_zeros(B, H)
     out = x.new_zeros(B, T, H)
     steps = range(T - 1, -1, -1) if reverse else range(T)
@@ -219,7 +231,7 @@ def denoiser(mel, ana, train=False, drop_masks=None):
 
 
 def _linear(x, ana, p):
-    return F.linear(_op(x), _op(ana[p + ".weight"]), ana[p + ".bias"])
+    return F.linear(_op(x, "denoiser.input"), _op(ana[p + ".weight"], "denoiser.weight"), ana[p + ".bias"])
 
 
 # --------------------------------------------------------------------------- UNet
@@ -236,21 +248,22 @@ def _conv1_bn2(a, ana, p, train):
     weight rounded, the shift added after the contraction (weights._conv_block, engine.cu conv_block)."""
     w1 = ana[p + ".conv1.weight"]
     if _rounding is None or train:
-        return _bn2d(F.conv2d(_op(a), _op(w1), padding=1), ana, p + ".bn2", train)
+        return _bn2d(F.conv2d(_op(a, "unet.bn_act"), _op(w1, "unet.weight"), padding=1), ana, p + ".bn2", train)
     q = p + ".bn2"
     scale = ana[q + ".weight"] / torch.sqrt(ana[q + ".running_var"] + BN_EPS)
     shift = ana[q + ".bias"] - ana[q + ".running_mean"] * scale
-    return F.conv2d(_op(a), _op(w1 * scale[:, None, None, None]), shift, padding=1)
+    return F.conv2d(_op(a, "unet.bn_act"), _op(w1 * scale[:, None, None, None], "unet.weight"), shift, padding=1)
 
 
 def conv_block_res(x, ana, p, train):
     """ConvBlockRes.forward restorer/modules.py:68-76 (pre-activation, lrelu 0.01)."""
     origin = x
     x = _conv1_bn2(F.leaky_relu(_bn2d(x, ana, p + ".bn1", train), 0.01), ana, p, train)
-    x = F.conv2d(_op(F.leaky_relu(x, 0.01)), _op(ana[p + ".conv2.weight"]), padding=1)
+    x = F.conv2d(_op(F.leaky_relu(x, 0.01), "unet.bn_act" if train else "unet.act"), _op(ana[p + ".conv2.weight"],
+                                                                                          "unet.weight"), padding=1)
     if (p + ".shortcut.weight") in ana:
-        return _stored(F.conv2d(_op(origin), _op(ana[p + ".shortcut.weight"]), ana[p + ".shortcut.bias"]) + x,
-                       "unet.block")
+        return _stored(F.conv2d(_op(origin, "unet.shortcut"), _op(ana[p + ".shortcut.weight"], "unet.weight"),
+                                ana[p + ".shortcut.bias"]) + x, "unet.block")
     return _stored(origin + x, "unet.block")
 
 
@@ -264,8 +277,8 @@ def encoder_block(x, ana, p, train):
 def decoder_block(x, skip, ana, p, train):
     """DecoderBlockRes.forward restorer/modules.py:149-157 (relu(bn1) -> ConvT 3x3 s2 ->
     prune last time row -> cat -> 4 ConvBlockRes)."""
-    x = F.conv_transpose2d(_op(F.relu(_bn2d(x, ana, p + ".bn1", train))), _op(ana[p + ".conv1.weight"]),
-                           stride=2)
+    x = F.conv_transpose2d(_op(F.relu(_bn2d(x, ana, p + ".bn1", train)), "unet.bn_act"),
+                           _op(ana[p + ".conv1.weight"], "unet.weight"), stride=2)
     x = x[:, :, 0:-1, :]
     x = torch.cat((x, skip), 1)
     for i in (2, 3, 4, 5):
@@ -349,10 +362,10 @@ def res_stack(x, voc, p):
     x = _stored(x, "vocoder.residual")
     for i in range(8):
         d = 3 ** i
-        h = F.conv1d(_op(F.leaky_relu(x, 0.01)), _op(_wn(voc, f"{p}.layers.{i}.1")), voc[f"{p}.layers.{i}.1.bias"],
-                     dilation=d, padding=d)
-        h = F.conv1d(_op(F.leaky_relu(h, 0.01)), _op(_wn(voc, f"{p}.layers.{i}.3")), voc[f"{p}.layers.{i}.3.bias"],
-                     padding=1)
+        h = F.conv1d(_op(F.leaky_relu(x, 0.01), "vocoder.act"), _op(_wn(voc, f"{p}.layers.{i}.1"), "vocoder.weight"),
+                     voc[f"{p}.layers.{i}.1.bias"], dilation=d, padding=d)
+        h = F.conv1d(_op(F.leaky_relu(h, 0.01), "vocoder.act"), _op(_wn(voc, f"{p}.layers.{i}.3"), "vocoder.weight"),
+                     voc[f"{p}.layers.{i}.3.bias"], padding=1)
         x = _stored(x + h, "vocoder.residual")
     return x
 
@@ -362,16 +375,18 @@ def upsample_net(x, voc, p, u):
     weight-normed ConvTranspose1d(k=2u, s=u, p=u//2+u%2, output_padding=u%2).  The skip_conv
     result is discarded by the reference (SURVEY D7) and is not computed here."""
     x = x + torch.sin(x)
-    return F.conv_transpose1d(_op(x), _op(_wn(voc, p + ".layer")), voc[p + ".layer.bias"], stride=u,
-                              padding=u // 2 + u % 2, output_padding=u % 2)
+    return F.conv_transpose1d(_op(x, "vocoder.act"), _op(_wn(voc, p + ".layer"), "vocoder.weight"),
+                              voc[p + ".layer.bias"], stride=u, padding=u // 2 + u % 2, output_padding=u % 2)
 
 
 def vocoder_generator(cond, voc):
     """vocoder Generator.forward generator.py:127-145 (condnet :33-54, generator :73-100)."""
     x = cond
     for i in (0, 2, 4, 6, 8):
-        x = F.elu(F.conv1d(_op(x), _op(_wn(voc, f"condnet.{i}")), voc[f"condnet.{i}.bias"], padding=1))
-    x = F.conv1d(_op(F.pad(x, (3, 3), mode="reflect")), _op(_wn(voc, "generator.1")), voc["generator.1.bias"])
+        x = F.elu(F.conv1d(_op(x, "vocoder.cond" if i == 0 else "vocoder.act"),
+                           _op(_wn(voc, f"condnet.{i}"), "vocoder.weight"), voc[f"condnet.{i}.bias"], padding=1))
+    x = F.conv1d(_op(F.pad(x, (3, 3), mode="reflect"), "vocoder.act"), _op(_wn(voc, "generator.1"), "vocoder.weight"),
+                 voc["generator.1.bias"])
     x = F.leaky_relu(x, 0.2)
     for j, u in enumerate(UPSAMPLE_SCALES):
         x = upsample_net(x, voc, f"generator.{3 + 3 * j}", u)

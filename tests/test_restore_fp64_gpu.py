@@ -113,14 +113,14 @@ def check_fp32(record_property, seam, tag, y, ref):
     assert loc < FP32_TOL[seam], f"{tag}worst {'frame' if log_mel else 'window'} {loc:.3e} against float64"
 
 
-def check_ratio(record_property, tag, e_engine, e_model):
+def check_ratio(record_property, tag, e_engine, e_model, delta=DELTA):
     ratio = e_engine / e_model
     record_property(f"{tag}E_engine", e_engine)
     record_property(f"{tag}E_model", e_model)
     record_property(f"{tag}ratio", ratio)
-    record_property(f"{tag}delta", DELTA)
-    assert 1 - DELTA <= ratio <= 1 + DELTA, \
-        f"{tag}E_engine / E_model = {e_engine:.4e} / {e_model:.4e} = {ratio:.4f}, outside 1 +- {DELTA}"
+    record_property(f"{tag}delta", delta)
+    assert 1 - delta <= ratio <= 1 + delta, \
+        f"{tag}E_engine / E_model = {e_engine:.4e} / {e_model:.4e} = {ratio:.4f}, outside 1 +- {delta}"
 
 
 # ---------------------------------------------------------------------------- inputs and float64 references
@@ -185,37 +185,39 @@ class Refs:
     def __init__(self, ana, voc):
         self.ana, self.voc, self.cache = ana, voc, {}
 
-    def _get(self, key, fn):
+    def _get(self, key, fn, rounding=None):
+        """fn() in float64, or under the operand-rounding model `rounding` (a format name or an OperandRounding)"""
+        from oracle import vf_oracle as O
+        key = key + (rounding,)
         if key not in self.cache:
             with torch.no_grad():
-                self.cache[key] = _f64(fn())
+                if rounding is None:
+                    self.cache[key] = _f64(fn())
+                else:
+                    with O.operand_rounding(rounding):
+                        self.cache[key] = _f64(fn())
         return self.cache[key]
 
     def restore(self, L, mode=0, rounding=None):
         from oracle import vf_oracle as O
+        masks = (lambda T: _item_mask(L)) if mode == 2 else None
+        return self._get(("restore", L, mode), lambda: O.restore_inmem(_item(L), self.ana, self.voc, mode=mode,
+                                                                       drop_masks_fn=masks), rounding)
 
-        def run():
-            masks = (lambda T: _item_mask(L)) if mode == 2 else None
-            if rounding is None:
-                return O.restore_inmem(_item(L), self.ana, self.voc, mode=mode, drop_masks_fn=masks)
-            with O.operand_rounding(rounding):
-                return O.restore_inmem(_item(L), self.ana, self.voc, mode=mode, drop_masks_fn=masks)
-        return self._get(("restore", L, mode, rounding), run)
-
-    def analysis(self, L, mode):
+    def analysis(self, L, mode, rounding=None):
         from oracle import vf_oracle as O
         masks = _item_mask(L) if mode == 2 else None
         return self._get(("analysis", L, mode), lambda: O.analysis(
-            _mel(L).to(DEV, torch.float64)[None, None], self.ana, mode == 2, masks)[0, 0]).reshape(-1, 128)
+            _mel(L).to(DEV, torch.float64)[None, None], self.ana, mode == 2, masks)[0, 0], rounding).reshape(-1, 128)
 
-    def vocoder(self, T):
+    def vocoder(self, T, rounding=None):
         from oracle import vf_oracle as O
         return self._get(("vocoder", T), lambda: O.vocoder_forward(_voc_mel(T).to(DEV, torch.float64)[None, None],
-                                                                   self.voc))
+                                                                   self.voc), rounding)
 
-    def oracle(self, L):
+    def oracle(self, L, rounding=None):
         from oracle import vf_oracle as O
-        return self._get(("oracle", L), lambda: O.oracle_wave(_item(L), self.voc) / 2 ** 15)
+        return self._get(("oracle", L), lambda: O.oracle_wave(_item(L), self.voc) / 2 ** 15, rounding)
 
 
 @pytest.fixture(scope="module")
