@@ -223,6 +223,48 @@ int vfx_resample(vfx_engine* e, const float* x, long long x_elems, const float* 
                  void* workspace, size_t workspace_bytes, void* stream);
 size_t vfx_resample_workspace_bytes(int B);
 
+/* One item of vfx_resample_src: output samples [y_first, y_first + y_len) of one recording's 44.1 kHz stream, read
+ * from the whole recording where it lies: its n_in samples are src[0], src[stride], ..., src[(n_in - 1) * stride]
+ * (a device pointer; stride >= 1 elements, e.g. one channel of an interleaved tensor).  up, down, rem, h_off, h_len:
+ * as in vfx_resample_item. */
+typedef struct vfx_resample_src_item {
+  const float* src;
+  long long stride;
+  long long n_in, y_first, h_off;
+  int y_len, up, down, rem, h_len;
+} vfx_resample_src_item;
+
+/* vfx_resample with every item reading its recording in place (device-resident input: no staged windows).  Same
+ * arithmetic, bit for bit, in the same kernel body; up = down = 1 is the copy that fills a row at 44.1 kHz, so one
+ * launch builds the rows of a batch at every rate.  y[B][L_cap]: row b receives item b's y_len samples, then zeros;
+ * lens_out[B] (device int32, optional) receives y_len.  The library validates every item before any launch: a non-null
+ * src; 1 <= stride and (n_in - 1) * stride within 2^62; up, down >= 1; the taps lie inside h[0, h_elems) (a copy needs
+ * none); 0 <= y_len <= L_cap; the outputs lie inside the stream's ceil(n_in * up / down) samples.  A bad item returns
+ * VFX_ERR_INVALID naming it, and nothing is launched or written.  The table is staged into the workspace:
+ * vfx_resample_src_workspace_bytes(B) bytes (needs no engine; 0 for B <= 0).  B <= 65535. */
+int vfx_resample_src(vfx_engine* e, const float* h, long long h_elems, const vfx_resample_src_item* items_host, int B,
+                     float* y, int L_cap, int* lens_out, void* workspace, size_t workspace_bytes, void* stream);
+size_t vfx_resample_src_workspace_bytes(int B);
+
+/* One item of vfx_scatter_rows: the first len samples of row b go to dst[dst_off, dst_off + len), dst a device
+ * buffer of dst_elems floats. */
+typedef struct vfx_scatter_item {
+  float* dst;
+  long long dst_elems, dst_off;
+  int len;
+} vfx_scatter_item;
+
+/* Row b of x[B][ldx] (device) -> items_host[b]'s destination, one launch for the batch: the rows of a ragged batch back
+ * into per-recording outputs (a restored segment at its offset in its recording, a generated waveform into its own
+ * buffer).  The library validates every item before any launch: a non-null dst; 0 <= len <= ldx;
+ * 0 <= dst_off and dst_off + len <= dst_elems; and no two items' destination ranges overlap.  A bad item returns
+ * VFX_ERR_INVALID naming it, and nothing is launched or written.  Items of length 0 write nothing (a table of them
+ * launches nothing).  The table is staged into the workspace: vfx_scatter_rows_workspace_bytes(B) bytes (0 for B <= 0).
+ * B <= 65535. */
+int vfx_scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* items_host, void* workspace,
+                     size_t workspace_bytes, void* stream);
+size_t vfx_scatter_rows_workspace_bytes(int B);
+
 /* ---- per-kernel test entry points (tests/ call the kernels through these) --------------- */
 
 /* Generic channels-last "shifted-window" convolution GEMM; the one kernel family behind every

@@ -49,6 +49,17 @@ class ResampleItem(ctypes.Structure):
                 ("x_len", _i), ("y_len", _i), ("up", _i), ("down", _i), ("rem", _i), ("h_len", _i)]
 
 
+class ResampleSrcItem(ctypes.Structure):
+    """struct vfx_resample_src_item (include/vfx_b200.h)."""
+    _fields_ = [("src", _vp), ("stride", _ll), ("n_in", _ll), ("y_first", _ll), ("h_off", _ll),
+                ("y_len", _i), ("up", _i), ("down", _i), ("rem", _i), ("h_len", _i)]
+
+
+class ScatterItem(ctypes.Structure):
+    """struct vfx_scatter_item (include/vfx_b200.h)."""
+    _fields_ = [("dst", _vp), ("dst_elems", _ll), ("dst_off", _ll), ("len", _i)]
+
+
 # name -> (restype, argtypes); must list every symbol include/vfx_b200.h declares
 SIGNATURES = {
     "vfx_last_error": (_c.c_char_p, []),
@@ -84,6 +95,10 @@ SIGNATURES = {
     "vfx_oracle_workspace_bytes": (_sz, [_vp, _i, _i]),
     "vfx_resample": (_i, [_vp, _vp, _ll, _vp, _ll, _c.POINTER(ResampleItem), _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "vfx_resample_workspace_bytes": (_sz, [_i]),
+    "vfx_resample_src": (_i, [_vp, _vp, _ll, _c.POINTER(ResampleSrcItem), _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "vfx_resample_src_workspace_bytes": (_sz, [_i]),
+    "vfx_scatter_rows": (_i, [_vp, _i, _ll, _c.POINTER(ScatterItem), _vp, _sz, _vp]),
+    "vfx_scatter_rows_workspace_bytes": (_sz, [_i]),
     "vfx_bn_stats": (_i, [_vp, _ll, _ll, _i, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "vfx_bn_act": (_i, [_i, _vp, _ll, _ll, _i, _ll, _i, _vp, _vp, _i, _i, _i, _f, _vp, _ll, _ll, _vp]),
     "vfx_dropout_apply": (_i, [_vp, _vp, _ll, _vp]),

@@ -134,7 +134,8 @@ def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
 
     Raises before anything is sized or launched, naming the item: ValueError for an empty list, a mel that is not
     [1, 1, T >= 1, 128], or a recording that is empty, not 1-D or all zeros (the reference divides by its zero peak);
-    AssertionError for a mel whose last dimension is not 128, as Vocoder.forward asserts."""
+    AssertionError for a mel whose last dimension is not 128, as Vocoder.forward asserts.  A recording that is a CUDA
+    tensor is not checked for all zeros: that would read it on the host."""
     what = {"mel": "forward_many", "wav": "oracle_many"}[kind]
     if len(items) == 0:
         raise ValueError(f"{what} takes a non-empty list")
@@ -152,12 +153,65 @@ def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
                 raise ValueError(f"{what}: item {i} has shape {shape}; each recording must be 1-D")
             if shape[0] == 0:
                 raise ValueError(f"{what}: item {i} is empty")
-            if not np.any(x):
+            if not is_cuda(x) and not np.any(x):          # a device item is not read on the host
                 raise ValueError(f"{what}: item {i} is all zeros; its peak normalisation would divide by zero")
             lengths.append(shape[0])
     if pack_lengths is not None:
         lengths = [int(n) for n in pack_lengths]
     return _pack(lengths, max_items)
+
+
+def is_cuda(w):
+    """Whether w is a CUDA tensor (anything else, e.g. an array or a list, is not)."""
+    return getattr(w, "is_cuda", False) is True
+
+
+def check_device_items(wavs, device, what):
+    """True when every item of wavs (restore_many / oracle_many) is a CUDA tensor, False when none is (the host path).
+    Raises ValueError naming the recording, before anything is launched, for a list that mixes CUDA and host items, and
+    for a CUDA item that is on another device than `device` (a torch.device), not float32, not 1-D, or of element stride
+    0 (an expanded tensor).  Any positive element stride is accepted."""
+    cuda = [is_cuda(w) for w in wavs]
+    if not any(cuda):
+        return False
+    if not all(cuda):
+        raise ValueError(f"{what}: recording {cuda.index(False)} is not a CUDA tensor but recording {cuda.index(True)} is; "
+                         "give every recording as a CUDA tensor, or none")
+    for i, w in enumerate(wavs):
+        if torch.device(w.device) != torch.device(device):
+            raise ValueError(f"{what}: recording {i} is on {w.device}; this engine runs on {device}")
+        if w.dtype != torch.float32:
+            raise ValueError(f"{what}: recording {i} has dtype {w.dtype}; CUDA recordings must be torch.float32")
+        if len(w.shape) != 1:
+            raise ValueError(f"{what}: recording {i} has shape {tuple(w.shape)}; each recording must be 1-D")
+        if w.stride(0) < 1:
+            raise ValueError(f"{what}: recording {i} has element stride {w.stride(0)} (an expanded tensor); its samples "
+                             "must be distinct elements (.contiguous() makes them so)")
+    return True
+
+
+def resample_rows(ranges, rates):
+    """The input rows of a batch of CUDA recordings: ranges = [(recording, a, b), ...] of their 44.1 kHz streams, rates
+    one per recording -> one (recording, rate, y_first, y_len) per row (Engine.resample_src; 44100 is a copy)."""
+    return [(i, int(rates[i]), int(a), int(b - a)) for i, a, b in ranges]
+
+
+def restore_out_len(n, mode):
+    """Samples restore_many returns for a recording of n samples at 44.1 kHz: its segments' _net_len, summed."""
+    return sum(_net_len(b - a, mode) for a, b in segment_bounds(int(n)))
+
+
+def restore_rows(segs, mode):
+    """Where each row of a restore_many batch of CUDA recordings goes: segs = [(recording, a, b), ...] (plan_many) -> one
+    (recording, dst_off, len) per row (Engine.scatter_rows): the segment's _net_len(b - a, mode) restored samples at its
+    offset in its recording's output, after the full 30 s segments before it."""
+    return [(i, (a // SEG_LENGTH) * _net_len(SEG_LENGTH, mode), _net_len(b - a, mode)) for i, a, b in segs]
+
+
+def oracle_rows(idx, lengths):
+    """Where each row of an oracle_many batch of CUDA recordings goes: items idx (plan_vocoder_many) of lengths[i]
+    samples at 44.1 kHz -> one (item, 0, _gen_len(1 + lengths[i] // 441)) per row: the whole output of the item."""
+    return [(i, 0, _gen_len(1 + lengths[i] // 441)) for i in idx]
 
 
 _STREAM_SHORT = "restore_stream: fewer than 1025 samples in total; the front end reflect-pads 1024"
@@ -504,23 +558,41 @@ class Vocoder:
         sample_rate: the recordings' rate in Hz, one positive int or one per recording.  A recording at another rate than
         44100 is resampled on the device (vfx_resample) straight into the batch, bit-identical to oracle_many on
         wavio._resample(wavs[i], rate_i, 44100), the host resampler oracle() reads files with; L_i is then its length at
-        44.1 kHz.  A call in which every rate is 44100 launches nothing for it."""
+        44.1 kHz.  A call in which every rate is 44100 launches nothing for it.
+
+        Device-resident recordings: when every item is a 1-D float32 CUDA tensor on the engine's device (any positive element
+        stride), they are read in place and element i is a new (1, (T_i + T_i % 2 + 4) * 441) float32 CUDA tensor,
+        bit-identical to torch.from_numpy of this call's element i on the items' host copies, at every sample_rate.  Each
+        batch's rows come from one vfx_resample_src launch and go to the outputs with one vfx_scatter_rows launch, all on
+        torch.cuda.current_stream(); the call returns without waiting for the GPU, and no sample crosses PCIe.  A list that
+        mixes CUDA and host items, or a CUDA item on another device, of another dtype or not 1-D, raises ValueError
+        before anything is launched.  A CUDA recording is not checked for all zeros (that would read it on the host): an
+        all-zero one gives whatever the device front end makes of its zero peak."""
         _check_cuda(cuda)
-        items = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
-        rates = resample.rates(sample_rate, len(items), "oracle_many")
         eng = self._engine
         dev = f"cuda:{eng.device}"
+        wavs = list(wavs)
+        on_dev = check_device_items(wavs, torch.device(dev), "oracle_many")
+        items = list(wavs) if on_dev else [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
+        rates = resample.rates(sample_rate, len(items), "oracle_many")
 
         def max_items(L):
             per_item = eng.oracle_workspace_bytes(2, L) - eng.oracle_workspace_bytes(1, L) + 4 * (L + _gen_len(1 + L // 441))
-            return eng._fit(per_item + _staging_extra(L, rates), 64, 2 << 30)
+            return eng._fit(per_item + (0 if on_dev else _staging_extra(L, rates)), 64, 2 << 30)
 
         # the recordings' lengths at 44.1 kHz (a recording that is not 1-D is refused by plan_vocoder_many)
-        lengths = [resample.out_len(a.shape[0], r) if a.ndim == 1 else 0 for a, r in zip(items, rates)]
-        outs = [None] * len(items)
+        lengths = [resample.out_len(a.shape[0], r) if len(a.shape) == 1 else 0 for a, r in zip(items, rates)]
+        if on_dev:                     # allocated before planning, so that max_items sees the memory they take
+            outs = [torch.empty((1, _gen_len(1 + n // 441)), device=dev) for n in lengths]
+        else:
+            outs = [None] * len(items)
         for L_cap, idx in plan_vocoder_many(items, "wav", max_items, pack_lengths=lengths):
             x, lens = _batch_input(eng, items, rates, [(i, 0, lengths[i]) for i in idx], L_cap, dev)
-            y = eng.oracle(x, lens=lens).cpu().numpy()
+            y = eng.oracle(x, lens=lens)
+            if on_dev:
+                eng.scatter_rows(y, [(outs[i], off, n) for i, off, n in oracle_rows(idx, lengths)])
+                continue
+            y = y.cpu().numpy()
             for k, i in enumerate(idx):
                 outs[i] = y[k:k + 1, :_gen_len(1 + lengths[i] // 441)].copy()
         return outs
@@ -547,8 +619,12 @@ def _pad_rows(rows, cap, dev):
 
 def _batch_input(eng, items, rates, ranges, cap, dev):
     """(x (B, cap), lens (B,) int32), both on dev: row k of x holds range k of ranges [(item, a, b), ...] of the items'
-    44.1 kHz streams, then zeros.  If any of `rates` (one per item) is not 44100, every row is resampled on the device
-    from its own input window (_stage, Engine.resample); otherwise the samples are copied (_pad_rows), no resampler runs."""
+    44.1 kHz streams, then zeros.  Items that are CUDA tensors (check_device_items) are read in place by one
+    vfx_resample_src launch at every rate (Engine.resample_src).  Host items: if any of `rates` (one per item) is not
+    44100, every row is resampled on the device from its own input window (_stage, Engine.resample); otherwise the
+    samples are copied (_pad_rows), no resampler runs."""
+    if isinstance(items[0], torch.Tensor):
+        return eng.resample_src([(items[i], r, a, n) for i, r, a, n in resample_rows(ranges, rates)], cap)
     if any(r != resample.RATE for r in rates):
         return eng.resample(*_stage(items, rates, ranges, dev), cap)
     return _pad_rows([torch.from_numpy(items[i][a:b]) for i, a, b in ranges], cap, dev)
@@ -566,6 +642,14 @@ def _drop_masks(drop_masks_fn, B, T):
     if tuple(masks.shape) != (2, B, T, 512):
         raise ValueError(f"dropout masks must have shape (2, {B}, {T}, 512), got {tuple(masks.shape)}")
     return masks
+
+
+def _upload_masks(masks, dev):
+    """Mode 2's keep-masks on dev, for a device-resident call: a host tensor goes through pinned memory with a
+    stream-ordered copy, so the host does not wait for the device."""
+    if masks is None or masks.is_cuda:
+        return masks
+    return masks.pin_memory().to(dev, non_blocking=True)
 
 
 def _stage(items, rates, segs, dev, extents=None):
@@ -722,34 +806,55 @@ class VoiceFixer:
         of the 44.1 kHz stream is computed from its own window of input samples, uploaded alone, straight into the
         batch.  Element i is then bit-identical to restore_many on wavio._resample(wavs[i], rate_i, 44100), the host
         resampler VoiceFixer.restore() reads files with; the plan is the same, so mode 2's default masks are drawn at the
-        same points.  A call in which every rate is 44100 launches nothing for it."""
+        same points.  A call in which every rate is 44100 launches nothing for it.
+
+        Device-resident recordings: when every item is a 1-D float32 CUDA tensor on the engine's device (any positive element
+        stride, e.g. x[:, c] of an interleaved (L, C) tensor), they are read in place, never written, and element i is a
+        new (1, L_i') float32 CUDA tensor, bit-identical to torch.from_numpy of this call's element i on the items' host
+        copies (modes 0 and 1, and mode 2 with drop_masks_fn=False, at every sample_rate; mode 2's random masks have the
+        same distribution).  Each batch's rows come from one vfx_resample_src launch and its restored segments go to their
+        offsets in the outputs with one vfx_scatter_rows launch, all on torch.cuda.current_stream(); the call returns
+        without waiting for the GPU, and no sample crosses PCIe.  A list that mixes CUDA and host items, or a CUDA item
+        on another device, of another dtype or not 1-D, raises ValueError before anything is launched."""
         _check_cuda(cuda)
-        items = []
-        for i, w in enumerate(wavs):
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+        wavs = list(wavs)
+        on_dev = check_device_items(wavs, torch.device(dev), "restore_many")
+        items = list(wavs) if on_dev else []
+        for i, w in ([] if on_dev else enumerate(wavs)):
             a = np.ascontiguousarray(w, dtype=np.float32)
             if a.ndim != 1:
                 raise ValueError(f"restore_many: recording {i} has shape {a.shape}; the list takes 1-D arrays")
             items.append(a)
         rates = resample.rates(sample_rate, len(items), "restore_many")
-        eng = self._engine
-        dev = f"cuda:{eng.device}"
 
         def max_items(L_cap):
-            extra = _staging_extra(L_cap, rates)
+            extra = 0 if on_dev else _staging_extra(L_cap, rates)
             if mode == 1:     # the pre-filter's workspace and its (B, L_cap) output live alongside the restore
                 extra += eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
             return eng.max_batch(L_cap, extra_per_item=extra)
 
         lengths = [resample.out_len(a.shape[0], r) for a, r in zip(items, rates)]
+        if on_dev:                     # allocated before planning, so that max_items sees the memory they take
+            outs = [torch.empty((1, restore_out_len(n, mode)), device=dev) for n in lengths]
         pieces = {}                                                      # (recording, start) -> restored segment
         for L_cap, segs in plan_many(lengths, mode, max_items):
             x, lens = _batch_input(eng, items, rates, segs, L_cap, dev)
             if mode == 1:
                 x, _, lens = eng.hf_cut(x, lens=lens)
             masks = _drop_masks(drop_masks_fn, len(segs), 1 + L_cap // 441) if mode == 2 else None
-            y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens).cpu().numpy()
+            if on_dev:
+                masks = _upload_masks(masks, dev)
+            y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens)
+            if on_dev:
+                eng.scatter_rows(y, [(outs[i], off, n) for i, off, n in restore_rows(segs, mode)])
+                continue
+            y = y.cpu().numpy()
             for k, (i, a, b) in enumerate(segs):
                 pieces[(i, a)] = y[k, :_net_len(b - a, mode)]
+        if on_dev:
+            return outs
         return [np.concatenate([pieces[(i, a)] for a, _ in segment_bounds(n)])[None] for i, n in enumerate(lengths)]
 
     # ------------------------------------------------------------------ batch entry point (extension)

@@ -373,6 +373,15 @@ __global__ void frame_extents_kernel(const int* __restrict__ frames, int B, int 
   ext[(EXT_UP0 + 3) * B + b] = Tc * 441;
 }
 
+// Row b of a (B, ldx) batch -> items[b].dst[dst_off, dst_off + len) (vfx_scatter_rows): one thread per sample.
+__global__ void __launch_bounds__(256) scatter_rows_kernel(const float* __restrict__ x, long long ldx,
+                                                           const vfx_scatter_item* __restrict__ items) {
+  const int b = blockIdx.y;
+  const vfx_scatter_item it = items[b];
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < it.len) it.dst[it.dst_off + j] = __ldg(x + (long long)b * ldx + j);
+}
+
 inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
   if (g > 132LL * 32) g = 132LL * 32;      // 32 blocks per SM of an H100 SXM
@@ -542,6 +551,15 @@ int voc_post(const float* x, int B, int L, const float* w, const float* bias, in
   VFX_REQUIRE(((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0, "voc_post: x and w must be 16-byte aligned");
   dim3 grid(ceil_div(out_len, POST_RUN * POST_GROUPS), B);
   voc_post_kernel<<<grid, 16 * POST_GROUPS, 0, st>>>(x, L, w, bias, lo, out_len, ext_gen, ext_len, scale, out);
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+int scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* items, int max_len, cudaStream_t st) {
+  VFX_REQUIRE(x && items && B > 0 && B <= 65535 && max_len > 0 && max_len <= ldx,
+              "scatter_rows: bad arguments (B %d, ldx %lld, max_len %d; B <= 65535)", B, ldx, max_len);
+  dim3 grid(ceil_div(max_len, 256), B);
+  scatter_rows_kernel<<<grid, 256, 0, st>>>(x, ldx, items);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

@@ -812,6 +812,68 @@ int check_resample_item(const vfx_resample_item& it, int b, long long x_elems, l
   return VFX_OK;
 }
 
+// vfx_resample_src: the item table is staged into the workspace, then one launch
+int resample_src_forward(Ctx& c, const float* h, const vfx_resample_src_item* items_host, int B, int L_cap, float* y,
+                         int* lens_out) {
+  vfx_resample_src_item* items = c.ws->alloc<vfx_resample_src_item>(B);
+  if (c.dry) return VFX_OK;
+  VFX_CUDA_CHECK(cudaMemcpyAsync(items, items_host, sizeof(vfx_resample_src_item) * B, cudaMemcpyHostToDevice, c.st));
+  return resample_src(h, items, B, L_cap, y, lens_out, c.st);
+}
+
+// One item of vfx_resample_src against the buffers (include/vfx_b200.h): VFX_ERR_INVALID with a message naming item b.
+int check_resample_src_item(const vfx_resample_src_item& it, int b, long long h_elems, int L_cap) {
+  VFX_REQUIRE(it.src, "resample_src: item %d: src is null", b);
+  VFX_REQUIRE(it.up >= 1 && it.down >= 1 && it.up <= (1 << 20), "resample_src: item %d: ratio %d/%d (up must lie in "
+              "[1, 2^20], down >= 1)", b, it.up, it.down);
+  VFX_REQUIRE(it.n_in >= 0 && it.n_in <= (1LL << 40), "resample_src: item %d: recording length %lld", b, it.n_in);
+  VFX_REQUIRE(it.stride >= 1 && (it.n_in <= 1 || it.stride <= (1LL << 62) / (it.n_in - 1)), "resample_src: item %d: "
+              "stride %lld (must be >= 1, and (n_in - 1) * stride within 2^62)", b, it.stride);
+  if (!(it.up == 1 && it.down == 1))
+    VFX_REQUIRE(it.h_off >= 0 && it.h_len >= 1 && it.h_off + it.h_len <= h_elems && it.rem >= 0, "resample_src: item "
+                "%d: taps h[%lld, %lld) (rem %d) are not inside the %lld given", b, it.h_off, it.h_off + it.h_len, it.rem,
+                h_elems);
+  const long long n_out = (it.n_in * it.up + it.down - 1) / it.down;
+  VFX_REQUIRE(it.y_len >= 0 && it.y_len <= L_cap, "resample_src: item %d: y_len %d is not in [0, L_cap = %d]", b,
+              it.y_len, L_cap);
+  VFX_REQUIRE(it.y_first >= 0 && it.y_first <= n_out - it.y_len, "resample_src: item %d: outputs [%lld, %lld) are not "
+              "inside the stream's %lld samples", b, it.y_first, it.y_first + it.y_len, n_out);
+  return VFX_OK;
+}
+
+// vfx_scatter_rows: the item table is staged into the workspace, then one launch
+int scatter_rows_forward(Ctx& c, const float* x, int B, long long ldx, const vfx_scatter_item* items_host,
+                         int max_len) {
+  vfx_scatter_item* items = c.ws->alloc<vfx_scatter_item>(B);
+  if (c.dry) return VFX_OK;
+  VFX_CUDA_CHECK(cudaMemcpyAsync(items, items_host, sizeof(vfx_scatter_item) * B, cudaMemcpyHostToDevice, c.st));
+  return scatter_rows(x, B, ldx, items, max_len, c.st);
+}
+
+// The items of vfx_scatter_rows (include/vfx_b200.h): each on its own, then no two destination ranges overlapping.
+// Sets *max_len to the longest item.
+int check_scatter_items(const vfx_scatter_item* items, int B, long long ldx, int* max_len) {
+  std::vector<std::pair<uintptr_t, int>> ranges;        // (first byte, item) of each non-empty destination range
+  *max_len = 0;
+  for (int b = 0; b < B; ++b) {
+    const vfx_scatter_item& it = items[b];
+    VFX_REQUIRE(it.dst, "scatter_rows: item %d: dst is null", b);
+    VFX_REQUIRE(it.len >= 0 && it.len <= ldx, "scatter_rows: item %d: len %d is not in [0, ldx = %lld]", b, it.len, ldx);
+    VFX_REQUIRE(it.dst_off >= 0 && it.dst_elems >= 0 && it.dst_off <= it.dst_elems - it.len, "scatter_rows: item %d: "
+                "destination [%lld, %lld) is not inside its %lld elements", b, it.dst_off, it.dst_off + it.len,
+                it.dst_elems);
+    if (it.len > 0) ranges.push_back({(uintptr_t)(it.dst + it.dst_off), b});
+    *max_len = std::max(*max_len, it.len);
+  }
+  std::sort(ranges.begin(), ranges.end());
+  for (size_t k = 1; k < ranges.size(); ++k) {
+    const vfx_scatter_item& p = items[ranges[k - 1].second];
+    VFX_REQUIRE(ranges[k - 1].first + sizeof(float) * p.len <= ranges[k].first, "scatter_rows: item %d: its destination "
+                "overlaps item %d's", ranges[k].second, ranges[k - 1].second);
+  }
+  return VFX_OK;
+}
+
 // Vocoder.oracle's mel basis: librosa.filters.mel(sr=44100, n_fft=2048, n_mels=128, fmin=0, fmax=22050, htk=True) with
 // its default norm="slaney" (vocoder/model/util.py:115-123), built in float64 as librosa builds it and cast to float32
 // (wavio.slaney_htk_mel_basis is the same formula on the host).  band: start[128] ++ len[128] of each row's non-zeros.
@@ -1221,6 +1283,45 @@ int vfx_resample(vfx_engine* e, const float* x, long long x_elems, const float* 
   for (int b = 0; b < B; ++b) VFX_TRY(check_resample_item(items_host[b], b, x_elems, h_elems, L_cap));
   return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
                       [&](Ctx& c) { return resample_forward(c, x, h, items_host, B, L_cap, y, lens_out); });
+}
+
+size_t vfx_resample_src_workspace_bytes(int B) {
+  if (B <= 0) return 0;
+  int rc;
+  const size_t peak = dry_peak(nullptr, VFX_MODE_EVAL, [&](Ctx& c) {
+    return resample_src_forward(c, nullptr, nullptr, B, 1, nullptr, nullptr);
+  }, &rc);
+  return rc == VFX_OK ? peak : 0;
+}
+
+int vfx_resample_src(vfx_engine* e, const float* h, long long h_elems, const vfx_resample_src_item* items_host, int B,
+                     float* y, int L_cap, int* lens_out, void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_ENTER(e);
+  VFX_REQUIRE(items_host && y && B > 0 && B <= 65535 && L_cap > 0 && workspace && h_elems >= 0,
+              "resample_src: bad arguments");
+  VFX_REQUIRE(h || h_elems == 0, "resample_src: h is null");
+  for (int b = 0; b < B; ++b) VFX_TRY(check_resample_src_item(items_host[b], b, h_elems, L_cap));
+  return planned_call(e, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return resample_src_forward(c, h, items_host, B, L_cap, y, lens_out); });
+}
+
+size_t vfx_scatter_rows_workspace_bytes(int B) {
+  if (B <= 0) return 0;
+  int rc;
+  const size_t peak = dry_peak(nullptr, VFX_MODE_EVAL, [&](Ctx& c) {
+    return scatter_rows_forward(c, nullptr, B, 1, nullptr, 1);
+  }, &rc);
+  return rc == VFX_OK ? peak : 0;
+}
+
+int vfx_scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* items_host, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  VFX_REQUIRE(x && items_host && B > 0 && B <= 65535 && ldx > 0 && workspace, "scatter_rows: bad arguments");
+  int max_len;
+  VFX_TRY(check_scatter_items(items_host, B, ldx, &max_len));
+  if (max_len == 0) return VFX_OK;
+  return planned_call(nullptr, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return scatter_rows_forward(c, x, B, ldx, items_host, max_len); });
 }
 
 int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream) {

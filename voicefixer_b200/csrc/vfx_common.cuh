@@ -174,5 +174,11 @@ size_t hf_cut_workspace(int B, int L);
 // a table vfx_resample has validated), then zeros; lens_out[b] (optional) <- y_len
 int resample(const float* x, const float* h, const vfx_resample_item* items, int B, int L_cap, float* y, int* lens_out,
              cudaStream_t st);
+// the same arithmetic on items that read their recordings in place (vfx_resample_src)
+int resample_src(const float* h, const vfx_resample_src_item* items, int B, int L_cap, float* y, int* lens_out,
+                 cudaStream_t st);
+// row b of x[B][ldx] -> items[b]'s destination (items: the device copy of a table vfx_scatter_rows has validated);
+// max_len: the longest item
+int scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* items, int max_len, cudaStream_t st);
 
 }  // namespace vfx

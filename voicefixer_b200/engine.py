@@ -70,7 +70,13 @@ class Planner(_WorkspaceQueries):
 
 
 class Engine(_WorkspaceQueries):
-    """One engine per process / GPU.  `ana`, `voc`: reference-layout state dicts (CPU tensors)."""
+    """One engine per process / GPU.  `ana`, `voc`: reference-layout state dicts (CPU tensors).
+
+    Every call launches on torch.cuda.current_stream().  The engine's workspace and its resampling taps are shared by
+    all its calls, so a call made on another stream than the one before it first makes its stream wait for the work
+    already queued on that one (_shared_stream): calls on several streams run in the order they were made, never at
+    the same time, and a buffer the engine replaces is not reused before every stream that read it has finished with
+    it.  Calls are made from one host thread at a time."""
 
     def __init__(self, ana=None, voc=None, device=None, precision=None, packed=None):
         if not torch.cuda.is_available():
@@ -86,6 +92,7 @@ class Engine(_WorkspaceQueries):
                        "vfx_engine_create")
         self.h = h
         self._ws = None
+        self._last_stream = None  # the stream of the last call that used the shared workspace or taps
         self.arena = None
         self.table = None
         if packed is None and ana is not None:
@@ -153,11 +160,23 @@ class Engine(_WorkspaceQueries):
             pass
 
     # ------------------------------------------------------------------ workspace
+    def _shared_stream(self):
+        """The current stream, made to wait for the work queued on the stream of the previous call that used the shared
+        workspace or taps, if that was another stream (a device-side wait: the host does not wait)."""
+        st = torch.cuda.current_stream(self.device)
+        if self._last_stream is not None and self._last_stream != st:
+            st.wait_stream(self._last_stream)
+        self._last_stream = st
+        return st
+
     def _workspace(self, nbytes):
         if nbytes == 0:
             raise _lib.VfxError("workspace query returned 0: the shape is out of range (restore() needs L > 1024 samples) or this "
                                 "engine holds the vocoder weights only (stand-alone Vocoder: restore/analysis are unavailable)")
+        st = self._shared_stream()
         if self._ws is None or self._ws.numel() < nbytes:
+            if self._ws is not None:   # not reused before st's queued work, which follows every earlier use, is done
+                self._ws.record_stream(st)
             self._ws = None     # (captured graphs own their workspace tensors; see make_graph)
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{self.device}")
         return self._ws
@@ -353,8 +372,12 @@ class Engine(_WorkspaceQueries):
                 self._taps_off[key] = (sum(len(t) for t in self._taps_host), len(h))
                 self._taps_host.append(h)
                 fresh = True
-        if fresh:
-            self._taps_dev = torch.from_numpy(np.concatenate(self._taps_host)).to(f"cuda:{self.device}")
+        if fresh:                              # pinned and stream-ordered: the upload makes the host wait for nothing
+            st = self._shared_stream()
+            if self._taps_dev is not None:     # not reused before st's queued work, which follows every earlier read, is done
+                self._taps_dev.record_stream(st)
+            host = torch.from_numpy(np.concatenate(self._taps_host)).pin_memory()
+            self._taps_dev = host.to(f"cuda:{self.device}", non_blocking=True)
         return self._taps_off
 
     def resample(self, x, items, L_cap):
@@ -384,6 +407,68 @@ class Engine(_WorkspaceQueries):
         _lib.check(self.lib.vfx_resample(self.h, _ptr(x), x.numel(), _ptr(h), 0 if h is None else h.numel(), table, B,
                                          _ptr(y), int(L_cap), _ptr(lens), _ptr(ws), ws.numel(), _stream()), "vfx_resample")
         return y, lens
+
+    @staticmethod
+    def resample_src_workspace_bytes(B):
+        """Workspace of resample_src() on B items (vfx_resample_src_workspace_bytes; no engine needed)."""
+        return int(_lib.load().vfx_resample_src_workspace_bytes(int(B)))
+
+    def resample_src(self, items, L_cap):
+        """resample() on recordings that are already on the device, read in place (vfx_resample_src): the same
+        arithmetic, bit for bit, without staged windows; a rate of 44100 is a copy, so one launch builds a batch's rows.
+
+        items: one (src, rate, y_first, y_len) per row: output samples [y_first, y_first + y_len) of the 44.1 kHz stream
+        of src, a 1-D float32 CUDA tensor on this engine's device with any element stride, at `rate`.  src is never
+        written.  Returns (y (B, L_cap) with row b's y_len samples then zeros, lens (B,) int32 device tensor of the
+        y_len)."""
+        dev = torch.device(f"cuda:{self.device}")
+        for b, (src, *_) in enumerate(items):
+            if not (src.is_cuda and src.device == dev and src.dtype == torch.float32 and src.dim() == 1):
+                raise ValueError(f"resample_src: item {b}: src must be a 1-D float32 tensor on {dev}")
+        B = len(items)
+        offs = self._taps_for([it[1] for it in items])
+        table = (_lib.ResampleSrcItem * B)()
+        for b, (src, rate, y_first, y_len) in enumerate(items):
+            up, down = resample.ratio(rate)
+            t = table[b]
+            t.src, t.stride, t.n_in = src.data_ptr(), src.stride(0), src.shape[0]
+            t.y_first, t.y_len = int(y_first), int(y_len)
+            t.up, t.down, t.rem = up, down, resample.taps(rate)[1]
+            t.h_off, t.h_len = offs.get((up, down), (0, 0))
+        h = self._taps_dev
+        y = torch.empty(B, int(L_cap), device=dev)
+        lens = torch.empty(B, dtype=torch.int32, device=dev)
+        ws = self._workspace(self.resample_src_workspace_bytes(B))
+        _lib.check(self.lib.vfx_resample_src(self.h, _ptr(h), 0 if h is None else h.numel(), table, B, _ptr(y),
+                                             int(L_cap), _ptr(lens), _ptr(ws), ws.numel(), _stream()),
+                   "vfx_resample_src")
+        return y, lens
+
+    @staticmethod
+    def scatter_rows_workspace_bytes(B):
+        """Workspace of scatter_rows() on B rows (vfx_scatter_rows_workspace_bytes; no engine needed)."""
+        return int(_lib.load().vfx_scatter_rows_workspace_bytes(int(B)))
+
+    def scatter_rows(self, x, items):
+        """Copies the rows of a batch into their own tensors in one launch (vfx_scatter_rows): row b of x (B, ldx), a
+        float32 CUDA tensor with unit column stride, gives its first len_b samples to dst_b.view(-1)[off_b : off_b +
+        len_b].  items: one (dst_b, off_b, len_b) per row, dst_b a contiguous float32 CUDA tensor on this device.  The
+        destination ranges must not overlap."""
+        dev = torch.device(f"cuda:{self.device}")
+        if not (x.is_cuda and x.device == dev and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1):
+            raise ValueError(f"scatter_rows: x must be a (B, ldx) float32 tensor on {dev} with unit column stride")
+        B = x.shape[0]
+        if len(items) != B:
+            raise ValueError(f"scatter_rows: {len(items)} items for {B} rows")
+        table = (_lib.ScatterItem * B)()
+        for b, (dst, off, n) in enumerate(items):
+            if not (dst.is_cuda and dst.device == dev and dst.dtype == torch.float32 and dst.is_contiguous()):
+                raise ValueError(f"scatter_rows: item {b}: dst must be a contiguous float32 tensor on {dev}")
+            t = table[b]
+            t.dst, t.dst_elems, t.dst_off, t.len = dst.data_ptr(), dst.numel(), int(off), int(n)
+        ws = self._workspace(self.scatter_rows_workspace_bytes(B))
+        _lib.check(self.lib.vfx_scatter_rows(_ptr(x), B, x.stride(0), table, _ptr(ws), ws.numel(), _stream()),
+                   "vfx_scatter_rows")
 
     def hf_cut(self, wav, ratio=0.95, lens=None):
         """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
