@@ -246,18 +246,21 @@ int vfx_resample_src(vfx_engine* e, const float* h, long long h_elems, const vfx
                      float* y, int L_cap, int* lens_out, void* workspace, size_t workspace_bytes, void* stream);
 size_t vfx_resample_src_workspace_bytes(int B);
 
-/* One item of vfx_scatter_rows: the first len samples of row b go to dst[dst_off, dst_off + len), dst a device
- * buffer of dst_elems floats. */
+/* One item of vfx_scatter_rows: samples [src_off, src_off + len) of row b go to dst[dst_off, dst_off + len), dst a
+ * device buffer of dst_elems floats.  src_off = 0 copies the row's first len samples (a zero-initialised item does);
+ * a live stream's window gives only its kept span, which starts src_off samples into the row.  src_off sits in what
+ * was the struct's tail padding: sizeof stays 32. */
 typedef struct vfx_scatter_item {
   float* dst;
   long long dst_elems, dst_off;
   int len;
+  int src_off;
 } vfx_scatter_item;
 
 /* Row b of x[B][ldx] (device) -> items_host[b]'s destination, one launch for the batch: the rows of a ragged batch back
  * into per-recording outputs (a restored segment at its offset in its recording, a generated waveform into its own
- * buffer).  The library validates every item before any launch: a non-null dst; 0 <= len <= ldx;
- * 0 <= dst_off and dst_off + len <= dst_elems; and no two items' destination ranges overlap.  A bad item returns
+ * buffer, a window's kept span into a block of its own).  The library validates every item before any launch: a
+ * non-null dst; 0 <= len <= ldx; 0 <= src_off and src_off + len <= ldx; 0 <= dst_off and dst_off + len <= dst_elems; and no two items' destination ranges overlap.  A bad item returns
  * VFX_ERR_INVALID naming it, and nothing is launched or written.  Items of length 0 write nothing (a table of them
  * launches nothing).  The table is staged into the workspace: vfx_scatter_rows_workspace_bytes(B) bytes (0 for B <= 0).
  * B <= 65535. */

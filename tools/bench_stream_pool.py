@@ -1,18 +1,24 @@
 """Many live streams through one StreamPool against one restore_stream generator per stream, mode 0, synthetic weights.
 Each stream is a seeded synthetic utterance of --seconds at 44.1 kHz, fed in --block-second blocks, restored in chunks
-of --chunk seconds with --ctx seconds of context on each side.
+of --chunk seconds with --ctx seconds of context on each side.  Two pools run: a host pool (numpy blocks in and out)
+and a device pool (the same blocks as CUDA tensors in and out, no host staging and no wait in a step).
 
   (a) throughput: all input available.  The pool is fed one block per stream in turn and steps whenever a full batch
       of windows is due (and at the end until it is empty); the generators are driven round-robin, one window each in
       turn.  Stream-audio seconds emitted per wall second, host clock around work that ends in a device synchronise.
-      The run asserts that every stream's pool output is bit-identical to its generator's.
+      The run asserts that every stream's pool output is bit-identical to its generator's, and the device pool's to
+      the host pool's; the device pool's wall time ends in a device synchronise.
   (b) real time: blocks arrive on a simulated clock (stream i starts at a seeded offset in [0, chunk) s and then gets
       one block per block period).  The pool steps whenever windows are due.  A window's lag is the time from the
       arrival of the block that made it due to the end of the step that emits it; N streams keep real time when no
       lag reaches one chunk (otherwise each step leaves more than it took).  Reports p50 / p99 step time, the largest
       lag and the median time to first audio (from a stream's start to the end of the step that emits its first block).
+      For the device pool a step ends when its work on the device is done (a CUDA event after it, timed from an event
+      recorded at the start), not when step() returns; the driver steps it again once that event has passed, so that
+      windows gather into batches while the device is busy, as they do while a host pool's step waits.
   (c) host share: the share of (a)'s step time outside the graph replay (staging on the host, uploads, resampling,
-      copy-back, cutting), from the summed wall time of the steps and CUDA events around replays of the same buckets.
+      copy-back, cutting), from the summed wall time of the steps and CUDA events around each replay inside them.
+      For the device pool the step time is the device time between CUDA events recorded before and after each step.
 
 Prints the card's name, power limit and maximum SM clock, then one JSON line.  Usage:
   python tools/bench_stream_pool.py [--streams 1,8,32,64,128] [--rt-streams 8,32,64,128,192,256] [--seconds 20]"""
@@ -51,12 +57,13 @@ def blocks_of(x, block):
     return [x[i:i + block] for i in range(0, len(x), block)]
 
 
-def warm(pool):
+def warm(pool, device=False):
     """Captures the graph of every bucket: a step of B windows, one per fresh stream, for each bucket B."""
     for B in pool.buckets:
         sids = [pool.open() for _ in range(B)]
         for sid in sids:
-            pool.push(sid, np.zeros(int((pool._sched.chunk + pool._sched.ctx)), np.float32) + 0.1)
+            x = np.zeros(int((pool._sched.chunk + pool._sched.ctx)), np.float32) + 0.1
+            pool.push(sid, torch.from_numpy(x).cuda() if device else x)
         pool.step()
         for sid in sids:
             pool.close(sid)
@@ -65,8 +72,13 @@ def warm(pool):
     assert pool.graph_count == len(pool.buckets)
 
 
-def run_pool(pool, streams, block, timed_steps=None):
-    """(a) for the pool: returns ([output per stream], wall seconds)."""
+def run_pool(pool, streams, block, timed_steps=None, device=False):
+    """(a) for the pool: returns ([output per stream], wall seconds).  device: push CUDA tensors (the streams are
+    uploaded before the clock starts) and time to a device synchronise; timed_steps then gets (bucket, start event, end
+    event) per step."""
+    if device:
+        streams = [torch.from_numpy(x).cuda() for x in streams]
+        torch.cuda.synchronize()
     blocks = [blocks_of(x, block) for x in streams]
     got = [[] for _ in streams]
     t0 = time.perf_counter()
@@ -76,9 +88,16 @@ def run_pool(pool, streams, block, timed_steps=None):
     def step():
         ts = time.perf_counter()
         n = min(pool.pending, pool.max_windows)
-        out = pool.step()
-        if timed_steps is not None:
-            timed_steps.append((pool.bucket(n), time.perf_counter() - ts))
+        if device and timed_steps is not None:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            ev[0].record()
+            out = pool.step()
+            ev[1].record()
+            timed_steps.append((pool.bucket(n), ev[0], ev[1]))
+        else:
+            out = pool.step()
+            if timed_steps is not None:
+                timed_steps.append((pool.bucket(n), time.perf_counter() - ts))
         for sid, ys in out.items():
             got[index[sid]] += ys
 
@@ -92,7 +111,11 @@ def run_pool(pool, streams, block, timed_steps=None):
             step()
     while pool.pending:
         step()
+    if device:
+        torch.cuda.synchronize()
     wall = time.perf_counter() - t0
+    if device:
+        return [torch.cat(g).cpu().numpy() for g in got], wall
     return [np.concatenate(g) for g in got], wall
 
 
@@ -114,6 +137,21 @@ def run_round_robin(vf, streams, block, args):
     return [np.concatenate(g) for g in got], time.perf_counter() - t0
 
 
+def time_replays(pool):
+    """Wraps the replay of each of the pool's graphs in CUDA events; returns the list that receives (start, end) of
+    every replay from then on, so the device time of the replays inside the steps can be summed afterwards."""
+    spans = []
+    for g in pool._graphs.values():
+        def replay(g=g, orig=g.replay):
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            ev[0].record()
+            orig()
+            ev[1].record()
+            spans.append(ev)
+        g.replay = replay
+    return spans
+
+
 def replay_ms(pool, B, reps=10):
     g = pool._graphs[B]
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
@@ -126,9 +164,12 @@ def replay_ms(pool, B, reps=10):
     return ev[0].elapsed_time(ev[1]) / reps
 
 
-def run_real_time(pool, streams, block, args, rng):
-    """(b): returns dict(steps, p50/p99 step ms, max / p99 lag s, median time to first audio s, keeps_real_time)."""
+def run_real_time(pool, streams, block, args, rng, device=False):
+    """(b): returns dict(steps, p50/p99 step ms, max / p99 lag s, median time to first audio s, keeps_real_time).
+    device: push CUDA tensors; a step ends when an event recorded after it completes on the device."""
     period = block / SR
+    if device:
+        streams = [torch.from_numpy(x).cuda() for x in streams]
     blocks = [blocks_of(x, block) for x in streams]
     start = rng.uniform(0, args.chunk, size=len(streams))
     sids = [pool.open() for _ in streams]
@@ -136,7 +177,11 @@ def run_real_time(pool, streams, block, args, rng):
     next_k = [0] * len(streams)
     due = deque()                                   # arrival time of the push that made each pending window due
     step_ms, lags, first = [], [], [None] * len(streams)
+    ends = []                                       # device pool: (end event, [(stream, arrival) per window emitted])
+    torch.cuda.synchronize()
+    ev0 = torch.cuda.Event(enable_timing=True)
     t0 = time.perf_counter()
+    ev0.record()
     left = len(streams)
     while left or pool.pending:
         now = time.perf_counter() - t0
@@ -150,19 +195,31 @@ def run_real_time(pool, streams, block, args, rng):
                     left -= 1
                 arrived = start[i] + next_k[i] * period
                 due.extend([arrived] * (pool.pending - before))
-        if not pool.pending:
-            time.sleep(0.0005)
+        if not pool.pending or (device and ends and not ends[-1][0].query()):
+            time.sleep(0.0005)                      # a device pool steps again once its previous step's work is done
             continue
         ts = time.perf_counter()
         out = pool.step()
         te = time.perf_counter()
         step_ms.append((te - ts) * 1e3)
-        for sid, ys in out.items():
-            for _ in ys:
-                lags.append(te - t0 - due.popleft())
-            i = index[sid]
+        emitted = [(index[sid], due.popleft()) for sid, ys in out.items() for _ in ys]
+        if device:
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record()
+            ends.append((ev, emitted))
+            continue
+        for i, arrived in emitted:
+            lags.append(te - t0 - arrived)
             if first[i] is None:
                 first[i] = te - t0 - start[i]
+    if device:
+        torch.cuda.synchronize()
+        for ev, emitted in ends:
+            te = ev0.elapsed_time(ev) / 1e3
+            for i, arrived in emitted:
+                lags.append(te - arrived)
+                if first[i] is None:
+                    first[i] = te - start[i]
     lags = np.array(lags)
     return {"streams": len(streams), "steps": len(step_ms),
             "step_ms_p50": float(np.percentile(step_ms, 50)), "step_ms_p99": float(np.percentile(step_ms, 99)),
@@ -195,45 +252,66 @@ def main():
     rt_counts = [int(v) for v in args.rt_streams.split(",") if v]
     streams = utterances(max(counts + rt_counts), args.seconds, args.seed)
 
-    # one pool for every run: its graphs are captured once, in the warm-up (as is restore_stream's workspace)
+    # one pool of each kind for every run: its graphs are captured once, in the warm-up (as is restore_stream's workspace)
     pool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows)
     print(f"pool: window {pool.window_len} samples, buckets {pool.buckets}", flush=True)
     warm(pool)
+    dpool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows)
+    warm(dpool, device=True)
     list(vf.restore_stream(blocks_of(streams[0][:3 * SR], block), args.chunk, args.ctx))
 
-    table_a, host = [], None
+    table_a, host, dev_share = [], None, None
     for n in counts:
-        steps = []
+        steps, dsteps = [], []
+        last = n == max(counts)
+        replays, dreplays = (time_replays(pool), time_replays(dpool)) if last else ([], [])
         pool_out, pool_s = run_pool(pool, streams[:n], block, timed_steps=steps)
+        dev_out, dev_s = run_pool(dpool, streams[:n], block, timed_steps=dsteps, device=True)
+        torch.cuda.synchronize()
         rr_out, rr_s = run_round_robin(vf, streams[:n], block, args)
         same = all(a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
                    for a, b in zip(pool_out, rr_out))
         assert same, f"N = {n}: the pool's output differs from restore_stream's"
+        dev_same = all(a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
+                       for a, b in zip(dev_out, pool_out))
+        assert dev_same, f"N = {n}: the device pool's output differs from the host pool's"
         audio_s = sum(len(y) for y in pool_out) / SR
         row = {"streams": n, "audio_s": audio_s, "pool_audio_s_per_s": audio_s / pool_s,
-               "round_robin_audio_s_per_s": audio_s / rr_s, "pool_s": pool_s, "round_robin_s": rr_s,
-               "steps": len(steps), "bit_identical": same}
+               "device_pool_audio_s_per_s": audio_s / dev_s, "round_robin_audio_s_per_s": audio_s / rr_s,
+               "pool_s": pool_s, "device_pool_s": dev_s, "round_robin_s": rr_s, "steps": len(steps),
+               "bit_identical": same and dev_same}
         table_a.append(row)
         print(json.dumps(row), flush=True)
-        if n == max(counts):                        # (c) at the largest N
-            per_bucket = {B: replay_ms(pool, B) for B in sorted({b for b, _ in steps})}
+        if last:                                    # (c) at the largest N
+            # the replays inside the steps, timed by events around each: their lengths are the steps' own (a replay
+            # repeated afterwards, replay_ms, reads the last step's lengths, and ragged rows cost what they hold)
+            replay_s = sum(a.elapsed_time(b) for a, b in replays) / 1e3
             step_s = sum(t for _, t in steps)
-            replay_s = sum(per_bucket[b] for b, _ in steps) / 1e3
             host = {"streams": n, "steps": len(steps), "step_s": step_s, "replay_s": replay_s,
-                    "host_share": 1.0 - replay_s / step_s, "replay_ms_per_bucket": per_bucket}
+                    "host_share": 1.0 - replay_s / step_s,
+                    "replay_ms_per_bucket_repeated": {B: replay_ms(pool, B) for B in sorted({b for b, _ in steps})}}
             print(json.dumps(host), flush=True)
+            replay_s = sum(a.elapsed_time(b) for a, b in dreplays) / 1e3
+            step_s = sum(a.elapsed_time(b) for _, a, b in dsteps) / 1e3
+            dev_share = {"streams": n, "steps": len(dsteps), "device_step_s": step_s, "replay_s": replay_s,
+                         "outside_replay_share": 1.0 - replay_s / step_s, "wall_s": dev_s,
+                         "outside_replay_share_of_wall": 1.0 - replay_s / dev_s}
+            print(json.dumps({"device_pool": dev_share}), flush=True)
 
-    rng = np.random.default_rng(args.seed + 1)
-    table_b = []
-    for n in rt_counts:
-        row = run_real_time(pool, streams[:n], block, args, rng)
-        table_b.append(row)
-        print(json.dumps(row), flush=True)
-    assert pool.graph_count == len(pool.buckets)    # nothing was captured after the warm-up
-    largest = max([r["streams"] for r in table_b if r["keeps_real_time"]], default=0)
+    table_b = {}
+    for kind, p in (("host", pool), ("device", dpool)):
+        rng = np.random.default_rng(args.seed + 1)
+        table_b[kind] = []
+        for n in rt_counts:
+            row = run_real_time(p, streams[:n], block, args, rng, device=kind == "device")
+            table_b[kind].append(row)
+            print(json.dumps({"pool": kind, **row}), flush=True)
+        assert p.graph_count == len(p.buckets)      # nothing was captured after the warm-up
+    largest = {kind: max([r["streams"] for r in rows if r["keeps_real_time"]], default=0)
+               for kind, rows in table_b.items()}
     print(json.dumps({"gpu": info, "precision": args.precision, "seconds": args.seconds, "block_s": args.block_seconds,
                       "chunk_s": args.chunk, "ctx_s": args.ctx, "throughput": table_a, "real_time": table_b,
-                      "largest_real_time_streams": largest, "host_share": host}))
+                      "largest_real_time_streams": largest, "host_share": host, "device_pool_share": dev_share}))
 
 
 if __name__ == "__main__":

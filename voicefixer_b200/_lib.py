@@ -57,7 +57,7 @@ class ResampleSrcItem(ctypes.Structure):
 
 class ScatterItem(ctypes.Structure):
     """struct vfx_scatter_item (include/vfx_b200.h)."""
-    _fields_ = [("dst", _vp), ("dst_elems", _ll), ("dst_off", _ll), ("len", _i)]
+    _fields_ = [("dst", _vp), ("dst_elems", _ll), ("dst_off", _ll), ("len", _i), ("src_off", _i)]
 
 
 # name -> (restype, argtypes); must list every symbol include/vfx_b200.h declares

@@ -214,6 +214,27 @@ def oracle_rows(idx, lengths):
     return [(i, 0, _gen_len(1 + lengths[i] // 441)) for i in idx]
 
 
+def stream_rows(rows):
+    """The tables of one device StreamPool step: rows = [(rate, base, n, (lo, hi, keep_lo, keep_hi)), ...], one per
+    window, its stream holding input samples [base, n) at `rate`, base a multiple of down ((up, down) =
+    resample.ratio(rate)), and every input the window reads at or after base.  Returns (gather, emit):
+
+    gather: one (n_in, y_first, y_len) per row (Engine.resample_src): the window is output samples [y_first, y_first +
+    y_len) of the held input read as a recording of its own, n_in = n - base samples.  With base = k * down, output J
+    of the stream is output J - k * up of that recording: both sum the same inputs with the same taps in the same
+    order, so the row is bit-identical to the window resampled from the whole stream.
+    emit: one (src_off, len) per row (Engine.scatter_rows): the kept samples [keep_lo, keep_hi) start src_off = keep_lo
+    - lo samples into the window's row."""
+    gather, emit = [], []
+    for rate, base, n, (lo, hi, keep_lo, keep_hi) in rows:
+        up, down = resample.ratio(rate)
+        if base % down:
+            raise ValueError(f"stream_rows: base {base} is not a multiple of down = {down} (rate {rate})")
+        gather.append((int(n - base), int(lo - base // down * up), int(hi - lo)))
+        emit.append((int(keep_lo - lo), int(keep_hi - keep_lo)))
+    return gather, emit
+
+
 _STREAM_SHORT = "restore_stream: fewer than 1025 samples in total; the front end reflect-pads 1024"
 
 
@@ -292,6 +313,42 @@ class _Stream:
             self.base = first
 
 
+class _DevStream(_Stream):
+    """One stream of a device StreamPool: _Stream's bookkeeping, its recent input at its own rate in one device buffer
+    (grown by doubling: a push copies its block in once, from any element stride).  Old input is dropped by moving the
+    start, as _Stream does, but only to a multiple of down ((up, down) = resample.ratio(rate)): base stays a multiple
+    of down, so the held input is a recording of its own to the resampler (stream_rows), and at most down - 1 samples
+    more than _Stream's are held."""
+
+    def __init__(self, rate, device):
+        super().__init__(rate)
+        self.down = resample.ratio(rate)[1]
+        self._data = torch.empty(0, device=device)
+
+    def append(self, a, st=None):
+        """a: a 1-D float32 tensor on the buffer's device.  st: the stream the copy runs on; a buffer this replaces is
+        not reused before st's queued work (which follows every earlier read of it) is done."""
+        m = a.shape[0]
+        if self._hi + m > self._data.shape[0]:
+            held = self.buf
+            data = torch.empty(max(4096, 2 * (held.shape[0] + m)), device=self._data.device)
+            data[:held.shape[0]].copy_(held)
+            self.release(st)
+            self._data = data
+            self._lo, self._hi = 0, held.shape[0]
+        self._data[self._hi:self._hi + m].copy_(a)
+        self._hi += m
+        self.n += m
+
+    def drop_before(self, first):
+        super().drop_before(first - first % self.down)
+
+    def release(self, st):
+        """Hands the buffer back to the allocator for reuse only after st's queued work is done."""
+        if st is not None and self._data.numel():
+            self._data.record_stream(st)
+
+
 class StreamPool:
     """Many live streams restored together (VoiceFixer.stream_pool), driven by one caller thread.
 
@@ -303,7 +360,20 @@ class StreamPool:
 
     A stream at another rate than 44.1 kHz is kept at its own rate on the host; its 44.1 kHz samples [0, m) are available
     once the input they read has arrived (resample.available), all of them after close().  Its windows are resampled on
-    the device (Engine.resample) into the step's input rows, bit-identical to wavio._resample on the whole stream."""
+    the device (Engine.resample) into the step's input rows, bit-identical to wavio._resample on the whole stream.
+
+    Host and device pools.  The first block pushed fixes the pool's kind for its lifetime: host blocks (anything numpy
+    takes), or 1-D float32 CUDA tensors on the engine's device, of any element stride >= 1 (e.g. x[:, c] of an
+    interleaved (L, C) tensor).  A host pool stages each step's windows on the host and returns numpy blocks, waiting
+    for the device at the end of every step.  A device pool keeps each stream's recent input in a device buffer at its
+    own rate (_DevStream); a step builds all its window rows with one Engine.resample_src launch (a copy at 44.1 kHz),
+    replays the bucket's graph, and copies each window's kept samples into a new 1-D float32 CUDA tensor with one
+    Engine.scatter_rows launch.  Everything is queued on torch.cuda.current_stream(); push, close and step return
+    without waiting for the GPU, except that the step which first uses a bucket captures its graph, and capturing
+    synchronises the device once.  Each stream's device blocks are bit-identical, block by block, to the host pool's
+    for the same audio and the same calls, at every rate and precision.  Calls on several CUDA streams run in the order
+    they were made (Engine._shared_stream), and a stream buffer a pool replaces or forgets is not reused before the
+    work that reads it is done."""
 
     def __init__(self, engine, chunk_seconds=2.0, context_seconds=1.0, max_windows=None, device=None):
         chunk = int(round(chunk_seconds * 44100))
@@ -330,6 +400,7 @@ class StreamPool:
         self._next_sid = 0
         self._graphs = {}                          # bucket -> captured restore graph
         self._bufs = None
+        self._kind = None                          # "host" or "device": fixed by the first block pushed
 
     # ------------------------------------------------------------------ the caller's side
     def open(self, sample_rate=44100):
@@ -337,16 +408,32 @@ class StreamPool:
         sid = self._next_sid
         rate = resample.check_rate(sample_rate, f"stream_pool.open: stream {sid}")
         self._next_sid += 1
-        self._streams[sid] = _Stream(rate)
+        self._streams[sid] = _DevStream(rate, self._dev) if self._kind == "device" else _Stream(rate)
         return sid
 
     def push(self, sid, block):
-        """Appends a 1-D block of any size, at the stream's own rate, to stream sid."""
+        """Appends a 1-D block of any size, at the stream's own rate, to stream sid: a host block, or in a device pool a
+        1-D float32 CUDA tensor on the engine's device (any element stride >= 1), which is read, never written.  A
+        block of the other kind than the pool's first, or a CUDA block that cannot be taken, raises ValueError naming
+        the stream, before anything changes."""
         s = self._open_stream(sid, "push")
-        a = np.asarray(block, dtype=np.float32)
-        if a.ndim != 1:
-            raise ValueError(f"stream_pool.push: stream {sid}: a block has shape {a.shape}; blocks are 1-D")
-        s.append(a)
+        cuda = is_cuda(block)
+        if self._kind is not None and cuda != (self._kind == "device"):
+            raise ValueError(f"stream_pool.push: stream {sid}: a {'CUDA' if cuda else 'host'} block in a pool of "
+                             f"{'CUDA' if self._kind == 'device' else 'host'} blocks; the first block pushed fixes a "
+                             "pool's kind for its lifetime")
+        if cuda:
+            self._check_device_block(sid, block)
+            if self._kind is None:
+                self._to_device()
+                s = self._streams[sid]
+            s.append(block, self._eng._shared_stream())
+        else:
+            a = np.asarray(block, dtype=np.float32)
+            if a.ndim != 1:
+                raise ValueError(f"stream_pool.push: stream {sid}: a block has shape {a.shape}; blocks are 1-D")
+            self._kind = "host"
+            s.append(a)
         self._schedule(sid, s, resample.available(s.n, s.rate), ended=False)
 
     def close(self, sid):
@@ -356,7 +443,7 @@ class StreamPool:
         try:
             self._schedule(sid, s, resample.out_len(s.n, s.rate), ended=True)
         except RuntimeError as e:
-            del self._streams[sid]
+            self._forget(sid)
             self._queue = deque(q for q in self._queue if q[0] != sid)
             raise RuntimeError(f"stream_pool.close: stream {sid}: {e}") from None
         s.closed = True
@@ -369,12 +456,17 @@ class StreamPool:
         batch = [self._queue.popleft() for _ in range(n)]
         out = {}
         if batch:
-            rows = self._run(batch)
-            for k, (sid, (lo, hi, keep_lo, keep_hi)) in enumerate(batch):
-                out.setdefault(sid, []).append(rows[k, keep_lo - lo:keep_hi - lo].copy())
+            if self._kind == "device":
+                blocks = self._run_device(batch)
+            else:
+                rows = self._run(batch)
+                blocks = [rows[k, keep_lo - lo:keep_hi - lo].copy()
+                          for k, (_, (lo, hi, keep_lo, keep_hi)) in enumerate(batch)]
+            for (sid, _), y in zip(batch, blocks):
+                out.setdefault(sid, []).append(y)
                 self._streams[sid].pending.popleft()
         for sid in [sid for sid, s in self._streams.items() if s.closed and not s.pending]:
-            del self._streams[sid]
+            self._forget(sid)
         for sid in out:
             if sid in self._streams:
                 self._trim(self._streams[sid])
@@ -404,6 +496,35 @@ class StreamPool:
         if s.closed:
             raise ValueError(f"stream_pool.{what}: stream {sid} is closed; its input has ended")
         return s
+
+    def _check_device_block(self, sid, block):
+        """Raises ValueError naming the stream for a CUDA block a device pool cannot take."""
+        who = f"stream_pool.push: stream {sid}: a CUDA block"
+        if torch.device(block.device) != torch.device(self._dev):
+            raise ValueError(f"{who} is on {block.device}; this pool runs on {self._dev}")
+        if block.dtype != torch.float32:
+            raise ValueError(f"{who} has dtype {block.dtype}; CUDA blocks must be torch.float32")
+        if len(block.shape) != 1:
+            raise ValueError(f"{who} has shape {tuple(block.shape)}; blocks are 1-D")
+        if block.stride(0) < 1:
+            raise ValueError(f"{who} has element stride {block.stride(0)} (an expanded tensor); its samples must be "
+                             "distinct elements (.contiguous() makes them so)")
+
+    def _to_device(self):
+        """Makes this a device pool; its streams, opened before any block was pushed, hold no input yet."""
+        for sid, s in self._streams.items():
+            assert s.n == 0 and not s.pending
+            d = _DevStream(s.rate, self._dev)
+            d.closed = s.closed
+            self._streams[sid] = d
+        self._kind = "device"
+
+    def _forget(self, sid):
+        """Drops stream sid; a device buffer goes back to the allocator once the work queued on the engine's last
+        stream, which follows every read of it, is done."""
+        s = self._streams.pop(sid)
+        if isinstance(s, _DevStream):
+            s.release(self._eng._last_stream)
 
     def _schedule(self, sid, s, avail, ended):
         windows, s.pos = self._sched.due(s.pos, avail, ended)
@@ -435,9 +556,10 @@ class StreamPool:
             pin = (lambda t: t.pin_memory()) if self._cuda else (lambda t: t)
             self._bufs = {"dev_in": torch.zeros((B, L), device=dev), "dev_out": torch.empty((B, L), device=dev),
                           "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
-                          "host_in": pin(torch.zeros((B, L))), "host_out": pin(torch.empty((B, L))),
-                          "host_lens": pin(torch.empty(B, dtype=torch.int32)),
                           "ws": torch.empty(self._eng.workspace_bytes(B, L), dtype=torch.uint8, device=dev)}
+            if self._kind != "device":             # a device pool stages nothing on the host
+                self._bufs.update({"host_in": pin(torch.zeros((B, L))), "host_out": pin(torch.empty((B, L))),
+                                   "host_lens": pin(torch.empty(B, dtype=torch.int32))})
         return self._bufs
 
     def _run(self, batch):
@@ -469,6 +591,25 @@ class StreamPool:
         if self._cuda:
             torch.cuda.current_stream().synchronize()
         return p["host_out"].numpy()
+
+    def _run_device(self, batch):
+        """Restores the windows of batch [(sid, (lo, hi, keep_lo, keep_hi)), ...] of a device pool and returns each
+        window's kept samples as a new CUDA tensor: one vfx_resample_src launch gathers the rows from the streams'
+        buffers, one graph replay restores them, one vfx_scatter_rows launch emits the kept spans.  Nothing waits."""
+        p = self._buffers()
+        n, B = len(batch), self.bucket(len(batch))
+        streams = [self._streams[sid] for sid, _ in batch]
+        gather, emit = stream_rows([(s.rate, s.base, s.n, w) for s, (_, w) in zip(streams, batch)])
+        self._eng.resample_src([(s.buf, s.rate, y_first, y_len) for s, (_, y_first, y_len) in zip(streams, gather)],
+                               self.window_len, y=p["dev_in"][:n], lens=p["dev_lens"][:n])
+        p["dev_lens"][n:B].fill_(1025)             # unused rows: any valid length; their output is never read
+        if B not in self._graphs:                  # captured once the lengths are in place: its warm-up runs read them
+            self._graphs[B] = self._eng.make_graph(p["dev_in"][:B], p["dev_out"][:B], mode=0, lens=p["dev_lens"][:B],
+                                                   ws=p["ws"])
+        self._graphs[B].replay()
+        blocks = [torch.empty(m, device=self._dev) for _, m in emit]
+        self._eng.scatter_rows(p["dev_out"][:n], [(y, 0, m, off) for y, (off, m) in zip(blocks, emit)])
+        return blocks
 
 
 class _ModelShim:
@@ -1002,7 +1143,9 @@ class VoiceFixer:
         blocks as they arrive, close() it at its end, and call step() to restore every window that is due, of every
         stream, in one ragged CUDA-graph replay.  Each stream's output is bit-identical to restore_stream on that
         stream's audio alone with the same chunk_seconds / context_seconds.  max_windows: the most windows one step
-        restores (default: as many as fit the device memory that is free, at most 64)."""
+        restores (default: as many as fit the device memory that is free, at most 64).  Blocks may be host arrays, or
+        1-D float32 CUDA tensors (any element stride), which the pool restores where they are and returns as new CUDA
+        tensors without waiting for the GPU (StreamPool: the first block pushed fixes which)."""
         _check_cuda(False)
         return StreamPool(self._engine, chunk_seconds, context_seconds, max_windows)
 

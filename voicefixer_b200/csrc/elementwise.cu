@@ -373,13 +373,14 @@ __global__ void frame_extents_kernel(const int* __restrict__ frames, int B, int 
   ext[(EXT_UP0 + 3) * B + b] = Tc * 441;
 }
 
-// Row b of a (B, ldx) batch -> items[b].dst[dst_off, dst_off + len) (vfx_scatter_rows): one thread per sample.
+// Row b of a (B, ldx) batch, from column src_off -> items[b].dst[dst_off, dst_off + len) (vfx_scatter_rows): one
+// thread per sample.
 __global__ void __launch_bounds__(256) scatter_rows_kernel(const float* __restrict__ x, long long ldx,
                                                            const vfx_scatter_item* __restrict__ items) {
   const int b = blockIdx.y;
   const vfx_scatter_item it = items[b];
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < it.len) it.dst[it.dst_off + j] = __ldg(x + (long long)b * ldx + j);
+  if (j < it.len) it.dst[it.dst_off + j] = __ldg(x + (long long)b * ldx + it.src_off + j);
 }
 
 inline int grid_for(long long total, int block = 256) {

@@ -842,6 +842,7 @@ int check_resample_src_item(const vfx_resample_src_item& it, int b, long long h_
 }
 
 // vfx_scatter_rows: the item table is staged into the workspace, then one launch
+static_assert(sizeof(vfx_scatter_item) == 32, "vfx_scatter_item: src_off must fit the tail padding");
 int scatter_rows_forward(Ctx& c, const float* x, int B, long long ldx, const vfx_scatter_item* items_host,
                          int max_len) {
   vfx_scatter_item* items = c.ws->alloc<vfx_scatter_item>(B);
@@ -859,6 +860,8 @@ int check_scatter_items(const vfx_scatter_item* items, int B, long long ldx, int
     const vfx_scatter_item& it = items[b];
     VFX_REQUIRE(it.dst, "scatter_rows: item %d: dst is null", b);
     VFX_REQUIRE(it.len >= 0 && it.len <= ldx, "scatter_rows: item %d: len %d is not in [0, ldx = %lld]", b, it.len, ldx);
+    VFX_REQUIRE(it.src_off >= 0 && it.src_off <= ldx - it.len, "scatter_rows: item %d: source columns [%d, %lld) are "
+                "not inside its row of ldx = %lld", b, it.src_off, (long long)it.src_off + it.len, ldx);
     VFX_REQUIRE(it.dst_off >= 0 && it.dst_elems >= 0 && it.dst_off <= it.dst_elems - it.len, "scatter_rows: item %d: "
                 "destination [%lld, %lld) is not inside its %lld elements", b, it.dst_off, it.dst_off + it.len,
                 it.dst_elems);

@@ -413,19 +413,26 @@ class Engine(_WorkspaceQueries):
         """Workspace of resample_src() on B items (vfx_resample_src_workspace_bytes; no engine needed)."""
         return int(_lib.load().vfx_resample_src_workspace_bytes(int(B)))
 
-    def resample_src(self, items, L_cap):
+    def resample_src(self, items, L_cap, y=None, lens=None):
         """resample() on recordings that are already on the device, read in place (vfx_resample_src): the same
         arithmetic, bit for bit, without staged windows; a rate of 44100 is a copy, so one launch builds a batch's rows.
 
         items: one (src, rate, y_first, y_len) per row: output samples [y_first, y_first + y_len) of the 44.1 kHz stream
         of src, a 1-D float32 CUDA tensor on this engine's device with any element stride, at `rate`.  src is never
         written.  Returns (y (B, L_cap) with row b's y_len samples then zeros, lens (B,) int32 device tensor of the
-        y_len)."""
+        y_len).  y, lens (optional): existing contiguous (B, L_cap) float32 / (B,) int32 tensors on this device to
+        write them into (e.g. the first rows of a captured graph's input), instead of new ones."""
         dev = torch.device(f"cuda:{self.device}")
         for b, (src, *_) in enumerate(items):
             if not (src.is_cuda and src.device == dev and src.dtype == torch.float32 and src.dim() == 1):
                 raise ValueError(f"resample_src: item {b}: src must be a 1-D float32 tensor on {dev}")
         B = len(items)
+        if y is not None and not (y.is_cuda and y.device == dev and y.dtype == torch.float32 and y.is_contiguous()
+                                  and tuple(y.shape) == (B, int(L_cap))):
+            raise ValueError(f"resample_src: y must be a contiguous ({B}, {int(L_cap)}) float32 tensor on {dev}")
+        if lens is not None and not (lens.device == dev and lens.dtype == torch.int32 and lens.is_contiguous()
+                                     and tuple(lens.shape) == (B,)):
+            raise ValueError(f"resample_src: lens must be a contiguous ({B},) int32 tensor on {dev}")
         offs = self._taps_for([it[1] for it in items])
         table = (_lib.ResampleSrcItem * B)()
         for b, (src, rate, y_first, y_len) in enumerate(items):
@@ -436,8 +443,10 @@ class Engine(_WorkspaceQueries):
             t.up, t.down, t.rem = up, down, resample.taps(rate)[1]
             t.h_off, t.h_len = offs.get((up, down), (0, 0))
         h = self._taps_dev
-        y = torch.empty(B, int(L_cap), device=dev)
-        lens = torch.empty(B, dtype=torch.int32, device=dev)
+        if y is None:
+            y = torch.empty(B, int(L_cap), device=dev)
+        if lens is None:
+            lens = torch.empty(B, dtype=torch.int32, device=dev)
         ws = self._workspace(self.resample_src_workspace_bytes(B))
         _lib.check(self.lib.vfx_resample_src(self.h, _ptr(h), 0 if h is None else h.numel(), table, B, _ptr(y),
                                              int(L_cap), _ptr(lens), _ptr(ws), ws.numel(), _stream()),
@@ -451,9 +460,10 @@ class Engine(_WorkspaceQueries):
 
     def scatter_rows(self, x, items):
         """Copies the rows of a batch into their own tensors in one launch (vfx_scatter_rows): row b of x (B, ldx), a
-        float32 CUDA tensor with unit column stride, gives its first len_b samples to dst_b.view(-1)[off_b : off_b +
-        len_b].  items: one (dst_b, off_b, len_b) per row, dst_b a contiguous float32 CUDA tensor on this device.  The
-        destination ranges must not overlap."""
+        float32 CUDA tensor with unit column stride, gives its samples [src_b, src_b + len_b) to dst_b.view(-1)[off_b :
+        off_b + len_b].  items: one (dst_b, off_b, len_b) or (dst_b, off_b, len_b, src_b) per row, dst_b a contiguous
+        float32 CUDA tensor on this device; src_b defaults to 0 (the row's first len_b samples).  The destination
+        ranges must not overlap."""
         dev = torch.device(f"cuda:{self.device}")
         if not (x.is_cuda and x.device == dev and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1):
             raise ValueError(f"scatter_rows: x must be a (B, ldx) float32 tensor on {dev} with unit column stride")
@@ -461,11 +471,12 @@ class Engine(_WorkspaceQueries):
         if len(items) != B:
             raise ValueError(f"scatter_rows: {len(items)} items for {B} rows")
         table = (_lib.ScatterItem * B)()
-        for b, (dst, off, n) in enumerate(items):
+        for b, (dst, off, n, *src_off) in enumerate(items):
             if not (dst.is_cuda and dst.device == dev and dst.dtype == torch.float32 and dst.is_contiguous()):
                 raise ValueError(f"scatter_rows: item {b}: dst must be a contiguous float32 tensor on {dev}")
             t = table[b]
             t.dst, t.dst_elems, t.dst_off, t.len = dst.data_ptr(), dst.numel(), int(off), int(n)
+            t.src_off = int(src_off[0]) if src_off else 0
         ws = self._workspace(self.scatter_rows_workspace_bytes(B))
         _lib.check(self.lib.vfx_scatter_rows(_ptr(x), B, x.stride(0), table, _ptr(ws), ws.numel(), _stream()),
                    "vfx_scatter_rows")
