@@ -45,6 +45,15 @@ enum vfx_precision { VFX_PREC_FP32 = 0, VFX_PREC_BF16 = 1, VFX_PREC_TF32 = 2, VF
 /* restore() modes, voicefixer/base.py:110-115. mode 1's pre-filter is vfx_hf_cut(). */
 enum vfx_mode { VFX_MODE_EVAL = 0, VFX_MODE_TRAIN_BN = 2 };
 
+/* Seeded dropout key of one item (vfx_restore_seeded, vfx_analysis_seeded, vfx_dropout_seeded; DESIGN.md §3).  Mode 2's
+ * keep bit of unit j in [0, 512) of frame t at dropout layer l (0: after dn.lin4, restorer/model.py:75; 1: after
+ * dn.lin11, model.py:94) is bit j % 32 of word (j % 128) / 32 of Philox4x32-10 with counter (t, 4 l + j / 128,
+ * stream & 0xffffffff, stream >> 32) and key (seed & 0xffffffff, seed >> 32); kept units are doubled, the others zeroed.
+ * The mask is a pure function of the key and the position: no mask tensor exists.  16 bytes, 8-byte aligned. */
+typedef struct vfx_drop_key {
+  unsigned long long seed, stream;
+} vfx_drop_key;
+
 const char* vfx_last_error(void);
 int vfx_version(void);
 
@@ -104,6 +113,11 @@ int vfx_frontend_mel(vfx_engine* e, const float* wav, int B, int L, float* mel, 
 int vfx_analysis(vfx_engine* e, const float* mel, int B, int T, int mode,
                  const uint8_t* drop_masks, float* mel_log_out, void* workspace,
                  size_t workspace_bytes, void* stream);
+/* vfx_analysis in mode 2 with seeded dropout: item b's masks come from keys[b] (device, B of them; vfx_drop_key)
+ * instead of a mask tensor.  Bit-identical to vfx_analysis(mode 2) with the masks the keys define.  B <= 65535; same
+ * workspace as vfx_analysis. */
+int vfx_analysis_seeded(vfx_engine* e, const float* mel, int B, int T, const vfx_drop_key* keys, float* mel_log_out,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 /* mel[B][T][128] -> wav[B][out_len].
  * Replaces Vocoder.forward (voicefixer/vocoder/base.py:42-56: de-weight, dB, normalise, tr_pre)
@@ -174,6 +188,14 @@ int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const 
 int vfx_restore_ragged_mode(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, int mode,
                             const uint8_t* drop_masks, float* wav_out, void* workspace, size_t workspace_bytes,
                             void* stream);
+
+/* Mode 2 with seeded dropout: lens NULL = B equal-length segments (vfx_restore), else a ragged batch as
+ * vfx_restore_ragged_mode, with its frame precondition.  Item b's masks come from keys[b] (device, B of them;
+ * vfx_drop_key), so row b depends on item b's samples and key only: bit-identical to the same call on item b alone,
+ * and to vfx_restore / vfx_restore_ragged_mode(mode 2) with the masks the keys define.  B <= 65535; same workspace as
+ * vfx_restore. */
+int vfx_restore_seeded(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, const vfx_drop_key* keys,
+                       float* wav_out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* mode 1 pre-filter, VoiceFixer.remove_higher_frequency (voicefixer/base.py:87-104) with the
  * librosa 0.10.1 stft/istft defaults (n_fft 2048, hop 512, Hann, center, zero pad):
@@ -381,6 +403,9 @@ int vfx_bn_act(int precision, const float* x, long long x_sB, long long ldx, int
                long long y_sB, long long ldy, void* stream);
 /* nn.Dropout(0.5) in train mode (restorer/model.py:75,94) in place: x[i] = keep[i] ? 2 x[i] : 0. */
 int vfx_dropout_apply(float* x, const uint8_t* keep, long long n, void* stream);
+/* Seeded dropout as the engine launches it in mode 2: x [B][T][512] in place (16-byte aligned), row b * T + t being
+ * frame t of item b, keys[b] (device, 8-byte aligned) its vfx_drop_key, layer 0 or 1.  B <= 65535. */
+int vfx_dropout_seeded(float* x, int B, int T, const vfx_drop_key* keys, int layer, void* stream);
 /* F.avg_pool2d(x, (2, 2)) (restorer/modules.py:103): x [B][H][W][C] (element strides, multiples of 4; x and y 16-byte
  * aligned, C % 4 == 0) -> dense y [B][H/2][W/2][C]. */
 int vfx_avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W, int C, float* y,

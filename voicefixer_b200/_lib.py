@@ -76,6 +76,7 @@ SIGNATURES = {
     "vfx_workspace_bytes_frames": (_sz, [_vp, _i, _i]),
     "vfx_frontend_mel": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "vfx_analysis": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_analysis_seeded": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_vocoder": (_i, [_vp, _vp, _i, _i, _i, _vp, _i, _f, _vp, _sz, _vp]),
     "vfx_vocoder_cond": (_i, [_vp, _vp, _i, _i, _vp, _i, _f, _vp, _sz, _vp]),
     "vfx_restore": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
@@ -88,6 +89,7 @@ SIGNATURES = {
     "vfx_gru_layer_ragged": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "vfx_restore_ragged": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "vfx_restore_ragged_mode": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "vfx_restore_seeded": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vfx_hf_cut_ragged": (_i, [_vp, _vp, _i, _i, _vp, _f, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vfx_vocoder_ragged": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _f, _vp, _sz, _vp]),
     "vfx_oracle_cond": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
@@ -102,6 +104,7 @@ SIGNATURES = {
     "vfx_bn_stats": (_i, [_vp, _ll, _ll, _i, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "vfx_bn_act": (_i, [_i, _vp, _ll, _ll, _i, _ll, _i, _vp, _vp, _i, _i, _i, _f, _vp, _ll, _ll, _vp]),
     "vfx_dropout_apply": (_i, [_vp, _vp, _ll, _vp]),
+    "vfx_dropout_seeded": (_i, [_vp, _i, _i, _vp, _i, _vp]),
     "vfx_avgpool2x2": (_i, [_vp, _ll, _ll, _ll, _i, _i, _i, _i, _vp, _vp]),
     "vfx_mask_log_pack": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "vfx_unet_head": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),

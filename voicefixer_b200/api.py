@@ -793,6 +793,53 @@ def _upload_masks(masks, dev):
     return masks.pin_memory().to(dev, non_blocking=True)
 
 
+def check_dropout_seed(s, who):
+    """s as an int if it is a valid seed of mode 2's seeded dropout (an integer in [0, 2^64), not a bool); else raises
+    ValueError `<who> has dropout_seed ...`."""
+    if isinstance(s, (bool, np.bool_)) or not isinstance(s, numbers.Integral) or not 0 <= int(s) < 1 << 64:
+        raise ValueError(f"{who} has dropout_seed {s!r}; a dropout seed is an integer in [0, 2^64)")
+    return int(s)
+
+
+def dropout_seeds(dropout_seed, mode, drop_masks_fn, n, what):
+    """restore_many's dropout_seed as one seed per recording: one int for all n recordings, or a list / tuple / array of
+    n of them (sample_rate's convention); None for dropout_seed=None.  Raises ValueError, naming the recording, for a bad
+    seed or a wrong count, and for a seed given in another mode than 2 or together with a drop_masks_fn."""
+    if dropout_seed is None:
+        return None
+    check_seeded(mode, drop_masks_fn, what)
+    if isinstance(dropout_seed, (list, tuple, np.ndarray)):
+        ss = list(np.asarray(dropout_seed, dtype=object).reshape(-1)) if isinstance(dropout_seed, np.ndarray) \
+            else list(dropout_seed)
+        if len(ss) != n:
+            raise ValueError(f"{what}: dropout_seed has {len(ss)} entries for {n} recordings; give one seed, or one per "
+                             "recording")
+    else:
+        ss = [dropout_seed] * n
+    return [check_dropout_seed(s, f"{what}: recording {i}") for i, s in enumerate(ss)]
+
+
+def check_seeded(mode, drop_masks_fn, what):
+    """Refuses a dropout seed outside mode 2, or next to a drop_masks_fn other than None (two sources of the masks)."""
+    if mode != 2:
+        raise ValueError(f"{what}: dropout_seed is mode 2's dropout; mode is {mode!r}")
+    if drop_masks_fn is not None:
+        raise ValueError(f"{what}: give dropout_seed or drop_masks_fn, not both")
+
+
+def drop_key_rows(segs, seeds):
+    """The seeded dropout keys of a batch (vfx_drop_key): segs = [(recording, a, b), ...] (plan_many's segments, a the
+    first sample of a 30 s segment), seeds one per recording -> uint64 (B, 2) rows (seed of the recording, a // SEG_LENGTH):
+    segment k of a recording draws its masks from stream k of its seed, whatever batch it runs in."""
+    return np.array([(seeds[i], a // SEG_LENGTH) for i, a, _ in segs], dtype=np.uint64).reshape(-1, 2)
+
+
+def _upload_keys(rows, dev):
+    """drop_key_rows on dev as the int64 (B, 2) tensor Engine.restore(drop_keys=) takes: 16 bytes per segment, from pinned
+    memory with a stream-ordered copy, so the host does not wait for the device."""
+    return torch.from_numpy(rows.view(np.int64)).pin_memory().to(dev, non_blocking=True)
+
+
 def _stage(items, rates, segs, dev, extents=None):
     """The device resampler's input for output ranges segs = [(recording, a, b), ...] of the 44.1 kHz streams: each
     range's input window (resample.window), concatenated on the host and uploaded as one staging buffer, and the items
@@ -876,19 +923,28 @@ class VoiceFixer:
         return out[0].cpu().numpy()
 
     @torch.no_grad()
-    def restore_inmem(self, wav_10k, cuda=False, mode=0, your_vocoder_func=None, drop_masks_fn=None):
+    def restore_inmem(self, wav_10k, cuda=False, mode=0, your_vocoder_func=None, drop_masks_fn=None, dropout_seed=None):
         """np (L,) float32 -> np (1, L) float32 (base.py:106-139).  The 30 s segments are
         independent (SURVEY D4), so all full segments run as one batch and the ragged tail as a
         second one; results are concatenated in order.
 
         drop_masks_fn (extension, mode 2 only): None = random Bernoulli(0.5) keep-masks like the reference's
         train-mode dropout; a callable (B, T) -> uint8 [2, B, T, 512] supplies them explicitly; False = no
-        dropout (deterministic train-mode BN only)."""
+        dropout (deterministic train-mode BN only).
+
+        dropout_seed (extension, mode 2 only, with drop_masks_fn=None): an int in [0, 2^64).  The masks are then
+        computed on the GPU from the seed (Philox4x32-10, DESIGN.md §3): segment k (the one starting at sample
+        k * SEG_LENGTH) uses philox.seeded_masks(dropout_seed, k, T_k), and no mask is drawn on the host or uploaded.
+        The result depends on the recording and the seed only; restore_many gives the same bits."""
         _check_cuda(cuda)
         if mode not in (0, 1, 2):
             raise ValueError("mode must be 0, 1 or 2")
+        if dropout_seed is not None:
+            check_seeded(mode, drop_masks_fn, "restore_inmem")
+            dropout_seed = check_dropout_seed(dropout_seed, "restore_inmem")
         wav = np.ascontiguousarray(wav_10k, dtype=np.float32)
-        segs = [wav[a:b] for a, b in segment_bounds(wav.shape[0])]
+        bounds = segment_bounds(wav.shape[0])
+        segs = [wav[a:b] for a, b in bounds]
         eng = self._engine
         dev = f"cuda:{eng.device}"
         groups = {}
@@ -907,12 +963,16 @@ class VoiceFixer:
                 x = torch.from_numpy(np.stack([segs[i] for i in idxs])).to(dev)
                 if mode == 1:
                     x, _ = eng.hf_cut(x)                                 # shorter: _net_len(L, 1)
-                masks = _drop_masks(drop_masks_fn, x.shape[0], 1 + x.shape[1] // 441) if mode == 2 else None
+                masks = keys = None
+                if dropout_seed is not None:
+                    keys = _upload_keys(drop_key_rows([(0,) + bounds[i] for i in idxs], [dropout_seed]), dev)
+                elif mode == 2:
+                    masks = _drop_masks(drop_masks_fn, x.shape[0], 1 + x.shape[1] // 441)
                 if your_vocoder_func is None:
-                    y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks)
+                    y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, drop_keys=keys)
                 else:                                                    # base.py:126-129
                     mel = eng.frontend(x)
-                    mel_log = eng.analysis(mel, mode=2 if mode == 2 else 0, drop_masks=masks)
+                    mel_log = eng.analysis(mel, mode=2 if mode == 2 else 0, drop_masks=masks, drop_keys=keys)
                     denoised = (10 ** torch.clip(mel_log, max=5))[:, None]
                     ys = []
                     for k in range(denoised.shape[0]):                   # the hook sees what the reference hands it:
@@ -929,7 +989,7 @@ class VoiceFixer:
         return out.cpu().numpy()
 
     @torch.no_grad()
-    def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None, sample_rate=44100):
+    def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None, sample_rate=44100, dropout_seed=None):
         """Extension of the reference API: restores a list of 1-D recordings of any lengths, in any mode, and returns a
         list of (1, L_i') arrays, element i what restore_inmem(wavs[i], cuda=True, mode=mode) returns -- bit-identical in
         modes 0 and 1 and in mode 2 with drop_masks_fn=False; in mode 2 with dropout, the same distribution.
@@ -956,7 +1016,16 @@ class VoiceFixer:
         same distribution).  Each batch's rows come from one vfx_resample_src launch and its restored segments go to their
         offsets in the outputs with one vfx_scatter_rows launch, all on torch.cuda.current_stream(); the call returns
         without waiting for the GPU, and no sample crosses PCIe.  A list that mixes CUDA and host items, or a CUDA item
-        on another device, of another dtype or not 1-D, raises ValueError before anything is launched."""
+        on another device, of another dtype or not 1-D, raises ValueError before anything is launched.
+
+        dropout_seed (mode 2, with drop_masks_fn=None): one int in [0, 2^64) for every recording, or a list / tuple /
+        array with one per recording; a bad seed or count raises ValueError naming the recording before anything is
+        launched.  Segment k of recording i then draws its masks on the GPU from (seed_i, k) (Philox4x32-10, DESIGN.md
+        §3): no mask is drawn on the host or exists anywhere, and each batch uploads only its 16-byte keys (from pinned
+        memory, without a host wait).  Element i depends on recording i and its seed only: it is bit-identical to
+        restore_inmem(wavs[i], cuda=True, mode=2, dropout_seed=seed_i) and to restore_many([wavs[i]], mode=2,
+        dropout_seed=seed_i)[0], whatever the other recordings, their order, the batch plan, host or CUDA input, or
+        sample_rate.  Recordings given the same seed share their masks segment by segment; distinct seeds avoid that."""
         _check_cuda(cuda)
         eng = self._engine
         dev = f"cuda:{eng.device}"
@@ -969,6 +1038,7 @@ class VoiceFixer:
                 raise ValueError(f"restore_many: recording {i} has shape {a.shape}; the list takes 1-D arrays")
             items.append(a)
         rates = resample.rates(sample_rate, len(items), "restore_many")
+        seeds = dropout_seeds(dropout_seed, mode, drop_masks_fn, len(items), "restore_many")
 
         def max_items(L_cap):
             extra = 0 if on_dev else _staging_extra(L_cap, rates)
@@ -984,10 +1054,14 @@ class VoiceFixer:
             x, lens = _batch_input(eng, items, rates, segs, L_cap, dev)
             if mode == 1:
                 x, _, lens = eng.hf_cut(x, lens=lens)
-            masks = _drop_masks(drop_masks_fn, len(segs), 1 + L_cap // 441) if mode == 2 else None
-            if on_dev:
-                masks = _upload_masks(masks, dev)
-            y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens)
+            masks = keys = None
+            if seeds is not None:
+                keys = _upload_keys(drop_key_rows(segs, seeds), dev)
+            elif mode == 2:
+                masks = _drop_masks(drop_masks_fn, len(segs), 1 + L_cap // 441)
+                if on_dev:
+                    masks = _upload_masks(masks, dev)
+            y = eng.restore(x, mode=2 if mode == 2 else 0, drop_masks=masks, lens=lens, drop_keys=keys)
             if on_dev:
                 eng.scatter_rows(y, [(outs[i], off, n) for i, off, n in restore_rows(segs, mode)])
                 continue

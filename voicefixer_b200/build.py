@@ -53,13 +53,13 @@ def build(force=False, verbose=False):
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     procs = []
+    headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + [
+        os.path.join(HERE, "..", "include", "vfx_b200.h")]
     for s in SOURCES:
         obj = os.path.join(objdir, s.replace(".cu", ".o"))
         src = os.path.join(CSRC, s)
-        if (not force and os.path.exists(obj) and os.path.getmtime(obj) > os.path.getmtime(src)
-                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "vfx_common.cuh"))
-                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "tc_ptx.cuh"))
-                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(HERE, "..", "include", "vfx_b200.h"))):
+        if (not force and os.path.exists(obj)
+                and all(os.path.getmtime(obj) > os.path.getmtime(d) for d in [src] + headers)):
             continue
         cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", src, "-o", obj]
         procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

@@ -1,5 +1,6 @@
 // HBM-bound elementwise / reduction kernels of the path (all channels-last).
 #include "vfx_common.cuh"
+#include "philox.cuh"
 
 namespace vfx {
 
@@ -121,6 +122,37 @@ __global__ void dropout_kernel(float* __restrict__ x, const uint8_t* __restrict_
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x)
     x[i] = keep[i] ? x[i] * 2.0f : 0.f;     // nn.Dropout(0.5): scale 1/(1-p)
+}
+
+// Seeded dropout (DESIGN.md §3): the keep bit of unit j of frame t of item b at `layer` is bit (j % 32) of word
+// (j % 128) / 32 of Philox4x32-10(counter (t, 4 layer + j / 128, stream lo, stream hi), key (seed lo, seed hi)),
+// (seed, stream) = keys[b].  One warp per frame row of 512 units: lane l serves 128-unit group g = l / 8 and computes its
+// Philox call (8 lanes share one); for word i it takes units 128 g + 32 i + 4 (l % 8) .. + 3, i.e. bits 4 (l % 8) .. + 3,
+// as one 16-byte access, so each warp access covers four whole 128-byte lines.  Rows t >= T_b are treated like the
+// others: nothing reads them.
+constexpr int DROP_ROWS = 8;                 // frame rows (warps) per block
+
+__global__ void __launch_bounds__(32 * DROP_ROWS) dropout_seeded_kernel(float* __restrict__ x, int T,
+                                                                        const vfx_drop_key* __restrict__ keys,
+                                                                        int layer) {
+  const int b = blockIdx.y;
+  const int t = blockIdx.x * DROP_ROWS + (threadIdx.x >> 5);
+  if (t >= T) return;
+  const int lane = threadIdx.x & 31, g = lane >> 3, s = lane & 7;
+  const unsigned long long seed = keys[b].seed, stream = keys[b].stream;
+  const philox4 r = philox4x32_10((uint32_t)t, (uint32_t)(4 * layer + g), (uint32_t)stream, (uint32_t)(stream >> 32),
+                                  (uint32_t)seed, (uint32_t)(seed >> 32));
+  float4* p = reinterpret_cast<float4*>(x + ((long long)b * T + t) * 512 + 128 * g + 4 * s);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t bits = r.w[i] >> (4 * s);
+    float4 v = p[8 * i];
+    v.x = (bits & 1u) ? v.x * 2.0f : 0.f;
+    v.y = (bits & 2u) ? v.y * 2.0f : 0.f;
+    v.z = (bits & 4u) ? v.z * 2.0f : 0.f;
+    v.w = (bits & 8u) ? v.w * 2.0f : 0.f;
+    p[8 * i] = v;
+  }
 }
 
 // F.avg_pool2d(x, (2,2)) voicefixer/restorer/modules.py:103 (floor: odd last column dropped)
@@ -447,6 +479,17 @@ int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, 
 int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st) {
   VFX_REQUIRE(x && keep && n > 0, "dropout_apply: bad arguments (n %lld)", n);
   dropout_kernel<<<grid_for(n), 256, 0, st>>>(x, keep, n);
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+int dropout_seeded(float* x, int B, int T, const vfx_drop_key* keys, int layer, cudaStream_t st) {
+  VFX_REQUIRE(x && keys && B > 0 && B <= 65535 && T > 0 && (layer == 0 || layer == 1),
+              "dropout_seeded: bad arguments (B %d, T %d, layer %d; B <= 65535, layer 0 or 1)", B, T, layer);
+  VFX_REQUIRE(aligned16(x) && ((uintptr_t)keys & 7) == 0,
+              "dropout_seeded: x must be 16-byte aligned and keys 8-byte aligned");
+  dim3 grid(ceil_div(T, DROP_ROWS), B);
+  dropout_seeded_kernel<<<grid, 32 * DROP_ROWS, 0, st>>>(x, T, keys, layer);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

@@ -469,10 +469,26 @@ int relu_inplace(Ctx& c, float* x, int B, int T, int C) {
                 (long long)T * C, C, c.st);
 }
 
+// Mode 2's dropout masks: explicit keep-masks uint8 [2][B][T][512], or one seeded key per item (both NULL: no dropout).
+// Either way the caller owns the memory, so the workspace does not depend on the choice.
+struct DropSrc {
+  const uint8_t* masks = nullptr;
+  const vfx_drop_key* keys = nullptr;
+};
+
+// Dropout `layer` (0: after lin4, 1: after lin11) in place on x [B][T][512]
+int dropout(Ctx& c, float* x, int B, int T, const DropSrc& drop, int layer) {
+  if (!c.train() || c.dry) return VFX_OK;
+  const long long n = (long long)B * T * 512;
+  if (drop.keys) return dropout_seeded(x, B, T, drop.keys, layer, c.st);
+  if (drop.masks) return dropout_apply(x, drop.masks + layer * n, n, c.st);
+  return VFX_OK;
+}
+
 // Ragged batch: every op but the GRU recurrence and the train-mode statistics is per frame (Linear GEMMs over B*T rows,
 // BatchNorm and ReLU via bn_act, dropout), so frames beyond an item's end only produce values that no later kernel reads;
 // the GRU and the statistics take the items' frame counts (EXT_FRAMES).
-int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop, float* lin_out) {
+int denoiser_forward(Ctx& c, const float* mel, int B, int T, const DropSrc& drop, float* lin_out) {
   const long long M = (long long)B * T;
   const int prec = c.prec();
   void* a = c.ws->alloc<float>(M * 512);          // operand scratch (fp32-sized)
@@ -486,19 +502,19 @@ int denoiser_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop
   VFX_TRY(relu_inplace(c, b, B, T, 256));
   VFX_TRY(bn_act_op(c, prec, p + "bn3", 1, b, (long long)T * 256, 256, B, T, 256, fr, 1, VFX_ACT_NONE, 0.f, a));
   VFX_TRY(linear(c, a, M, 256, p + "lin4", 512, b, nullptr, 0));
-  if (c.train() && drop && !c.dry) VFX_TRY(dropout_apply(b, drop, M * 512, c.st));
+  VFX_TRY(dropout(c, b, B, T, drop, 0));
   VFX_TRY(relu_inplace(c, b, B, T, 512));
   VFX_TRY(bn_gru(c, p + "g7", b, B, T, a, gi, y0, b));       // result in b
   VFX_TRY(bn_gru(c, p + "g8", b, B, T, a, gi, y0, b));
   VFX_TRY(bn_act_op(c, prec, p + "bn9", 1, b, (long long)T * 512, 512, B, T, 512, fr, 1, VFX_ACT_LRELU, 0.f, a));
   VFX_TRY(linear(c, a, M, 512, p + "lin11", 512, b, nullptr, 0));
-  if (c.train() && drop && !c.dry) VFX_TRY(dropout_apply(b, drop + M * 512, M * 512, c.st));
+  VFX_TRY(dropout(c, b, B, T, drop, 1));
   VFX_TRY(bn_act_op(c, prec, p + "bn13", 1, b, (long long)T * 512, 512, B, T, 512, fr, 1, VFX_ACT_LRELU, 0.f, a));
   VFX_TRY(linear(c, a, M, 512, p + "lin15", 128, lin_out, nullptr, 0));
   return c.rc;
 }
 
-int analysis_forward(Ctx& c, const float* mel, int B, int T, const uint8_t* drop, float* mel_log_out) {
+int analysis_forward(Ctx& c, const float* mel, int B, int T, const DropSrc& drop, float* mel_log_out) {
   const int Tp = (T + 63) / 64 * 64;
   // mode 2: the reference's train-mode BatchNorm raises "Expected more than 1 value per channel when training"
   // when the UNet centre is 1x1, i.e. for segments of at most 64 frames (checked on the capacity; a ragged item that
@@ -907,7 +923,7 @@ void slaney_htk_mel_basis(std::vector<float>& basis, std::vector<int>& band) {
 }
 
 // lens (ragged batch): per-item lengths on the device; L is then the capacity (row stride of wav / wav_out)
-int restore_forward(Ctx& c, const float* wav, int B, int L, const uint8_t* drop, const int* lens, float* wav_out) {
+int restore_forward(Ctx& c, const float* wav, int B, int L, const DropSrc& drop, const int* lens, float* wav_out) {
   const int T = 1 + L / 441;
   if (lens) {
     int* ext = c.ws->alloc<int>((size_t)EXT_LEVELS * B);
@@ -1072,10 +1088,10 @@ int vfx_engine_set_tensor(vfx_engine* e, const char* name, const void* dev_ptr, 
 // vfx_restore_ragged's extent table, so one workspace size serves both entry points.
 static size_t dry_run(vfx_engine* e, int B, int T, int L, int* rc) {
   const size_t peak = dry_peak(e, VFX_MODE_TRAIN_BN, [&](Ctx& c) {
-    if (L > 0) return restore_forward(c, nullptr, B, L, nullptr, nullptr, nullptr);
+    if (L > 0) return restore_forward(c, nullptr, B, L, DropSrc(), nullptr, nullptr);
     float* mel = c.ws->alloc<float>((size_t)B * T * 128);
     const bool voc_only = e->finalized && !(e->parts & VFX_PART_ANALYSIS);
-    const int r = voc_only ? VFX_OK : analysis_forward(c, mel, B, T, nullptr, mel);
+    const int r = voc_only ? VFX_OK : analysis_forward(c, mel, B, T, DropSrc(), mel);
     return r != VFX_OK ? r : vocoder_forward(c, mel, B, T, 1, nullptr, -1, 1.f);
   }, rc);
   return peak + std::max<size_t>(4096, ext_table_bytes(B));
@@ -1169,8 +1185,27 @@ int vfx_analysis(vfx_engine* e, const float* mel, int B, int T, int mode, const 
   VFX_NEED_ANALYSIS(e);
   VFX_REQUIRE(mel && mel_log_out && B > 0 && T > 0 && workspace, "analysis: bad arguments");
   VFX_REQUIRE(mode == VFX_MODE_EVAL || mode == VFX_MODE_TRAIN_BN, "analysis: bad mode %d", mode);
+  DropSrc drop;
+  drop.masks = drop_masks;
   return planned_call(e, mode, workspace, workspace_bytes, stream,
-                      [&](Ctx& c) { return analysis_forward(c, mel, B, T, drop_masks, mel_log_out); });
+                      [&](Ctx& c) { return analysis_forward(c, mel, B, T, drop, mel_log_out); });
+}
+
+// The key table of a seeded call: checked before any launch, since the dropout kernel's grid holds B in y
+#define VFX_DROP_KEYS(what)                                                                                          \
+  VFX_REQUIRE(keys && ((uintptr_t)keys & 7) == 0, what ": keys must be a non-null, 8-byte aligned device pointer");   \
+  VFX_REQUIRE(B <= 65535, what ": B=%d exceeds 65535", B)
+
+int vfx_analysis_seeded(vfx_engine* e, const float* mel, int B, int T, const vfx_drop_key* keys, float* mel_log_out,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_DROP_KEYS("analysis_seeded");
+  VFX_ENTER(e);
+  VFX_NEED_ANALYSIS(e);
+  VFX_REQUIRE(mel && mel_log_out && B > 0 && T > 0 && workspace, "analysis_seeded: bad arguments");
+  DropSrc drop;
+  drop.keys = keys;
+  return planned_call(e, VFX_MODE_TRAIN_BN, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return analysis_forward(c, mel, B, T, drop, mel_log_out); });
 }
 
 int vfx_vocoder(vfx_engine* e, const float* mel, int B, int T, int input_is_log, float* wav_out, int trim_len,
@@ -1220,7 +1255,7 @@ int vfx_oracle(vfx_engine* e, const float* wav, int B, int L_cap, const int* len
                       [&](Ctx& c) { return oracle_forward(c, wav, B, L_cap, lens, scale, wav_out); });
 }
 
-static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
+static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode, const DropSrc& drop,
                          const int* lens, float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
   VFX_ENTER(e);
   VFX_NEED_ANALYSIS(e);
@@ -1228,19 +1263,31 @@ static int restore_entry(vfx_engine* e, const float* wav, int B, int L, int mode
   VFX_REQUIRE(mode == VFX_MODE_EVAL || mode == VFX_MODE_TRAIN_BN, "restore: bad mode %d", mode);
   VFX_REQUIRE(L > 1024, "restore: L=%d must exceed 1024 samples", L);
   return planned_call(e, mode, workspace, workspace_bytes, stream,
-                      [&](Ctx& c) { return restore_forward(c, wav, B, L, drop_masks, lens, wav_out); });
+                      [&](Ctx& c) { return restore_forward(c, wav, B, L, drop, lens, wav_out); });
 }
 
 int vfx_restore(vfx_engine* e, const float* wav, int B, int L, int mode, const uint8_t* drop_masks,
                 float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
-  return restore_entry(e, wav, B, L, mode, drop_masks, nullptr, wav_out, workspace, workspace_bytes, stream);
+  DropSrc drop;
+  drop.masks = drop_masks;
+  return restore_entry(e, wav, B, L, mode, drop, nullptr, wav_out, workspace, workspace_bytes, stream);
 }
 
 int vfx_restore_ragged_mode(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, int mode,
                             const uint8_t* drop_masks, float* wav_out, void* workspace, size_t workspace_bytes,
                             void* stream) {
   VFX_REQUIRE(lens, "restore_ragged: lens is null");
-  return restore_entry(e, wav, B, L_cap, mode, drop_masks, lens, wav_out, workspace, workspace_bytes, stream);
+  DropSrc drop;
+  drop.masks = drop_masks;
+  return restore_entry(e, wav, B, L_cap, mode, drop, lens, wav_out, workspace, workspace_bytes, stream);
+}
+
+int vfx_restore_seeded(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, const vfx_drop_key* keys,
+                       float* wav_out, void* workspace, size_t workspace_bytes, void* stream) {
+  VFX_DROP_KEYS("restore_seeded");
+  DropSrc drop;
+  drop.keys = keys;
+  return restore_entry(e, wav, B, L_cap, VFX_MODE_TRAIN_BN, drop, lens, wav_out, workspace, workspace_bytes, stream);
 }
 
 int vfx_restore_ragged(vfx_engine* e, const float* wav, int B, int L_cap, const int* lens, float* wav_out,
@@ -1372,6 +1419,10 @@ int vfx_bn_act(int precision, const float* x, long long x_sB, long long ldx, int
 
 int vfx_dropout_apply(float* x, const uint8_t* keep, long long n, void* stream) {
   return dropout_apply(x, keep, n, (cudaStream_t)stream);
+}
+
+int vfx_dropout_seeded(float* x, int B, int T, const vfx_drop_key* keys, int layer, void* stream) {
+  return dropout_seeded(x, B, T, keys, layer, (cudaStream_t)stream);
 }
 
 int vfx_avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W, int C, float* y,

@@ -113,6 +113,8 @@ int bn_stats(const float* x, long long x_sB, long long ldx, int B, long long P, 
              const float* gamma, const float* beta, float* scale, float* shift, double* acc,
              const int* seq, int per_row, cudaStream_t st);
 int dropout_apply(float* x, const uint8_t* keep, long long n, cudaStream_t st);
+// seeded dropout in place on x fp32 [B][T][512] at denoiser dropout `layer` (0 or 1), item b keyed by keys[b] (device)
+int dropout_seeded(float* x, int B, int T, const vfx_drop_key* keys, int layer, cudaStream_t st);
 int avgpool2x2(const float* x, long long x_sB, long long x_sH, long long x_sW, int B, int H, int W,
                int C, float* y, cudaStream_t st);
 // Ragged batches: the kernels below that take `ext_*` / `lens` pointers (device int32 [B], NULL = every item spans the

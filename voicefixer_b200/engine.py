@@ -214,14 +214,21 @@ class Engine(_WorkspaceQueries):
         _lib.check(self.lib.vfx_frontend_mel(self.h, _ptr(wav), B, L, _ptr(mel), _ptr(sp), _stream()), "vfx_frontend_mel")
         return (mel, sp) if return_sp else mel
 
-    def analysis(self, mel, mode=0, drop_masks=None):
-        """mel (B, T, 128) linear -> log10 mel (B, T, 128)."""
+    def analysis(self, mel, mode=0, drop_masks=None, drop_keys=None):
+        """mel (B, T, 128) linear -> log10 mel (B, T, 128).  drop_keys (mode 2, in place of drop_masks): seeded dropout
+        keys, as in restore() (vfx_analysis_seeded)."""
         mel = self._dev(mel)
         B, T, F = mel.shape
         if F != 128:
             raise AssertionError("mel must have 128 bins")
+        if drop_keys is not None:
+            self._check_keys(drop_keys, B, mode, drop_masks)
         out = torch.empty_like(mel)
         ws = self._workspace(self.workspace_bytes_frames(B, T))
+        if drop_keys is not None:
+            _lib.check(self.lib.vfx_analysis_seeded(self.h, _ptr(mel), B, T, _ptr(drop_keys), _ptr(out), _ptr(ws),
+                                                    ws.numel(), _stream()), "vfx_analysis_seeded")
+            return out
         dm = None
         if drop_masks is not None:
             dm = drop_masks.to(device=mel.device, dtype=torch.uint8).contiguous()
@@ -292,20 +299,33 @@ class Engine(_WorkspaceQueries):
                                        _stream()), "vfx_oracle")
         return out
 
-    def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None, lens=None):
+    def restore(self, wav, mode=0, drop_masks=None, out=None, ws=None, lens=None, drop_keys=None):
         """wav (B, L) on device -> restored wav (B, L) on device (one launch sequence).
 
         lens (ragged batch): int32 device tensor (B,) of per-item lengths <= L.  Row b of `wav` then holds item b in its
         first lens[b] samples; row b of the result is bit-identical to restoring that item alone, followed by zeros.
         Lengths are read on the device (vfx_restore_ragged_mode), so a captured graph serves any lengths.  In mode 2,
         drop_masks is (2, B, T_cap, 512) with T_cap = 1 + L // 441 (item b reads [:, b, :T_b]) and every item needs more
-        than 64 frames (1 + lens[b] // 441 > 64; an item below that gets finite, unspecified samples)."""
+        than 64 frames (1 + lens[b] // 441 > 64; an item below that gets finite, unspecified samples).
+
+        drop_keys (mode 2, in place of drop_masks): seeded dropout (vfx_restore_seeded), a contiguous int64 CUDA tensor
+        (B, 2) whose row b holds the bit patterns of item b's (seed, stream) (vfx_drop_key; a value >= 2^63 appears as
+        its negative two's complement).  Item b's masks are then philox.seeded_masks(seed_b, stream_b, T_b), computed in
+        the kernels, so its row depends on its own samples and key only."""
         wav = self._dev(wav)
         B, L = wav.shape
+        if drop_keys is not None:
+            self._check_keys(drop_keys, B, mode, drop_masks)
         if out is None:
             out = torch.empty_like(wav)
         if ws is None:
             ws = self._workspace(self.workspace_bytes(B, L))
+        if drop_keys is not None:
+            if lens is not None:
+                _check_lens(lens, B)
+            _lib.check(self.lib.vfx_restore_seeded(self.h, _ptr(wav), B, L, _ptr(lens), _ptr(drop_keys), _ptr(out),
+                                                   _ptr(ws), ws.numel(), _stream()), "vfx_restore_seeded")
+            return out
         dm = None
         if drop_masks is not None:
             dm = drop_masks.to(device=wav.device, dtype=torch.uint8).contiguous()
@@ -319,6 +339,15 @@ class Engine(_WorkspaceQueries):
         _lib.check(self.lib.vfx_restore(self.h, _ptr(wav), B, L, int(mode), _ptr(dm), _ptr(out), _ptr(ws), ws.numel(),
                                         _stream()), "vfx_restore")
         return out
+
+    def _check_keys(self, keys, B, mode, drop_masks):
+        if drop_masks is not None:
+            raise ValueError("drop_keys and drop_masks are two sources of the same masks: give one of them")
+        if int(mode) != 2:
+            raise ValueError(f"drop_keys is mode 2's dropout; mode is {mode}")
+        if not (keys.is_cuda and keys.device == torch.device(f"cuda:{self.device}") and keys.dtype == torch.int64
+                and tuple(keys.shape) == (B, 2) and keys.is_contiguous()):
+            raise ValueError(f"drop_keys must be a contiguous int64 tensor of shape ({B}, 2) on cuda:{self.device}")
 
     def make_graph(self, wav, out, mode=0, lens=None, ws=None):
         """Captures the whole restore() launch sequence (~360 kernels) for the given device buffers into a
