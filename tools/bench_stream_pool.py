@@ -1,4 +1,5 @@
-"""Many live streams through one StreamPool against one restore_stream generator per stream, mode 0, synthetic weights.
+"""Many live streams through one StreamPool against one restore_stream generator per stream, synthetic weights, in each
+mode of --mode (0, 1 or 2, one session; in mode 2 stream i has dropout seed i in the pool and in its generator).
 Each stream is a seeded synthetic utterance of --seconds at 44.1 kHz, fed in --block-second blocks, restored in chunks
 of --chunk seconds with --ctx seconds of context on each side.  Two pools run: a host pool (numpy blocks in and out)
 and a device pool (the same blocks as CUDA tensors in and out, no host staging and no wait in a step).
@@ -20,8 +21,9 @@ and a device pool (the same blocks as CUDA tensors in and out, no host staging a
       copy-back, cutting), from the summed wall time of the steps and CUDA events around each replay inside them.
       For the device pool the step time is the device time between CUDA events recorded before and after each step.
 
-Prints the card's name, power limit and maximum SM clock, then one JSON line.  Usage:
-  python tools/bench_stream_pool.py [--streams 1,8,32,64,128] [--rt-streams 8,32,64,128,192,256] [--seconds 20]"""
+Prints the card's name, power limit and maximum SM clock, then one JSON line with the results of each mode.  Usage:
+  python tools/bench_stream_pool.py [--streams 1,8,32,64,128] [--rt-streams 8,32,64,128,192,256] [--seconds 20]
+                                    [--mode 0,1,2]"""
 import argparse
 import json
 import os
@@ -72,6 +74,11 @@ def warm(pool, device=False):
     assert pool.graph_count == len(pool.buckets)
 
 
+def seed_of(pool, i):
+    """Stream i's dropout seed: i in mode 2, none otherwise."""
+    return i if pool.mode == 2 else None
+
+
 def run_pool(pool, streams, block, timed_steps=None, device=False):
     """(a) for the pool: returns ([output per stream], wall seconds).  device: push CUDA tensors (the streams are
     uploaded before the clock starts) and time to a device synchronise; timed_steps then gets (bucket, start event, end
@@ -82,7 +89,7 @@ def run_pool(pool, streams, block, timed_steps=None, device=False):
     blocks = [blocks_of(x, block) for x in streams]
     got = [[] for _ in streams]
     t0 = time.perf_counter()
-    sids = [pool.open() for _ in streams]
+    sids = [pool.open(dropout_seed=seed_of(pool, i)) for i in range(len(streams))]
     index = {sid: i for i, sid in enumerate(sids)}
 
     def step():
@@ -119,10 +126,11 @@ def run_pool(pool, streams, block, timed_steps=None, device=False):
     return [np.concatenate(g) for g in got], wall
 
 
-def run_round_robin(vf, streams, block, args):
+def run_round_robin(vf, streams, block, args, mode):
     """(a) for N restore_stream generators driven round-robin, one window each in turn."""
-    gens = [vf.restore_stream(iter(blocks_of(x, block)), chunk_seconds=args.chunk, context_seconds=args.ctx)
-            for x in streams]
+    gens = [vf.restore_stream(iter(blocks_of(x, block)), chunk_seconds=args.chunk, context_seconds=args.ctx, mode=mode,
+                              dropout_seed=i if mode == 2 else None)
+            for i, x in enumerate(streams)]
     got = [[] for _ in streams]
     t0 = time.perf_counter()
     live = list(range(len(gens)))
@@ -172,7 +180,7 @@ def run_real_time(pool, streams, block, args, rng, device=False):
         streams = [torch.from_numpy(x).cuda() for x in streams]
     blocks = [blocks_of(x, block) for x in streams]
     start = rng.uniform(0, args.chunk, size=len(streams))
-    sids = [pool.open() for _ in streams]
+    sids = [pool.open(dropout_seed=seed_of(pool, i)) for i in range(len(streams))]
     index = {sid: i for i, sid in enumerate(sids)}
     next_k = [0] * len(streams)
     due = deque()                                   # arrival time of the push that made each pending window due
@@ -227,38 +235,15 @@ def run_real_time(pool, streams, block, args, rng, device=False):
             "first_audio_s_p50": float(np.median(first)), "keeps_real_time": bool(lags.max() < args.chunk)}
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--streams", default="1,8,32,64,128")
-    ap.add_argument("--rt-streams", default="8,32,64,128,192,256")
-    ap.add_argument("--seconds", type=float, default=20.0)
-    ap.add_argument("--block-seconds", type=float, default=0.1)
-    ap.add_argument("--chunk", type=float, default=1.0)
-    ap.add_argument("--ctx", type=float, default=0.5)
-    ap.add_argument("--max-windows", type=int, default=None)
-    ap.add_argument("--precision", default="tf32")
-    ap.add_argument("--seed", type=int, default=0)
-    args = ap.parse_args()
-    from voicefixer_b200 import synthetic
-    from voicefixer_b200.api import VoiceFixer
-    from voicefixer_b200.engine import Engine
-
-    info = gpu_info()
-    print("gpu:", info, flush=True)
-    eng = Engine(synthetic.make_analysis_state(0), synthetic.make_vocoder_state(1), precision=args.precision)
-    vf = VoiceFixer.from_engine(eng)
-    block = int(round(args.block_seconds * SR))
-    counts = [int(v) for v in args.streams.split(",") if v]
-    rt_counts = [int(v) for v in args.rt_streams.split(",") if v]
-    streams = utterances(max(counts + rt_counts), args.seconds, args.seed)
-
-    # one pool of each kind for every run: its graphs are captured once, in the warm-up (as is restore_stream's workspace)
-    pool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows)
-    print(f"pool: window {pool.window_len} samples, buckets {pool.buckets}", flush=True)
+def run_mode(vf, mode, args, streams, block, counts, rt_counts):
+    """(a), (b) and (c) in one mode: a host and a device pool, captured once in the warm-up (as is restore_stream's
+    workspace), against N restore_stream generators."""
+    pool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows, mode=mode)
+    print(f"mode {mode}: pool window {pool.window_len} samples, buckets {pool.buckets}", flush=True)
     warm(pool)
-    dpool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows)
+    dpool = vf.stream_pool(args.chunk, args.ctx, max_windows=args.max_windows, mode=mode)
     warm(dpool, device=True)
-    list(vf.restore_stream(blocks_of(streams[0][:3 * SR], block), args.chunk, args.ctx))
+    list(vf.restore_stream(blocks_of(streams[0][:3 * SR], block), args.chunk, args.ctx, mode=mode))
 
     table_a, host, dev_share = [], None, None
     for n in counts:
@@ -268,7 +253,7 @@ def main():
         pool_out, pool_s = run_pool(pool, streams[:n], block, timed_steps=steps)
         dev_out, dev_s = run_pool(dpool, streams[:n], block, timed_steps=dsteps, device=True)
         torch.cuda.synchronize()
-        rr_out, rr_s = run_round_robin(vf, streams[:n], block, args)
+        rr_out, rr_s = run_round_robin(vf, streams[:n], block, args, mode)
         same = all(a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
                    for a, b in zip(pool_out, rr_out))
         assert same, f"N = {n}: the pool's output differs from restore_stream's"
@@ -276,7 +261,7 @@ def main():
                        for a, b in zip(dev_out, pool_out))
         assert dev_same, f"N = {n}: the device pool's output differs from the host pool's"
         audio_s = sum(len(y) for y in pool_out) / SR
-        row = {"streams": n, "audio_s": audio_s, "pool_audio_s_per_s": audio_s / pool_s,
+        row = {"mode": mode, "streams": n, "audio_s": audio_s, "pool_audio_s_per_s": audio_s / pool_s,
                "device_pool_audio_s_per_s": audio_s / dev_s, "round_robin_audio_s_per_s": audio_s / rr_s,
                "pool_s": pool_s, "device_pool_s": dev_s, "round_robin_s": rr_s, "steps": len(steps),
                "bit_identical": same and dev_same}
@@ -305,13 +290,46 @@ def main():
         for n in rt_counts:
             row = run_real_time(p, streams[:n], block, args, rng, device=kind == "device")
             table_b[kind].append(row)
-            print(json.dumps({"pool": kind, **row}), flush=True)
+            print(json.dumps({"mode": mode, "pool": kind, **row}), flush=True)
         assert p.graph_count == len(p.buckets)      # nothing was captured after the warm-up
     largest = {kind: max([r["streams"] for r in rows if r["keeps_real_time"]], default=0)
                for kind, rows in table_b.items()}
+    return {"throughput": table_a, "real_time": table_b, "largest_real_time_streams": largest, "host_share": host,
+            "device_pool_share": dev_share}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--streams", default="1,8,32,64,128")
+    ap.add_argument("--rt-streams", default="8,32,64,128,192,256")
+    ap.add_argument("--seconds", type=float, default=20.0)
+    ap.add_argument("--block-seconds", type=float, default=0.1)
+    ap.add_argument("--chunk", type=float, default=1.0)
+    ap.add_argument("--ctx", type=float, default=0.5)
+    ap.add_argument("--max-windows", type=int, default=None)
+    ap.add_argument("--precision", default="tf32")
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--mode", default="0", help="comma-separated modes from 0, 1, 2, run one after the other")
+    args = ap.parse_args()
+    modes = [int(v) for v in args.mode.split(",") if v]
+    if not modes or any(m not in (0, 1, 2) for m in modes):
+        ap.error(f"--mode takes modes from 0, 1, 2; got {args.mode!r}")
+    from voicefixer_b200 import synthetic
+    from voicefixer_b200.api import VoiceFixer
+    from voicefixer_b200.engine import Engine
+
+    info = gpu_info()
+    print("gpu:", info, flush=True)
+    eng = Engine(synthetic.make_analysis_state(0), synthetic.make_vocoder_state(1), precision=args.precision)
+    vf = VoiceFixer.from_engine(eng)
+    block = int(round(args.block_seconds * SR))
+    counts = [int(v) for v in args.streams.split(",") if v]
+    rt_counts = [int(v) for v in args.rt_streams.split(",") if v]
+    streams = utterances(max(counts + rt_counts), args.seconds, args.seed)
+
+    results = {m: run_mode(vf, m, args, streams, block, counts, rt_counts) for m in modes}
     print(json.dumps({"gpu": info, "precision": args.precision, "seconds": args.seconds, "block_s": args.block_seconds,
-                      "chunk_s": args.chunk, "ctx_s": args.ctx, "throughput": table_a, "real_time": table_b,
-                      "largest_real_time_streams": largest, "host_share": host, "device_pool_share": dev_share}))
+                      "chunk_s": args.chunk, "ctx_s": args.ctx, "modes": results}))
 
 
 if __name__ == "__main__":

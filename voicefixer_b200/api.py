@@ -235,55 +235,88 @@ def stream_rows(rows):
     return gather, emit
 
 
-_STREAM_SHORT = "restore_stream: fewer than 1025 samples in total; the front end reflect-pads 1024"
-
-
 class StreamSchedule:
-    """The window rule of VoiceFixer.restore_stream and StreamPool, in samples at 44.1 kHz.  Each chunk of `chunk`
-    samples is restored inside the window [pos - ctx, pos + chunk + ctx), clipped to the stream, as soon as that window has
-    arrived; at the end of the stream the last windows are flushed without (full) look-ahead.  Only the chunk itself is
-    kept from each window."""
+    """The window rule of VoiceFixer.restore_stream and StreamPool in `mode`, in samples at 44.1 kHz.  Each chunk of
+    `chunk` samples is restored inside the window [pos - ctx, pos + chunk + ctx), clipped to the stream, as soon as that
+    window has arrived; at the end of the stream the last windows are flushed without (full) look-ahead.  Only the chunk
+    itself is kept from each window.  No window is shorter than min_len, the shortest window the mode can restore, or
+    longer than capacity.
 
-    def __init__(self, chunk, ctx):
-        self.chunk, self.ctx = int(chunk), int(ctx)
-        # the longest window due() returns: chunk + 2 ctx for a full window; a flush window shorter than 1025 samples is
-        # widened to 1025 + ctx; with ctx = 0 a flush window may take in a tail of up to 1024 samples after its chunk
+    Mode 1's pre-filter keeps the first 512 * (n // 512) samples of a window of n (as restore_inmem keeps them of each
+    30 s segment, voicefixer/base.py:121-122), so a window [lo, hi) emits only the kept samples below
+    lo + 512 * ((hi - lo) // 512); pos still moves past the lost ones.  With ctx >= 511 no sample is lost but the
+    stream's last (hi - lo) % 512 <= 511 (a flush window that reaches the stream's end keeps everything up to it); with
+    ctx = 0 every window loses its last (hi - lo) % 512 samples, as the 30 s segments do."""
+
+    # the shortest window of each mode: the front end reflect-pads 1024 (base.py:78); mode 1's pre-filter keeps
+    # 512 * (L // 512) samples, which must exceed 1024 (plan_many); mode 2 needs 1 + L // 441 > 64 frames (_MODE2_MSG)
+    MIN_LEN = {0: 1025, 1: 1536, 2: 64 * 441}
+    _WHY = {0: "the front end reflect-pads 1024",
+            1: "mode 1's pre-filter keeps 512 * (L // 512) samples of L and the front end reflect-pads 1024",
+            2: "mode 2's train-mode statistics need more than 64 frames (1 + L // 441 > 64)"}
+
+    def __init__(self, chunk, ctx, mode=0):
+        if mode not in (0, 1, 2):
+            raise ValueError("mode must be 0, 1 or 2")
+        self.chunk, self.ctx, self.mode = int(chunk), int(ctx), mode
+        self.min_len = m = self.MIN_LEN[mode]
+        # the longest window due() returns: chunk + 2 ctx for a full window; a flush window shorter than min_len samples
+        # is widened to min_len + ctx; with ctx = 0 a flush window may take in a tail of up to min_len - 1 samples after
+        # its chunk
         if self.ctx == 0:
-            self.capacity = max(self.chunk + 1024, 1025)
+            self.capacity = max(self.chunk + m - 1, m)
         else:
-            self.capacity = max(self.chunk + 2 * self.ctx, 1025 + self.ctx)
+            self.capacity = max(self.chunk + 2 * self.ctx, m + self.ctx)
+
+    def check_first_window(self, who):
+        """Raises ValueError `<who>: ...` when a stream's first window, chunk + ctx samples, is shorter than min_len."""
+        if self.chunk + self.ctx < self.min_len:
+            raise ValueError(f"{who}: chunk_seconds + context_seconds is {self.chunk + self.ctx} samples, the length of "
+                             f"a stream's first window; {self._WHY[self.mode]}, so it needs at least {self.min_len}")
 
     def due(self, pos, avail, ended):
         """([(lo, hi, keep_lo, keep_hi), ...], new pos): the windows that are due once samples [0, avail) of the stream
         have arrived (and nothing more will, if `ended`) and every sample before `pos` has been scheduled.  Window
-        [lo, hi) is restored whole and its samples [keep_lo, keep_hi) are emitted; the new pos follows the last of them.
-        Raises RuntimeError, restore_stream's message, when an ended stream leaves a flush window that cannot reach 1025
-        samples (the front end reflect-pads 1024)."""
-        chunk, ctx = self.chunk, self.ctx
+        [lo, hi) is restored whole and its samples [keep_lo, keep_hi) are emitted; the new pos follows the last of them
+        (in mode 1 also the samples the pre-filter dropped).  Raises RuntimeError, restore_stream's message, when an
+        ended stream leaves a flush window that cannot reach min_len samples."""
+        chunk, ctx, m = self.chunk, self.ctx, self.min_len
         windows = []
         while avail >= pos + chunk + ctx:                                # a full chunk plus its look-ahead has arrived
-            windows.append((max(0, pos - ctx), pos + chunk + ctx, pos, pos + chunk))
+            lo, hi = max(0, pos - ctx), pos + chunk + ctx
+            windows.append((lo, hi, pos, self._kept(lo, hi, pos, pos + chunk)))
             pos += chunk
         while ended and pos < avail:                                     # flush: the last windows have no (full) look-ahead
             hi = min(avail, pos + chunk + ctx)
             keep_hi = min(avail, pos + chunk)
-            if avail - keep_hi <= 1024 and avail - keep_hi > 0 and ctx == 0:  # never leave a tail the front end cannot pad
+            if 0 < avail - keep_hi < m and ctx == 0:                     # never leave a tail too short to restore
                 keep_hi = hi = avail
+            if self.mode == 1 and hi == avail:       # the next window would re-read this one's end: lose nothing mid-stream
+                keep_hi = avail
             lo = max(0, pos - ctx)
-            if hi - lo <= 1024:                                          # reflect padding needs > 1024 samples (base.py:78)
-                lo = max(0, hi - 1025 - ctx)
-                if hi - lo <= 1024:
-                    raise RuntimeError(_STREAM_SHORT)
-            windows.append((lo, hi, pos, keep_hi))
+            if hi - lo < m:                                              # e.g. reflect padding needs > 1024 (base.py:78)
+                lo = max(0, hi - m - ctx)
+                if hi - lo < m:
+                    raise RuntimeError(f"restore_stream: fewer than {m} samples in total; {self._WHY[self.mode]}")
+            windows.append((lo, hi, pos, self._kept(lo, hi, pos, keep_hi)))
             pos = keep_hi
         return windows, pos
 
+    def _kept(self, lo, hi, keep_lo, keep_hi):
+        """keep_hi, clipped in mode 1 to the samples the pre-filter keeps of the window [lo, hi)."""
+        if self.mode != 1:
+            return keep_hi
+        return max(keep_lo, min(keep_hi, lo + 512 * ((hi - lo) // 512)))
+
 
 class _Stream:
-    """One stream of a StreamPool: its recent input at its own rate and where its schedule stands."""
+    """One stream of a StreamPool: its recent input at its own rate, where its schedule stands, and in mode 2 its dropout
+    seed; window k of the stream (counting from 0) draws its masks from key (seed, k)."""
 
-    def __init__(self, rate):
+    def __init__(self, rate, seed=None):
         self.rate = rate
+        self.seed = seed
+        self.restored = 0                          # windows restored so far: the index of the oldest pending one
         self._data = np.zeros(0, dtype=np.float32)  # buf = _data[_lo:_hi], grown by doubling: a push copies its block once
         self._lo = self._hi = 0
         self.base = 0                              # buf holds input samples [base, n) at `rate`
@@ -320,8 +353,8 @@ class _DevStream(_Stream):
     of down, so the held input is a recording of its own to the resampler (stream_rows), and at most down - 1 samples
     more than _Stream's are held."""
 
-    def __init__(self, rate, device):
-        super().__init__(rate)
+    def __init__(self, rate, device, seed=None):
+        super().__init__(rate, seed)
         self.down = resample.ratio(rate)[1]
         self._data = torch.empty(0, device=device)
 
@@ -373,26 +406,34 @@ class StreamPool:
     synchronises the device once.  Each stream's device blocks are bit-identical, block by block, to the host pool's
     for the same audio and the same calls, at every rate and precision.  Calls on several CUDA streams run in the order
     they were made (Engine._shared_stream), and a stream buffer a pool replaces or forgets is not reused before the
-    work that reads it is done."""
+    work that reads it is done.
 
-    def __init__(self, engine, chunk_seconds=2.0, context_seconds=1.0, max_windows=None, device=None):
+    mode (0, 1 or 2, for the pool's lifetime): restore_stream's mode.  In mode 1 each bucket's graph runs the ragged
+    pre-filter and then the restore (restore_many's pair); in mode 2 a restore with train-mode statistics and seeded
+    dropout, window k of a stream keyed (the stream's dropout_seed, k) whatever step or bucket it runs in and whatever
+    the other streams do.  The keys go to the device from pinned memory without a host wait, so a device step is still
+    two library launches and one replay."""
+
+    def __init__(self, engine, chunk_seconds=2.0, context_seconds=1.0, max_windows=None, device=None, mode=0):
         chunk = int(round(chunk_seconds * 44100))
         ctx = int(round(context_seconds * 44100))
         if chunk <= 0 or ctx < 0:
             raise ValueError("chunk_seconds must be positive and context_seconds non-negative")
-        if chunk + ctx <= 1024:
-            raise ValueError(f"stream_pool: chunk_seconds + context_seconds is {chunk + ctx} samples, the length of a "
-                             "stream's first window; the front end reflect-pads 1024, so it needs at least 1025")
+        self._sched = StreamSchedule(chunk, ctx, mode)
+        self._sched.check_first_window("stream_pool")
         if max_windows is not None and (isinstance(max_windows, (bool, np.bool_))
                                         or not isinstance(max_windows, numbers.Integral) or max_windows < 1):
             raise ValueError(f"stream_pool: max_windows is {max_windows!r}; give a positive integer or None")
+        self.mode = mode
         self._eng = engine
         self._dev = device or f"cuda:{engine.device}"
         self._cuda = torch.device(self._dev).type == "cuda"
-        self._sched = StreamSchedule(chunk, ctx)
         self.window_len = L = self._sched.capacity
-        # a row of input and of output per window, and the resampler's output row (its staged input is smaller)
-        fit = engine.max_batch(L, extra_per_item=4 * 3 * L)
+        # a row of input and of output per window, and the resampler's output row (its staged input is smaller); in
+        # mode 1 also the pre-filter's, twice its output row: each bucket's graph holds rows of its own, and the buckets
+        # (powers of two up to max_windows, and max_windows) hold fewer than two rows per window in all
+        extra = 4 * 3 * L + (prefilter_bytes(engine, L) + 4 * L if mode == 1 else 0)
+        fit = engine.max_batch(L, extra_per_item=extra)
         self.max_windows = fit if max_windows is None else min(int(max_windows), fit)
         self.buckets = sorted({1 << k for k in range(self.max_windows.bit_length())} | {self.max_windows})
         self._streams = {}
@@ -403,12 +444,17 @@ class StreamPool:
         self._kind = None                          # "host" or "device": fixed by the first block pushed
 
     # ------------------------------------------------------------------ the caller's side
-    def open(self, sample_rate=44100):
-        """Starts a stream whose blocks come at sample_rate Hz; returns its id."""
+    def open(self, sample_rate=44100, dropout_seed=None):
+        """Starts a stream whose blocks come at sample_rate Hz; returns its id.  dropout_seed (mode 2): an int in
+        [0, 2^64) whose masks the stream's windows draw, as restore_stream(mode=2, dropout_seed=...) draws them; without
+        it one is drawn from torch's CPU generator (torch.manual_seed controls it).  A bad rate or seed, or a seed in
+        another mode, raises ValueError naming the stream, and uses up no id."""
         sid = self._next_sid
-        rate = resample.check_rate(sample_rate, f"stream_pool.open: stream {sid}")
+        who = f"stream_pool.open: stream {sid}"
+        rate = resample.check_rate(sample_rate, who)
+        seed = stream_dropout_seed(self.mode, dropout_seed, who)
         self._next_sid += 1
-        self._streams[sid] = _DevStream(rate, self._dev) if self._kind == "device" else _Stream(rate)
+        self._streams[sid] = _DevStream(rate, self._dev, seed) if self._kind == "device" else _Stream(rate, seed)
         return sid
 
     def push(self, sid, block):
@@ -465,6 +511,7 @@ class StreamPool:
             for (sid, _), y in zip(batch, blocks):
                 out.setdefault(sid, []).append(y)
                 self._streams[sid].pending.popleft()
+                self._streams[sid].restored += 1
         for sid in [sid for sid, s in self._streams.items() if s.closed and not s.pending]:
             self._forget(sid)
         for sid in out:
@@ -514,7 +561,7 @@ class StreamPool:
         """Makes this a device pool; its streams, opened before any block was pushed, hold no input yet."""
         for sid, s in self._streams.items():
             assert s.n == 0 and not s.pending
-            d = _DevStream(s.rate, self._dev)
+            d = _DevStream(s.rate, self._dev, s.seed)
             d.closed = s.closed
             self._streams[sid] = d
         self._kind = "device"
@@ -535,8 +582,8 @@ class StreamPool:
 
     def _trim(self, s):
         """Drops input that no window of s will read again: before its oldest pending window, and before the lowest
-        start a later window can have (a short flush window is widened by up to 1025 samples before pos - ctx)."""
-        keep = max(0, s.pos - self._sched.ctx - 1025)
+        start a later window can have (a short flush window is widened by up to min_len samples before pos - ctx)."""
+        keep = max(0, s.pos - self._sched.ctx - self._sched.min_len)
         if s.pending:
             keep = min(keep, s.pending[0][0])
         first, stop = resample.window(s.n, s.rate, keep, keep + 1)
@@ -554,13 +601,41 @@ class StreamPool:
         if self._bufs is None:
             B, L, dev = self.max_windows, self.window_len, self._dev
             pin = (lambda t: t.pin_memory()) if self._cuda else (lambda t: t)
+            ws = self._eng.graph_workspace_bytes(B, L, 1) if self.mode == 1 else self._eng.workspace_bytes(B, L)
             self._bufs = {"dev_in": torch.zeros((B, L), device=dev), "dev_out": torch.empty((B, L), device=dev),
                           "dev_lens": torch.empty(B, dtype=torch.int32, device=dev),
-                          "ws": torch.empty(self._eng.workspace_bytes(B, L), dtype=torch.uint8, device=dev)}
+                          "ws": torch.empty(ws, dtype=torch.uint8, device=dev)}
+            if self.mode == 2:                     # the windows' dropout keys, read by every bucket's graph
+                self._bufs["dev_keys"] = torch.zeros((B, 2), dtype=torch.int64, device=dev)
             if self._kind != "device":             # a device pool stages nothing on the host
                 self._bufs.update({"host_in": pin(torch.zeros((B, L))), "host_out": pin(torch.empty((B, L))),
                                    "host_lens": pin(torch.empty(B, dtype=torch.int32))})
         return self._bufs
+
+    def _graph(self, B):
+        """The restore graph of bucket B, captured on first use (once its lengths and keys are in place: the capture's
+        warm-up runs read them)."""
+        if B not in self._graphs:
+            p = self._bufs
+            keys = {"drop_keys": p["dev_keys"][:B]} if self.mode == 2 else {}
+            self._graphs[B] = self._eng.make_graph(p["dev_in"][:B], p["dev_out"][:B], mode=self.mode,
+                                                   lens=p["dev_lens"][:B], ws=p["ws"], **keys)
+        return self._graphs[B]
+
+    def _put_keys(self, batch, B):
+        """Mode 2: fills rows [0, B) of the key buffer, row k with window k's (stream seed, window index), unused rows
+        with (0, 0), from pinned memory with a stream-ordered copy (a fresh pinned buffer per step: the host does not
+        wait for the previous step's copy)."""
+        if self.mode != 2:
+            return
+        rows = np.zeros((B, 2), dtype=np.uint64)
+        seen = {}
+        for k, (sid, _) in enumerate(batch):
+            s = self._streams[sid]
+            seen[sid] = j = seen.get(sid, s.restored - 1) + 1
+            rows[k] = (s.seed, j)
+        keys = torch.from_numpy(rows.view(np.int64))
+        self._bufs["dev_keys"][:B].copy_(keys.pin_memory() if self._cuda else keys, non_blocking=True)
 
     def _run(self, batch):
         """Restores the windows of batch [(sid, (lo, hi, keep_lo, keep_hi)), ...] and returns the output rows (host)."""
@@ -568,7 +643,7 @@ class StreamPool:
         n, B = len(batch), self.bucket(len(batch))
         streams = [self._streams[sid] for sid, _ in batch]
         lens = p["host_lens"]
-        lens[:B] = 1025                            # unused rows: any valid length; their output is never read
+        lens[:B] = self._sched.min_len             # unused rows: any valid length; their output is never read
         lens[:n] = torch.tensor([hi - lo for _, (lo, hi, _, _) in batch], dtype=torch.int32)
         if any(s.rate != resample.RATE for s in streams):
             x, lens_dev = self._eng.resample(*_stage([s.buf for s in streams], [s.rate for s in streams],
@@ -583,10 +658,8 @@ class StreamPool:
                 hin[k, :hi - lo] = s.buf[lo - s.base:hi - s.base]
             p["dev_in"][:n].copy_(p["host_in"][:n], non_blocking=True)
             p["dev_lens"][:B].copy_(lens[:B], non_blocking=True)
-        if B not in self._graphs:                  # captured once the lengths are staged: its warm-up runs read them
-            self._graphs[B] = self._eng.make_graph(p["dev_in"][:B], p["dev_out"][:B], mode=0, lens=p["dev_lens"][:B],
-                                                   ws=p["ws"])
-        self._graphs[B].replay()
+        self._put_keys(batch, B)
+        self._graph(B).replay()
         p["host_out"][:n].copy_(p["dev_out"][:n], non_blocking=True)
         if self._cuda:
             torch.cuda.current_stream().synchronize()
@@ -602,11 +675,9 @@ class StreamPool:
         gather, emit = stream_rows([(s.rate, s.base, s.n, w) for s, (_, w) in zip(streams, batch)])
         self._eng.resample_src([(s.buf, s.rate, y_first, y_len) for s, (_, y_first, y_len) in zip(streams, gather)],
                                self.window_len, y=p["dev_in"][:n], lens=p["dev_lens"][:n])
-        p["dev_lens"][n:B].fill_(1025)             # unused rows: any valid length; their output is never read
-        if B not in self._graphs:                  # captured once the lengths are in place: its warm-up runs read them
-            self._graphs[B] = self._eng.make_graph(p["dev_in"][:B], p["dev_out"][:B], mode=0, lens=p["dev_lens"][:B],
-                                                   ws=p["ws"])
-        self._graphs[B].replay()
+        p["dev_lens"][n:B].fill_(self._sched.min_len)  # unused rows: any valid length; their output is never read
+        self._put_keys(batch, B)
+        self._graph(B).replay()
         blocks = [torch.empty(m, device=self._dev) for _, m in emit]
         self._eng.scatter_rows(p["dev_out"][:n], [(y, 0, m, off) for y, (off, m) in zip(blocks, emit)])
         return blocks
@@ -827,6 +898,25 @@ def check_seeded(mode, drop_masks_fn, what):
         raise ValueError(f"{what}: give dropout_seed or drop_masks_fn, not both")
 
 
+def stream_dropout_seed(mode, dropout_seed, who):
+    """The dropout seed of one stream (restore_stream, StreamPool.open): dropout_seed checked (check_seeded,
+    check_dropout_seed), or in mode 2 without one a 64-bit seed drawn from torch's CPU generator, so that
+    torch.manual_seed controls it as it controls restore_inmem's default masks; None outside mode 2."""
+    if dropout_seed is not None:
+        check_seeded(mode, None, who)
+        return check_dropout_seed(dropout_seed, who)
+    if mode != 2:
+        return None
+    lo, hi = (int(v) for v in torch.randint(0, 1 << 32, (2,), dtype=torch.int64))
+    return hi << 32 | lo
+
+
+def prefilter_bytes(eng, L):
+    """Device bytes per item that mode 1's pre-filter adds alongside a restore of items of (at most) L samples: its
+    workspace's growth per item and its (L,) float32 output row."""
+    return eng.hf_cut_workspace_bytes(2, L) - eng.hf_cut_workspace_bytes(1, L) + 4 * L
+
+
 def drop_key_rows(segs, seeds):
     """The seeded dropout keys of a batch (vfx_drop_key): segs = [(recording, a, b), ...] (plan_many's segments, a the
     first sample of a 30 s segment), seeds one per recording -> uint64 (B, 2) rows (seed of the recording, a // SEG_LENGTH):
@@ -1043,7 +1133,7 @@ class VoiceFixer:
         def max_items(L_cap):
             extra = 0 if on_dev else _staging_extra(L_cap, rates)
             if mode == 1:     # the pre-filter's workspace and its (B, L_cap) output live alongside the restore
-                extra += eng.hf_cut_workspace_bytes(2, L_cap) - eng.hf_cut_workspace_bytes(1, L_cap) + 4 * L_cap
+                extra += prefilter_bytes(eng, L_cap)
             return eng.max_batch(L_cap, extra_per_item=extra)
 
         lengths = [resample.out_len(a.shape[0], r) for a, r in zip(items, rates)]
@@ -1169,9 +1259,9 @@ class VoiceFixer:
 
     # ------------------------------------------------------------------ streaming entry point (extension, SURVEY 8f-3)
     @torch.no_grad()
-    def restore_stream(self, blocks, chunk_seconds=2.0, context_seconds=1.0, cuda=True):
-        """Low-latency form of restore_inmem (mode 0) for audio that arrives in blocks: a generator that takes an iterable
-        of 1-D float32 blocks of any sizes (44.1 kHz mono) and yields restored blocks as soon as they can be computed.
+    def restore_stream(self, blocks, chunk_seconds=2.0, context_seconds=1.0, cuda=True, mode=0, dropout_seed=None):
+        """Low-latency form of restore_inmem for audio that arrives in blocks: a generator that takes an iterable of 1-D
+        float32 blocks of any sizes (44.1 kHz mono) and yields restored blocks as soon as they can be computed.
 
         The reference has no streaming path: it cuts a recording into hard 30 s segments whose BiGRU and UNet see the whole
         segment (voicefixer/base.py:116-138).  Here every emitted chunk of `chunk_seconds` is restored inside a window that
@@ -1181,22 +1271,43 @@ class VoiceFixer:
         `workloads.stream`).  With chunk_seconds = 30 and context_seconds = 0 the windows ARE the reference's segments
         and the concatenated output equals restore_inmem's exactly; smaller windows trade fidelity to whole-segment
         processing for latency (how much depends on the trained weights' context dependence; it cannot be pinned with
-        the synthetic checkpoints available offline, DESIGN.md 7).  The total output length equals the input length."""
+        the synthetic checkpoints available offline, DESIGN.md 7).  The total output length equals the input length in
+        modes 0 and 2.
+
+        mode: restore_inmem's mode, run per window as its eager B = 1 calls.  Mode 1 runs the pre-filter and then the
+        restore on each window and emits only the samples the pre-filter keeps (StreamSchedule): with context_seconds
+        of at least 511 samples only the stream's last <= 511 samples are lost, as restore_inmem loses them of a
+        recording shorter than 30 s; with no context each chunk loses chunk % 512, as restore_inmem's segments do.
+        Mode 2 restores each window with train-mode statistics and seeded dropout: window k (counting from 0) draws its
+        masks from (dropout_seed, k) on the GPU, so with 30 s chunks and no context the output is bit-identical to
+        restore_inmem(mode=2, dropout_seed=dropout_seed).  dropout_seed: an int in [0, 2^64), mode 2 only; without one,
+        one is drawn from torch's CPU generator when the generator starts (torch.manual_seed controls it).  The shortest
+        window a mode restores (StreamSchedule.min_len) is 1025 samples in mode 0, 1536 in mode 1 and 28 224 (more than
+        64 frames) in mode 2: chunk_seconds + context_seconds must reach it, and so must the whole stream."""
         _check_cuda(cuda)
         chunk = int(round(chunk_seconds * 44100))
         ctx = int(round(context_seconds * 44100))
         if chunk <= 0 or ctx < 0:
             raise ValueError("chunk_seconds must be positive and context_seconds non-negative")
+        sched = StreamSchedule(chunk, ctx, mode)
+        sched.check_first_window("restore_stream")
+        seed = stream_dropout_seed(mode, dropout_seed, "restore_stream")
         eng = self._engine
         dev = f"cuda:{eng.device}"
-        sched = StreamSchedule(chunk, ctx)
         buf = np.zeros(0, dtype=np.float32)       # samples [base, base + len(buf)) of the stream
         base = 0                                  # stream index of buf[0]
         pos = 0                                   # next sample to emit
+        k = 0                                     # windows restored so far
 
         def run(lo, hi, keep_lo, keep_hi):
             x = torch.from_numpy(np.ascontiguousarray(buf[lo - base: hi - base]))[None].to(dev)
-            y = eng.restore(x, mode=0)
+            if mode == 1:                                                # restore_inmem's calls
+                x, _ = eng.hf_cut(x)
+                y = eng.restore(x, mode=0)
+            elif mode == 2:
+                y = eng.restore(x, mode=2, drop_keys=_upload_keys(np.array([(seed, k)], dtype=np.uint64), dev))
+            else:
+                y = eng.restore(x, mode=0)
             return y[0, keep_lo - lo: keep_hi - lo].cpu().numpy()
 
         for block in blocks:
@@ -1205,23 +1316,28 @@ class VoiceFixer:
             windows, pos = sched.due(pos, base + len(buf), ended=False)
             for w in windows:
                 yield run(*w)
-            drop = max(0, pos - ctx) - base                              # audio older than the next window's left context
+                k += 1
+            # audio no later window reads: before the next window's left context, less the widening of a short flush
+            # window (StreamPool._trim's bound)
+            drop = max(0, pos - ctx - sched.min_len) - base
             if drop > 0:
                 buf, base = buf[drop:], base + drop
         windows, pos = sched.due(pos, base + len(buf), ended=True)
         for w in windows:
             yield run(*w)
+            k += 1
 
-    def stream_pool(self, chunk_seconds=2.0, context_seconds=1.0, max_windows=None):
+    def stream_pool(self, chunk_seconds=2.0, context_seconds=1.0, max_windows=None, mode=0):
         """Extension: restore_stream for many live streams at once (StreamPool).  open() a stream per caller, push() its
         blocks as they arrive, close() it at its end, and call step() to restore every window that is due, of every
         stream, in one ragged CUDA-graph replay.  Each stream's output is bit-identical to restore_stream on that
-        stream's audio alone with the same chunk_seconds / context_seconds.  max_windows: the most windows one step
-        restores (default: as many as fit the device memory that is free, at most 64).  Blocks may be host arrays, or
-        1-D float32 CUDA tensors (any element stride), which the pool restores where they are and returns as new CUDA
-        tensors without waiting for the GPU (StreamPool: the first block pushed fixes which)."""
+        stream's audio alone with the same chunk_seconds / context_seconds / mode (and in mode 2 the dropout_seed given
+        to open()).  max_windows: the most windows one step restores (default: as many as fit the device memory that is
+        free, at most 64).  Blocks may be host arrays, or 1-D float32 CUDA tensors (any element stride), which the pool
+        restores where they are and returns as new CUDA tensors without waiting for the GPU (StreamPool: the first block
+        pushed fixes which)."""
         _check_cuda(False)
-        return StreamPool(self._engine, chunk_seconds, context_seconds, max_windows)
+        return StreamPool(self._engine, chunk_seconds, context_seconds, max_windows, mode=mode)
 
     def restore(self, input, output, cuda=False, mode=0, your_vocoder_func=None):
         wav_10k = self._load_wav(input, sample_rate=44100)               # base.py:141-146

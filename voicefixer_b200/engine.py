@@ -349,34 +349,61 @@ class Engine(_WorkspaceQueries):
                 and tuple(keys.shape) == (B, 2) and keys.is_contiguous()):
             raise ValueError(f"drop_keys must be a contiguous int64 tensor of shape ({B}, 2) on cuda:{self.device}")
 
-    def make_graph(self, wav, out, mode=0, lens=None, ws=None):
+    def make_graph(self, wav, out, mode=0, lens=None, ws=None, drop_keys=None):
         """Captures the whole restore() launch sequence (~360 kernels) for the given device buffers into a
         CUDA graph; returns an object whose .replay() re-runs it (inputs are read from `wav`, results land in
         `out`).  Shapes, buffers and the workspace are frozen into the graph.  With `lens` (ragged batch) the graph
         reads the lengths from that buffer at every replay: refill it, like `wav`, before replay().
 
-        ws (optional): a uint8 device workspace of at least workspace_bytes(*wav.shape) bytes for the graph to use, e.g.
-        one that several graphs share because they never replay at the same time; without it the graph gets its own."""
+        ws (optional): a uint8 device workspace of at least graph_workspace_bytes(*wav.shape, mode) bytes for the graph to
+        use, e.g. one that several graphs share because they never replay at the same time; without it the graph gets
+        its own.
+
+        mode 1 (needs lens): the graph runs restore_many's pair, the ragged pre-filter (hf_cut) into a (B, L) row buffer
+        and lengths of the graph's own, then restore(mode=0) on them: row b of `out` holds item b's 512 * (lens[b] // 512)
+        restored samples, then zeros.  Both use `ws`, one after the other.  drop_keys (mode 2, optional): seeded dropout
+        (restore()), a contiguous int64 (B, 2) CUDA buffer read at every replay, like lens."""
         assert wav.is_cuda and out.is_cuda and wav.shape == out.shape
+        B, L = wav.shape
+        mid = mid_lens = None
+        if mode == 1:
+            if lens is None:
+                raise ValueError("make_graph: mode 1 runs the ragged pre-filter, which needs lens")
+            mid = torch.empty_like(wav)
+            mid_lens = torch.empty(B, dtype=torch.int32, device=wav.device)
         # the graph bakes raw device pointers in: it gets its OWN workspace unless given one, and the returned object keeps
         # every buffer it touches alive (a later, larger call may replace the engine's shared workspace)
-        need = self.workspace_bytes(*wav.shape)
+        need = self.graph_workspace_bytes(B, L, mode)
         if ws is None:
             ws = torch.empty(need, dtype=torch.uint8, device=wav.device)
         elif not (ws.is_cuda and ws.dtype == torch.uint8 and ws.numel() >= need):
             raise ValueError(f"make_graph: ws must be a uint8 CUDA tensor of at least {need} bytes")
+
+        def run():
+            if mode == 1:
+                self.hf_cut(wav, lens=lens, out=mid, lens_out=mid_lens, ws=ws)
+                self.restore(mid, mode=0, out=out, ws=ws, lens=mid_lens)
+            else:
+                self.restore(wav, mode=mode, out=out, ws=ws, lens=lens, drop_keys=drop_keys)
+
         side = torch.cuda.Stream(device=wav.device)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                                # warm-up: one-time attribute / table setup
             for _ in range(2):
-                self.restore(wav, mode=mode, out=out, ws=ws, lens=lens)
+                run()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            self.restore(wav, mode=mode, out=out, ws=ws, lens=lens)
-        g._keep = (ws, wav, out, lens, self.arena)
+            run()
+        g._keep = (ws, wav, out, lens, mid, mid_lens, drop_keys, self.arena)
         return g
+
+    def graph_workspace_bytes(self, B, L, mode=0):
+        """The workspace make_graph's graph uses on B items of (at most) L samples in `mode`: restore()'s, and in mode 1
+        the pre-filter's if that is larger (the two run one after the other)."""
+        need = self.workspace_bytes(B, L)
+        return max(need, self.hf_cut_workspace_bytes(B, L)) if mode == 1 else need
 
     @staticmethod
     def hf_cut_workspace_bytes(B, L):
@@ -510,25 +537,42 @@ class Engine(_WorkspaceQueries):
         _lib.check(self.lib.vfx_scatter_rows(_ptr(x), B, x.stride(0), table, _ptr(ws), ws.numel(), _stream()),
                    "vfx_scatter_rows")
 
-    def hf_cut(self, wav, ratio=0.95, lens=None):
+    def hf_cut(self, wav, ratio=0.95, lens=None, out=None, lens_out=None, ws=None):
         """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
 
         lens (ragged batch): int32 device tensor (B,); item b is the first lens[b] samples of row b and is filtered as if
         alone.  Returns (out (B, L), cut bins, lens_out): row b holds 512 * (lens[b] // 512) samples, then zeros, and
-        lens_out (int32 device tensor) holds those lengths, ready for restore(..., lens=lens_out)."""
+        lens_out (int32 device tensor) holds those lengths, ready for restore(..., lens=lens_out).
+
+        out, lens_out (ragged batch only), ws (optional): caller-owned buffers to write the result, the lengths and the
+        intermediate spectra into, instead of new ones and the engine's shared workspace (e.g. inside a captured graph,
+        which must not bake in a workspace a later call may replace): a contiguous float32 CUDA tensor of the result's
+        shape, a contiguous (B,) int32 CUDA tensor, and a uint8 CUDA tensor of at least hf_cut_workspace_bytes(B, L)."""
         wav = self._dev(wav)
         B, L = wav.shape
         cut = torch.empty(B, dtype=torch.int32, device=wav.device)
-        ws = self._workspace(self.hf_cut_workspace_bytes(B, L))
+        if ws is None:
+            ws = self._workspace(self.hf_cut_workspace_bytes(B, L))
+        elif not (ws.is_cuda and ws.dtype == torch.uint8 and ws.numel() >= self.hf_cut_workspace_bytes(B, L)):
+            raise ValueError(f"hf_cut: ws must be a uint8 CUDA tensor of at least {self.hf_cut_workspace_bytes(B, L)} bytes")
+        shape = (B, L) if lens is not None else (B, 512 * (L // 512))
+        if out is None:
+            out = torch.empty(shape, device=wav.device)
+        elif not (out.is_cuda and out.device == wav.device and out.dtype == torch.float32 and out.is_contiguous()
+                  and tuple(out.shape) == shape):
+            raise ValueError(f"hf_cut: out must be a contiguous float32 tensor of shape {shape} on {wav.device}")
         if lens is not None:
             _check_lens(lens, B)
-            out = torch.empty(B, L, device=wav.device)
-            lens_out = torch.empty(B, dtype=torch.int32, device=wav.device)
+            if lens_out is None:
+                lens_out = torch.empty(B, dtype=torch.int32, device=wav.device)
+            else:
+                _check_lens(lens_out, B)
             _lib.check(self.lib.vfx_hf_cut_ragged(self.h, _ptr(wav), B, L, _ptr(lens), float(ratio), _ptr(out),
                                                   _ptr(lens_out), _ptr(cut), _ptr(ws), ws.numel(), _stream()),
                        "vfx_hf_cut_ragged")
             return out, cut, lens_out
-        out = torch.empty(B, 512 * (L // 512), device=wav.device)
+        if lens_out is not None:
+            raise ValueError("hf_cut: lens_out is the ragged batch's output lengths; it needs lens")
         _lib.check(self.lib.vfx_hf_cut(self.h, _ptr(wav), B, L, float(ratio), _ptr(out), _ptr(cut), _ptr(ws), ws.numel(),
                                        _stream()), "vfx_hf_cut")
         return out, cut
