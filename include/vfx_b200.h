@@ -80,6 +80,10 @@ unsigned long long vfx_launch_count(void);
 /* How many of them were tensor-core convolutions whose operands were staged by TMA (launches without per-item extents
  * whose operands a tensor map can express, DESIGN.md §4.1); the others were staged with cp.async. */
 unsigned long long vfx_conv_tma_launch_count(void);
+/* How many of those TMA-fed launches also loaded their residual and stored their outputs through tensor maps (the
+ * others -- a residual or output base not 16-byte aligned, or a stride not a multiple of 16 bytes -- ran the row-loop
+ * epilogue, DESIGN.md §4.1). */
+unsigned long long vfx_conv_tma_store_launch_count(void);
 /* With option "profile" = 1 every launch group is bracketed by CUDA events on the call's stream;
  * this synchronises, writes one line per tag "tag count total_ms flops bytes" and clears the log. */
 int vfx_profile_report(vfx_engine* e, char* buf, size_t cap);

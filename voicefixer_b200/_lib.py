@@ -71,6 +71,7 @@ SIGNATURES = {
     "vfx_engine_finalize": (_i, [_vp]),
     "vfx_launch_count": (_c.c_ulonglong, []),
     "vfx_conv_tma_launch_count": (_c.c_ulonglong, []),
+    "vfx_conv_tma_store_launch_count": (_c.c_ulonglong, []),
     "vfx_profile_report": (_i, [_vp, _c.c_char_p, _sz]),
     "vfx_workspace_bytes": (_sz, [_vp, _i, _i]),
     "vfx_workspace_bytes_frames": (_sz, [_vp, _i, _i]),

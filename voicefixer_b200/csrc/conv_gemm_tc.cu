@@ -19,20 +19,27 @@
 //      operands whose strides or weight offsets the maps do not take (tma_plan).
 //  - Two consumer warpgroups (224 registers), 64 rows each: one m64nBN wgmma group in flight per warpgroup, into one of
 //    two partial accumulators, while the previous slice's partial is added to the fp32 accumulator.
-//  - Staged epilogue: the tile goes through a shared fp32 buffer and is processed row by row (bias, fp32 residual,
-//    eval-BN affine, activation, operand for the next layer), with 16-byte accesses where the host found every pointer,
-//    stride and column offset aligned.  A thread's column parameters are read once per tile and all its residual rows
-//    are loaded before its first store, so a tile waits on global memory once, not once per row.
+//  - Epilogue, in one of two forms chosen on the host (tma_store_plan), each element in the same order: bias, fp32
+//    residual, raw output, eval-BN affine, activation, operand for the next layer.
+//      TMA store (TMA launches whose residual and outputs tensor maps can express): the producer thread loads the tile's
+//      residual into the dense, swizzled epilogue buffer during the K loop, as soon as the previous tile's stores have
+//      read it; the consumers combine their accumulator fragments with it in registers, write each output into the
+//      buffer and one thread stores it with TMA stores, which run while the next tile's K loop does.  The maps' clipping
+//      drops what the launch does not store.  Raw and operand outputs share the buffer: the operand is written once the
+//      raw output's stores have read it.
+//      Row loop (the others): the tile goes through a padded shared fp32 buffer and is processed row by row, with 16-byte
+//      accesses where the host found every pointer, stride and column offset aligned.  A thread's column parameters are
+//      read once per tile and all its residual rows are loaded before its first store.
 // kind tf32 reads fp32 operands and ignores their low 13 mantissa bits: producers round tf32 operands to nearest, and the
 // encoded stream of vfx_conv_desc.res_enc / raw_enc is read as round-to-nearest(lrelu(x)) by construction.
 // Ragged batches (seq_in / seq_out): each item's extent on the sequence axis acts as that item's own edge, so every row
 // inside it is computed from the same operands as with the item alone; a tile none of whose rows is stored is skipped.
 //
 // What still stands between this kernel and the roof: the A halo of the taps is re-read from L2 for every tap, every
-// CTA reads its own copy of the weights from L2, the ring is 4 stages deep at BN = 128 (the fp32 epilogue buffer takes
-// the rest of shared memory), the per-slice sum costs BN / 2 FADDs per slice in the consumers, and the epilogue runs
-// after the K loop with the tensor cores idle: its residual loads are issued together but only once the K loop is done,
-// and its stores do not overlap the next tile's wgmma.
+// CTA reads its own copy of the weights from L2, the ring is 5 stages deep at BN = 128 (the fp32 epilogue buffer takes
+// the rest of shared memory), the per-slice sum costs BN / 2 FADDs per slice in the consumers, and the consumers still
+// spend the epilogue's arithmetic and shared-memory passes with the tensor cores idle (one buffer: a launch with both a
+// raw and an operand output also waits for the raw stores to read it).
 #include "tc_ptx.cuh"
 #include "wgmma_ptx.cuh"
 
@@ -57,23 +64,37 @@ struct OutRow { long long raw, act, res; int ok; };
 // (qw, qh, b) at a multiple of the box: a whole number of lines, or a piece of one line, of one item, or whole items,
 // so that its input rows are one box of the input tensor.  Tile row r is position (r % tw, r / tw % th, r / (tw th));
 // rows from tw th tb on do not exist (their shared memory is not written and their results are not stored).
+// With the TMA-store epilogue (tma_store_plan) the residual and the outputs have maps of their own over the output grid
+// (N, Wq', Hq', B), Wq' / Hq' the positions q with q s + r inside OW / OH: the tile's boxes at (n0, w0, h0, b0) are then
+// its rows, and the maps' clipping drops the rows and columns the row-loop epilogue does not store.
 struct TmaPlan {
   CUtensorMap a;           // input  (Cin, W, H, B),    box (128 bytes, tw, th, tb)
   CUtensorMap w;           // weights (Cin, N, groups), box (128 bytes, BN, 1): tap t is group wtap[t]
+  CUtensorMap r, o, oa;    // residual, raw and operand output, box (128 bytes or BN columns, tw, th, tb)
   int tw, th, tb;
   int ntw, nth, mtiles;    // boxes per line, per item's lines, in all
   int wtap[9];
 };
 
-template <int BN, bool TMA> struct Cfg {
+// The staged tile of the TMA-store epilogue: column boxes of ob = min(BN * esz, 128) bytes by BM rows, dense, each in the
+// swizzle of its map (16-byte chunk c of row r at c ^ (r & 7) in 128-byte rows, c ^ (r / 2 & 3) in 64-byte ones).
+// Byte offset of column c of row r in elements of esz bytes:
+template <int BN, int ESZ> __device__ __forceinline__ uint32_t st_offset(int r, int c) {
+  constexpr int OB = BN * ESZ < 128 ? BN * ESZ : 128, CPB = OB / ESZ;
+  const uint32_t o = (uint32_t)(r * OB + c % CPB * ESZ);
+  return (uint32_t)(c / CPB * (BM * OB)) + (o ^ ((o >> 7) & (OB / 16 - 1)) << 4);
+}
+
+// TST: the TMA-store epilogue (TMA producer only); without it, the row-loop epilogue and its row table
+template <int BN, bool TMA, bool TST> struct Cfg {
   static constexpr int STAGE = A_BYTES + BN * 128;
-  static constexpr int EPI_LD = BN + 8;            // fp32 words per epilogue row; +8 keeps the fragment stores conflict-free
+  static constexpr int EPI_LD = TST ? BN : BN + 8; // fp32 words per epilogue row; +8 keeps the fragment stores conflict-free
   static constexpr int EPI = BM * EPI_LD * 4;
   static constexpr int PROWS = TMA ? 0 : BM * 24;  // the cp.async producer's row table
-  static constexpr int ROWS = PROWS + BM * (int)sizeof(OutRow);     // + the epilogue's
+  static constexpr int ROWS = TST ? 16 : PROWS + BM * (int)sizeof(OutRow);   // + the epilogue's (TST: its two mbarriers)
   static constexpr int FIXED = 1024 + EPI + ROWS;  // + 1024: alignment of the ring
   static constexpr int FIT = (SMEM_MAX - FIXED) / (STAGE + 16);
-  static constexpr int STAGES = FIT < 8 ? FIT : 8;                  // 4 at BN = 128, 7 at 64, 8 at 32
+  static constexpr int STAGES = FIT < 8 ? FIT : 8;                  // 4 at BN = 128 (TST: 5), 7 at 64, 8 at 32
   // cp.async: the producer signals slice k full after issuing slice k + AHEAD (cp.async.wait_group AHEAD).  It must wait
   // for an empty slot before issuing, and the consumers free slot k - 1 only once slice k is full, so AHEAD <= STAGES - 2:
   // with more, the producer waits for a slot the consumers can only free after a signal it has not sent yet.
@@ -81,7 +102,7 @@ template <int BN, bool TMA> struct Cfg {
   // that thread may block on the empty barrier of the oldest stage with every other stage in flight.
   static constexpr int AHEAD = STAGES - 2;
   static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
-  static_assert(STAGES >= 3 && SMEM <= SMEM_MAX, "conv_gemm_tc: shared-memory plan");
+  static_assert(STAGES >= (TST ? 5 : 3) && SMEM <= SMEM_MAX, "conv_gemm_tc: shared-memory plan");
 };
 
 // output-grid row m -> item b and grid position (qh, qw); false beyond the problem (M < 2^31: 32-bit divisions)
@@ -126,13 +147,15 @@ __device__ __forceinline__ float act_out(const vfx_conv_desc& d, float v, float 
 // TMA: the operands arrive through the tensor maps of `tp` and the M tiles are its boxes; otherwise through cp.async
 // with 128 consecutive rows of the flattened output grid per M tile, `tp` unused, and the per-item extents
 // (seq_in / seq_out) honoured where the descriptor carries them.
-// vec: every output / residual pointer, stride and column offset allows 4-column vector accesses.
-template <int BN, int KIND, bool TMA>
+// vec: every output / residual pointer, stride and column offset allows 4-column vector accesses (row-loop epilogue).
+// TST: the tile leaves through TMA stores of tp.o / tp.oa, and its residual arrives through tp.r during its K loop.
+template <int BN, int KIND, bool TMA, bool TST>
 __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_constant__ vfx_conv_desc d,
                                                                  const __grid_constant__ TmaPlan tp, const int nkc,
                                                                  const int vec) {
+  static_assert(TMA || !TST, "conv_gemm_tc: the TMA-store epilogue needs the TMA producer's tile boxes");
   using T = typename OpT<KIND>::T;
-  using C = Cfg<BN, TMA>;
+  using C = Cfg<BN, TMA, TST>;
   constexpr bool SEQ = !TMA;
   constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
   constexpr int S = C::STAGES, STAGE = C::STAGE, AHEAD = C::AHEAD;
@@ -142,8 +165,11 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
   float* const epi = reinterpret_cast<float*>(gbase + S * STAGE);
   int4* const prow = reinterpret_cast<int4*>(gbase + S * STAGE + C::EPI);        // (cp.async producer only)
   long long* const pbase = reinterpret_cast<long long*>(prow + BM);
-  OutRow* const crow = reinterpret_cast<OutRow*>(gbase + S * STAGE + C::EPI + C::PROWS);
+  OutRow* const crow = reinterpret_cast<OutRow*>(gbase + S * STAGE + C::EPI + C::PROWS);   // (row-loop epilogue only)
   const uint32_t full0 = sbase + S * STAGE + C::EPI + C::ROWS, empty0 = full0 + 8 * S;
+  // TMA-store epilogue: the staged tile, and its two mbarriers (full: the buffer is free and the tile's residual has
+  // landed; empty: the stores of the tile before have read the buffer)
+  const uint32_t epi_s = sbase + S * STAGE, efull = epi_s + C::EPI, eempty = efull + 8;
 
   const int tid = threadIdx.x;
   if (tid == 0) {
@@ -152,6 +178,10 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       // after its own copies of the stage have landed
       mbar_init(full0 + 8 * s, TMA ? 1 : 128);
       mbar_init(empty0 + 8 * s, 8);     // every consumer warp, after its wgmma group has read the stage
+    }
+    if (TST) {
+      mbar_init(efull, 1);              // the producer thread's arrival (with the residual's bytes)
+      mbar_init(eempty, 1);             // the consumer thread that issues the stores
     }
   }
   __syncthreads();
@@ -169,12 +199,26 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
     if constexpr (TMA) {
       if (tid != 0) return;
       const uint32_t bytes = (uint32_t)(tp.tw * tp.th * tp.tb * 128 + BN * 128);   // of one stage: whole boxes, zeros included
+      const uint32_t rbytes = d.residual ? (uint32_t)(tp.tw * tp.th * tp.tb * BN * 4) : 0u;   // of a tile's residual
+      // TST: tile i's residual goes into the epilogue buffer once the stores of tile i - 1 have read it.  That is signalled
+      // after the consumers' slice min(2, slices - 1) of tile i, so the wait comes after slice S >= 5 of the tile has been
+      // issued (or after its last): by then slices 0 to 3 are in the ring, and the ring stays full up to that point.
+      const int rl = niter < S ? niter : S;
+      auto epi_load = [&](int i, int n0, int w0, int h0, int b0) {
+        if (i > 0) mbar_wait(eempty, (i - 1) & 1);
+        if (!rbytes) { mbar_arrive(efull); return; }
+        mbar_expect_tx(efull, rbytes);
+#pragma unroll
+        for (int bx = 0; bx < BN / 32; ++bx) tma_load_4d(epi_s + bx * BM * 128, &tp.r, efull, n0 + 32 * bx, w0, h0, b0);
+      };
       uint32_t k = 0;                                 // K slices issued by this CTA
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      int i = 0;                                      // tiles begun by this CTA
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++i) {
         const int mt = t / ntn, u = mt / tp.ntw;
         const int n0 = t % ntn * BN;
         const int w0 = mt % tp.ntw * tp.tw, h0 = u % tp.nth * tp.th, b0 = u / tp.nth * tp.tb;
         for (int it = 0; it < niter; ++it, ++k) {
+          if (TST && it == rl) epi_load(i, n0, w0, h0, b0);
           const int s = k % S;
           if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
           const int tap = it / nkc;
@@ -184,6 +228,7 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
           tma_load_4d(sa, &tp.a, full, c, w0 + d.dw[tap], h0 + d.dh[tap], b0);
           tma_load_3d(sa + A_BYTES, &tp.w, full, c, n0, tp.wtap[tap]);
         }
+        if (TST && rl == niter) epi_load(i, n0, w0, h0, b0);
       }
       return;
     }
@@ -274,16 +319,25 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
   };
   // slice kk's group has completed: free its stage and add it.  Summing the K slices here rounds to nearest, so the
   // error of long reductions (9 taps x 768 channels) does not build up as a bias.
+  uint32_t k = 0;                                     // K slices consumed by this CTA
+  int ti = 0;                                         // tiles begun by this CTA
+  const uint32_t rel = niter > 3 ? 2 : niter - 1;     // (the producer waits for it after slice S > rel + 1)
   auto retire = [&](float (&p)[BN / 2], uint32_t kk) {
     wgmma_fence_operand(p);                           // the reads of p below stay after the wgmma_wait that precedes
     __syncwarp();
     if (l == 0) mbar_arrive(empty0 + 8 * (kk % S));
+    // TST: after the tile's slice `rel`, the thread that issued the previous tile's stores hands the buffer back to the
+    // producer once they have read it, early enough for the residual load to hide behind the rest of the K loop and late
+    // enough for the stores to have read it (waiting stalls that thread's warpgroup)
+    if (TST && ct == 0 && kk == k + rel && ti > 0) {
+      bulk_wait_read<0>();
+      mbar_arrive(eempty);
+    }
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] += p[i];
   };
 
-  uint32_t k = 0;                                     // K slices consumed by this CTA
-  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++ti) {
     const int mt = t / ntn;
     const int n0 = t % ntn * BN;
     if (skips) {
@@ -318,6 +372,107 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
 
     // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is
     //      row cw*64 + w*16 + l/4 + 8h, column 8j + 2(l%4) + e
+    if constexpr (TST) {
+      // Each thread combines its own fragments with bias and the staged residual, in registers, then writes each output
+      // into the buffer in its map's layout; one thread stores the boxes.  The element order is the row-loop epilogue's.
+      const int u = mt / tp.ntw;
+      const int w0 = mt % tp.ntw * tp.tw, h0 = u % tp.nth * tp.th, b0 = u / tp.nth * tp.tb;
+      const int rq = cw * 64 + w * 16 + (l >> 2);
+      uint8_t* const eb = reinterpret_cast<uint8_t*>(epi);
+      mbar_wait(efull, ti & 1);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * (l & 3);
+        float bv[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int n = n0 + c + e;                   // columns from N on are clipped by the stores
+          bv[e] = d.bias && n < d.N ? d.bias[n < d.bias_mod ? n : n % d.bias_mod] : 0.f;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* const v = acc + 4 * j + 2 * h;
+          const float2 rv = d.residual ? *reinterpret_cast<const float2*>(eb + st_offset<BN, 4>(rq + 8 * h, c)) : make_float2(0.f, 0.f);
+          v[0] = add_in(d, v[0], bv[0], rv.x);
+          v[1] = add_in(d, v[1], bv[1], rv.y);
+        }
+      }
+      // the buffer's generic writes -> the async proxy, then one thread stores its column boxes of ob bytes (cpb columns)
+      auto store = [&](const CUtensorMap* map, int ob, int cpb) {
+        fence_proxy_async();
+        named_sync(2, 256);
+        if (ct == 0) {
+          for (int bx = 0; bx < BN / cpb; ++bx) tma_store_4d(map, epi_s + bx * BM * ob, n0 + bx * cpb, w0, h0, b0);
+          bulk_commit();
+        }
+      };
+      // fragment pair q = 2 j + h of this thread: its fp32 slot in the buffer (the residual's and the raw output's layout)
+      auto slot = [&](int q) { return eb + st_offset<BN, 4>(rq + 8 * (q & 1), 8 * (q >> 1) + 2 * (l & 3)); };
+      if (d.out_raw) {
+#pragma unroll
+        for (int q = 0; q < BN / 4; ++q)
+          *reinterpret_cast<float2*>(slot(q)) = make_float2(raw_out(d, acc[2 * q]), raw_out(d, acc[2 * q + 1]));
+        store(&tp.o, 128, 32);
+      }
+      if (out_act) {
+        // one buffer: the operand overwrites the raw output once its stores have read it
+        if (d.out_raw) {
+          if (ct == 0) bulk_wait_read<0>();
+          named_sync(2, 256);
+        }
+        // Leaky ReLU (or none) is applied in registers.  The other activations run as a loop over the thread's own slots
+        // (unrolled, their code per element overflows the instruction cache).  A tf32 operand goes into the slot, a
+        // 16-bit pair into the slot's first word.
+        const bool cheap = d.act == VFX_ACT_LRELU || d.act == VFX_ACT_NONE;
+        if (cheap) {
+#pragma unroll
+          for (int q = 0; q < BN / 4; ++q) {
+            const int n = n0 + 8 * (q >> 1) + 2 * (l & 3);
+            const bool in0 = d.act_scale && n < d.N, in1 = d.act_scale && n + 1 < d.N;
+            float y0 = d.act_scale ? fmaf(acc[2 * q], in0 ? d.act_scale[n] : 1.f, in0 ? d.act_shift[n] : 0.f) : acc[2 * q];
+            float y1 = d.act_scale ? fmaf(acc[2 * q + 1], in1 ? d.act_scale[n + 1] : 1.f, in1 ? d.act_shift[n + 1] : 0.f) : acc[2 * q + 1];
+            if (d.act == VFX_ACT_LRELU) {
+              y0 = y0 > 0.f ? y0 : y0 * d.act_param;
+              y1 = y1 > 0.f ? y1 : y1 * d.act_param;
+            }
+            if (ESZ == 4)
+              *reinterpret_cast<float2*>(slot(q)) = make_float2(round_tf32(y0), round_tf32(y1));
+            else
+              *reinterpret_cast<uint32_t*>(slot(q)) = pack16<KIND == 2>(y0, y1);
+          }
+        } else {
+#pragma unroll
+          for (int q = 0; q < BN / 4; ++q) *reinterpret_cast<float2*>(slot(q)) = make_float2(acc[2 * q], acc[2 * q + 1]);
+        }
+#pragma unroll 2
+        for (int q = 0; q < (cheap ? 0 : BN / 4); ++q) {
+          const int n = n0 + 8 * (q >> 1) + 2 * (l & 3);
+          const bool in0 = d.act_scale && n < d.N, in1 = d.act_scale && n + 1 < d.N;
+          float2* const p = reinterpret_cast<float2*>(slot(q));
+          const float2 v = *p;
+          const float y0 = act_out(d, v.x, in0 ? d.act_scale[n] : 1.f, in0 ? d.act_shift[n] : 0.f);
+          const float y1 = act_out(d, v.y, in1 ? d.act_scale[n + 1] : 1.f, in1 ? d.act_shift[n + 1] : 0.f);
+          if (ESZ == 4)
+            *p = make_float2(round_tf32(y0), round_tf32(y1));
+          else
+            *reinterpret_cast<uint32_t*>(p) = pack16<KIND == 2>(y0, y1);
+        }
+        constexpr int OB = BN * ESZ < 128 ? BN * ESZ : 128;
+        if (ESZ == 2) {
+          // into the 16-bit layout, which overlaps other threads' slots: all are read before any is overwritten
+          uint32_t y[BN / 4];
+#pragma unroll
+          for (int q = 0; q < BN / 4; ++q) y[q] = *reinterpret_cast<const uint32_t*>(slot(q));
+          named_sync(2, 256);
+#pragma unroll
+          for (int q = 0; q < BN / 4; ++q)
+            *reinterpret_cast<uint32_t*>(eb + st_offset<BN, ESZ>(rq + 8 * (q & 1), 8 * (q >> 1) + 2 * (l & 3))) = y[q];
+        }
+        store(&tp.oa, OB, OB / ESZ);
+      }
+      continue;
+    }
+    named_sync(2, 256);                               // the previous tile's epilogue has finished reading epi / crow
     named_sync(2, 256);                               // the previous tile's epilogue has finished reading epi / crow
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
@@ -418,6 +573,7 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       }
     }
   }
+  if (TST && ct == 0) bulk_wait<0>();                // the last tile's stores, before the CTA's shared memory goes
 }
 
 // The tile boxes and the two tensor maps of a launch without per-item extents.  Returns 1 with `tp` filled, 0 where a
@@ -428,6 +584,12 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
 // Weights: the taps' [N][Cin] matrices start at arbitrary offsets (the ConvTranspose phase groups use some taps of a
 // larger array), so the third dimension counts in units of the greatest common divisor of the offsets' differences,
 // from the lowest offset.  Rows n >= N of a box are then zeros, not the next matrix.
+CUtensorMapDataType map_dtype(int precision) {
+  return precision == VFX_PREC_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+         : precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+
 int tma_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
   const long long esz = (long long)prec_esz(precision), LIM = 1LL << 40;          // tensor-map strides are below 2^40 bytes
   if (d.W <= 0 || d.H <= 0) return 0;
@@ -469,9 +631,7 @@ int tma_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
   // ---- encode
   const EncodeTiled encode = tensor_map_encoder();
   VFX_REQUIRE(encode, "conv_gemm_tc: this CUDA driver has no cuTensorMapEncodeTiled");
-  const CUtensorMapDataType dt = precision == VFX_PREC_TF32   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                 : precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                              : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = map_dtype(precision);
   const cuuint32_t bk = (cuuint32_t)(128 / esz), ones[4] = {1, 1, 1, 1};
   const cuuint32_t abox[4] = {bk, (cuuint32_t)tp.tw, (cuuint32_t)tp.th, (cuuint32_t)tp.tb}, wbox[3] = {bk, (cuuint32_t)bn, 1};
   CUresult r = encode(&tp.a, dt, 4, const_cast<void*>(d.a), adim, astr, abox, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -484,14 +644,61 @@ int tma_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
   return 1;
 }
 
-template <int BN, int KIND, bool TMA>
+// A map of the output grid, dimensions (N, Wq', Hq', B), over the tensor at p (elements of esz bytes from column col,
+// strides sB / sH / sW): base p + col + rh sH + rw sW, strides (sw sW, sh sH, sB), box (cols, tw, th, tb) in the 128- or
+// 64-byte swizzle of a cols * esz byte row.  Returns 1, 0 where a map cannot express it, or an error.
+int grid_map(CUtensorMap& m, CUtensorMapDataType dt, long long esz, const void* p, int col, long long sB, long long sH,
+             long long sW, int cols, const vfx_conv_desc& d, const TmaPlan& tp) {
+  const long long LIM = 1LL << 40;
+  const int wq = d.Wq < ceil_div(d.OW - d.rw, d.sw) ? d.Wq : ceil_div(d.OW - d.rw, d.sw);
+  const int hq = d.Hq < ceil_div(d.OH - d.rh, d.sh) ? d.Hq : ceil_div(d.OH - d.rh, d.sh);
+  if (wq <= 0 || hq <= 0) return 0;                 // nothing is stored (the row-loop epilogue tests each row)
+  const char* base = static_cast<const char*>(p) + (col + d.rh * sH + d.rw * sW) * esz;
+  if ((uintptr_t)base & 15) return 0;
+  const cuuint64_t dim[4] = {(cuuint64_t)d.N, (cuuint64_t)wq, (cuuint64_t)hq, (cuuint64_t)d.B};
+  const long long src[3] = {d.sw * sW, d.sh * sH, sB};
+  cuuint64_t str[3];
+  long long dense = d.N * esz;
+  for (int i = 0; i < 3; ++i) {
+    const long long s = dim[i + 1] > 1 ? src[i] * esz : dense;
+    if (s <= 0 || s >= LIM || s % 16) return 0;
+    str[i] = (cuuint64_t)s;
+    dense = s < LIM / (long long)dim[i + 1] ? s * (long long)dim[i + 1] : LIM;
+  }
+  const cuuint32_t box[4] = {(cuuint32_t)cols, (cuuint32_t)tp.tw, (cuuint32_t)tp.th, (cuuint32_t)tp.tb}, ones[4] = {1, 1, 1, 1};
+  const EncodeTiled encode = tensor_map_encoder();
+  VFX_REQUIRE(encode, "conv_gemm_tc: this CUDA driver has no cuTensorMapEncodeTiled");
+  const CUresult r = encode(&m, dt, 4, const_cast<char*>(base), dim, str, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            cols * esz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  VFX_REQUIRE(r == CUDA_SUCCESS, "conv_gemm_tc: output-grid tensor map refused (CUresult %d)", (int)r);
+  return 1;
+}
+
+// The residual and output maps of the TMA-store epilogue, for a launch tma_plan has planned.  Returns 1 with them in
+// `tp`, 0 where one of them cannot be expressed (a base not 16-byte aligned, such as an odd column, or a stride not a
+// multiple of 16 bytes: the launch keeps the row-loop epilogue), or an error.
+int tma_store_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
+  const long long esz = (long long)prec_esz(precision);
+  const int acols = bn * esz < 128 ? bn : (int)(128 / esz);      // operand columns per 128-byte (or BN-wide) box
+  int ok = 1;
+  if (d.residual)
+    ok = grid_map(tp.r, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.residual, d.r_col, d.r_sB, d.r_sH, d.r_sW, 32, d, tp);
+  if (d.out_raw && ok == 1)
+    ok = grid_map(tp.o, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out_raw, d.o_col, d.o_sB, d.o_sH, d.o_sW, 32, d, tp);
+  if (d.out_act && ok == 1)
+    ok = grid_map(tp.oa, map_dtype(precision), esz, d.out_act, d.oa_col, d.oa_sB, d.oa_sH, d.oa_sW, acols, d, tp);
+  return ok;
+}
+
+template <int BN, int KIND, bool TMA, bool TST>
 int launch(const vfx_conv_desc& d, const TmaPlan& tp, int vec, cudaStream_t st) {
-  constexpr int smem = Cfg<BN, TMA>::SMEM;
+  constexpr int smem = Cfg<BN, TMA, TST>::SMEM;
   static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
   int dev = 0;
   VFX_CUDA_CHECK(cudaGetDevice(&dev));
   if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, TMA, TST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     if (dev < 64) attr_set |= 1ull << dev;
   }
   const int sms = sm_count(dev);
@@ -501,20 +708,25 @@ int launch(const vfx_conv_desc& d, const TmaPlan& tp, int vec, cudaStream_t st) 
   const long long tiles = mtiles * ceil_div(d.N, BN);
   const int grid = (int)(tiles < sms ? tiles : sms);
   if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
-  conv_gemm_wgmma_kernel<BN, KIND, TMA><<<grid, NT, smem, st>>>(d, tp, nkc, vec);
+  conv_gemm_wgmma_kernel<BN, KIND, TMA, TST><<<grid, NT, smem, st>>>(d, tp, nkc, vec);
   VFX_LAUNCH_CHECK();
   if (TMA) ++g_conv_tma_launches;
+  if (TST) ++g_conv_tma_store_launches;
   return VFX_OK;
 }
 
-// Launches without per-item extents go through TMA where tma_plan can express them.  The cp.async instantiation reads
-// the extents only where the descriptor has them, so it also runs the others.
+// Launches without per-item extents go through TMA where tma_plan can express them, and among those, the ones whose
+// residual and outputs tma_store_plan can express leave through TMA stores.  The cp.async instantiation reads the extents
+// only where the descriptor has them, so it also runs the others.
 template <int BN, int KIND>
 int launch_bn(int precision, const vfx_conv_desc& d, int vec, cudaStream_t st) {
   TmaPlan tp{};
   int tma = 0;
   if (!d.seq_in && !d.seq_out && (tma = tma_plan(precision, d, BN, tp)) < 0) return tma;
-  return tma ? launch<BN, KIND, true>(d, tp, vec, st) : launch<BN, KIND, false>(d, tp, vec, st);
+  if (!tma) return launch<BN, KIND, false, false>(d, tp, vec, st);
+  const int tst = tma_store_plan(precision, d, BN, tp);
+  if (tst < 0) return tst;
+  return tst ? launch<BN, KIND, true, true>(d, tp, vec, st) : launch<BN, KIND, true, false>(d, tp, vec, st);
 }
 
 template <int KIND>

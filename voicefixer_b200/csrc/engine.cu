@@ -24,6 +24,7 @@ void set_error(const char* fmt, ...) {
 
 unsigned long long g_launches = 0;
 unsigned long long g_conv_tma_launches = 0;
+unsigned long long g_conv_tma_store_launches = 0;
 
 struct Tensor { const void* p; size_t bytes; };
 
@@ -1050,6 +1051,7 @@ int vfx_engine_destroy(vfx_engine* e) {
 
 unsigned long long vfx_launch_count(void) { return vfx::g_launches; }
 unsigned long long vfx_conv_tma_launch_count(void) { return vfx::g_conv_tma_launches; }
+unsigned long long vfx_conv_tma_store_launch_count(void) { return vfx::g_conv_tma_store_launches; }
 
 int vfx_profile_report(vfx_engine* e, char* buf, size_t cap) {
   VFX_REQUIRE(e && buf && cap > 0, "profile_report: bad arguments");

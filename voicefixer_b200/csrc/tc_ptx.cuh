@@ -1,4 +1,4 @@
-// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu, resstack_pair.cu): TMA tile loads, cp.async operand
+// PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu, resstack_pair.cu): TMA tile loads and stores, cp.async operand
 // staging with zero fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups
 // and the shared-memory matrix descriptor; on the host, the SM count and the tensor-map encoder their launches use.
 #pragma once
@@ -48,6 +48,16 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* map, uint3
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
                ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+// TMA tile store: one thread writes a box of shared memory (in the map's swizzle) to the tensor, clipping whatever lies
+// outside it.  The writers of the box fence_proxy_async() and synchronise before it is issued; the stores of one
+// commit_group form a bulk group, and wait_read<N> returns once all but the newest N groups have read shared memory.
+__device__ __forceinline__ void tma_store_4d(const void* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // named barriers over a subset of the CTA's warps (id 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

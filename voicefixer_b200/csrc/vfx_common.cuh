@@ -24,6 +24,7 @@ void set_error(const char* fmt, ...);
 
 extern unsigned long long g_launches;   // kernels launched by this library (bench.py's gpu_launches)
 extern unsigned long long g_conv_tma_launches;   // those of them that were conv_gemm_tc launches fed by TMA
+extern unsigned long long g_conv_tma_store_launches;   // ... and of those, the ones whose epilogue stored through TMA
 #define VFX_LAUNCH_CHECK()                                                            \
   do { ++vfx::g_launches; VFX_CUDA_CHECK(cudaGetLastError()); } while (0)
 
