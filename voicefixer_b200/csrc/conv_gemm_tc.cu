@@ -3,22 +3,18 @@
 //
 //   out[b, oh, ow, n] = bias[n % bias_mod] + residual + sum_{tap} sum_{c} W[tap][n][c] * A[b, qh+dh, qw+dw, c]
 //
-// Persistent, warp-specialised kernel: grid = min(tiles, SMs), each CTA walks a static stride over the 128 x BN output
-// tiles in N-fastest order (the N tiles of one M tile run together, so their A rows come from HBM about once).
-//  - Producer: for every K slice (tap, 128-byte channel slice) the shifted input rows and the tap's weight rows go into
-//    a ring of 128-byte-swizzled K-major tiles; whatever lies outside the input (convolution padding), beyond Cin or
-//    beyond N arrives as zeros, so any tap offset, stride and edge is handled without a separate padded tensor.  Stages
-//    are handed over through full / empty mbarriers; the ring is filled for the next tile while the consumers run the
-//    epilogue.  Two forms (TMA below):
-//      TMA: one thread issues two tensor-map loads per slice, a box of the [B][H][W][Cin] input at the tile's origin plus
-//      the tap's offset and a box of the weights; the out-of-bounds fill of the maps supplies the zeros and the loads
-//      themselves complete the stage's full barrier.  A box is a rectangle of one tensor, so an M tile is a rectangle of
-//      the output grid (TmaPlan) and not 128 consecutive rows of the flattened one.
-//      cp.async: the producer warpgroup (56 registers) stages 16-byte chunks with zero-fill copies from a per-tile row
-//      table.  It serves the launches a tensor map cannot express: ragged batches, whose zeros depend on the item, and
-//      operands whose strides or weight offsets the maps do not take (tma_plan).
-//  - Two consumer warpgroups (224 registers), 64 rows each: one m64nBN wgmma group in flight per warpgroup, into one of
-//    two partial accumulators, while the previous slice's partial is added to the fp32 accumulator.
+// Persistent, warp-specialised kernel on the pipeline of tc_pipeline.cuh (ring, feed and K loop): grid = min(tiles,
+// SMs), each CTA walks a static stride over the 128 x BN output tiles in N-fastest order (the N tiles of one M tile run
+// together, so their A rows come from HBM about once).
+//  - Producer: the K slices are (tap, 128-byte channel slice), tap outer; a slice is the shifted input rows and the tap's
+//    weight rows.  Whatever lies outside the input (convolution padding), beyond Cin or beyond N arrives as zeros, so any
+//    tap offset, stride and edge is handled without a separate padded tensor.  Two forms (TMA below):
+//      TMA: two tensor-map loads per slice, a box of the [B][H][W][Cin] input at the tile's origin plus the tap's offset
+//      and a box of the weights; the out-of-bounds fill of the maps supplies the zeros.  A box is a rectangle of one
+//      tensor, so an M tile is a rectangle of the output grid (TmaPlan) and not 128 consecutive rows of the flattened one.
+//      cp.async: zero-fill copies from a per-tile row table.  It serves the launches a tensor map cannot express: ragged
+//      batches, whose zeros depend on the item, and operands whose strides or weight offsets the maps do not take
+//      (tma_plan).
 //  - Epilogue, in one of two forms chosen on the host (tma_store_plan), each element in the same order: bias, fp32
 //    residual, raw output, eval-BN affine, activation, operand for the next layer.
 //      TMA store (TMA launches whose residual and outputs tensor maps can express): the producer thread loads the tile's
@@ -40,22 +36,11 @@
 // the rest of shared memory), the per-slice sum costs BN / 2 FADDs per slice in the consumers, and the consumers still
 // spend the epilogue's arithmetic and shared-memory passes with the tensor cores idle (one buffer: a launch with both a
 // raw and an operand output also waits for the raw stores to read it).
-#include "tc_ptx.cuh"
-#include "wgmma_ptx.cuh"
+#include "tc_pipeline.cuh"
 
 namespace vfx {
 
 namespace {
-
-constexpr int BM = 128, NT = 384;                  // warpgroup 0 produces, warpgroups 1 and 2 consume
-constexpr int A_BYTES = BM * 128;
-constexpr int SMEM_MAX = 227 * 1024;               // dynamic shared memory of one sm_90 CTA
-constexpr int PROD_REGS = 56, CONS_REGS = 224;     // 128 x 56 + 256 x 224 <= 384 x 168 (the launch allocation)
-
-template <int KIND> struct OpT;
-template <> struct OpT<0> { using T = tf32_t; static constexpr int ESZ = 4; };
-template <> struct OpT<1> { using T = __nv_bfloat16; static constexpr int ESZ = 2; };
-template <> struct OpT<2> { using T = __half; static constexpr int ESZ = 2; };
 
 // epilogue offsets of one tile row (ok == 0: the row is not stored)
 struct OutRow { long long raw, act, res; int ok; };
@@ -85,24 +70,14 @@ template <int BN, int ESZ> __device__ __forceinline__ uint32_t st_offset(int r, 
   return (uint32_t)(c / CPB * (BM * OB)) + (o ^ ((o >> 7) & (OB / 16 - 1)) << 4);
 }
 
-// TST: the TMA-store epilogue (TMA producer only); without it, the row-loop epilogue and its row table
+// TST: the TMA-store epilogue (TMA producer only); without it, the row-loop epilogue and its row table.  Shared memory
+// beside the ring: the epilogue buffer, then the row tables (TST: the buffer's two mbarriers).
 template <int BN, bool TMA, bool TST> struct Cfg {
-  static constexpr int STAGE = A_BYTES + BN * 128;
   static constexpr int EPI_LD = TST ? BN : BN + 8; // fp32 words per epilogue row; +8 keeps the fragment stores conflict-free
   static constexpr int EPI = BM * EPI_LD * 4;
   static constexpr int PROWS = TMA ? 0 : BM * 24;  // the cp.async producer's row table
-  static constexpr int ROWS = TST ? 16 : PROWS + BM * (int)sizeof(OutRow);   // + the epilogue's (TST: its two mbarriers)
-  static constexpr int FIXED = 1024 + EPI + ROWS;  // + 1024: alignment of the ring
-  static constexpr int FIT = (SMEM_MAX - FIXED) / (STAGE + 16);
-  static constexpr int STAGES = FIT < 8 ? FIT : 8;                  // 4 at BN = 128 (TST: 5), 7 at 64, 8 at 32
-  // cp.async: the producer signals slice k full after issuing slice k + AHEAD (cp.async.wait_group AHEAD).  It must wait
-  // for an empty slot before issuing, and the consumers free slot k - 1 only once slice k is full, so AHEAD <= STAGES - 2:
-  // with more, the producer waits for a slot the consumers can only free after a signal it has not sent yet.
-  // TMA has no such rule: a slice's full barrier is completed by its loads, whatever the issuing thread does next, so
-  // that thread may block on the empty barrier of the oldest stage with every other stage in flight.
-  static constexpr int AHEAD = STAGES - 2;
-  static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
-  static_assert(STAGES >= (TST ? 5 : 3) && SMEM <= SMEM_MAX, "conv_gemm_tc: shared-memory plan");
+  static constexpr int ROWS = TST ? 16 : PROWS + BM * (int)sizeof(OutRow);   // + the epilogue's
+  using Plan = RingPlan<A_BYTES + BN * 128, EPI + ROWS, TST ? 5 : 3>;   // 4 stages at BN = 128 (TST: 5), 7 at 64, 8 at 32
 };
 
 // output-grid row m -> item b and grid position (qh, qw); false beyond the problem (M < 2^31: 32-bit divisions)
@@ -158,27 +133,21 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
   using C = Cfg<BN, TMA, TST>;
   constexpr bool SEQ = !TMA;
   constexpr int ESZ = OpT<KIND>::ESZ, AL = 16 / ESZ, BK = 128 / ESZ;   // elements per 16-byte chunk / per K slice
-  constexpr int S = C::STAGES, STAGE = C::STAGE, AHEAD = C::AHEAD;
+  constexpr int S = C::Plan::STAGES, STAGE = C::Plan::STAGE;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* const gbase = smem_raw + (sbase - smem_u32(smem_raw));
+  const Ring<typename C::Plan> ring{(smem_u32(smem_raw) + 1023u) & ~1023u};
+  uint8_t* const gbase = smem_raw + (ring.base - smem_u32(smem_raw));
   float* const epi = reinterpret_cast<float*>(gbase + S * STAGE);
   int4* const prow = reinterpret_cast<int4*>(gbase + S * STAGE + C::EPI);        // (cp.async producer only)
   long long* const pbase = reinterpret_cast<long long*>(prow + BM);
   OutRow* const crow = reinterpret_cast<OutRow*>(gbase + S * STAGE + C::EPI + C::PROWS);   // (row-loop epilogue only)
-  const uint32_t full0 = sbase + S * STAGE + C::EPI + C::ROWS, empty0 = full0 + 8 * S;
   // TMA-store epilogue: the staged tile, and its two mbarriers (full: the buffer is free and the tile's residual has
   // landed; empty: the stores of the tile before have read the buffer)
-  const uint32_t epi_s = sbase + S * STAGE, efull = epi_s + C::EPI, eempty = efull + 8;
+  const uint32_t epi_s = ring.base + S * STAGE, efull = epi_s + C::EPI, eempty = efull + 8;
 
   const int tid = threadIdx.x;
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) {
-      // full: the issuing thread's expect_tx plus the bytes of the stage's two loads (TMA), or every producer thread
-      // after its own copies of the stage have landed
-      mbar_init(full0 + 8 * s, TMA ? 1 : 128);
-      mbar_init(empty0 + 8 * s, 8);     // every consumer warp, after its wgmma group has read the stage
-    }
+    ring.init(TMA);
     if (TST) {
       mbar_init(efull, 1);              // the producer thread's arrival (with the residual's bytes)
       mbar_init(eempty, 1);             // the consumer thread that issues the stores
@@ -219,11 +188,10 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
         const int w0 = mt % tp.ntw * tp.tw, h0 = u % tp.nth * tp.th, b0 = u / tp.nth * tp.tb;
         for (int it = 0; it < niter; ++it, ++k) {
           if (TST && it == rl) epi_load(i, n0, w0, h0, b0);
-          const int s = k % S;
-          if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+          ring.acquire(k);
           const int tap = it / nkc;
           const int c = (it - tap * nkc) * BK;
-          const uint32_t sa = sbase + s * STAGE, full = full0 + 8 * s;
+          const uint32_t sa = ring.stage(k), full = ring.full(k);
           mbar_expect_tx(full, bytes);
           tma_load_4d(sa, &tp.a, full, c, w0 + d.dw[tap], h0 + d.dh[tap], b0);
           tma_load_3d(sa + A_BYTES, &tp.w, full, c, n0, tp.wtap[tap]);
@@ -260,12 +228,11 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
         named_sync(1, 128);
       }
       for (int it = 0; it < niter; ++it, ++k) {
-        const int s = k % S;
-        if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+        ring.acquire(k);
         const int tap = it / nkc;
         const int c = (it - tap * nkc) * BK + chunk * AL;
         const bool c_ok = c < d.Cin;
-        const uint32_t sa = sbase + s * STAGE, sb = sa + A_BYTES;
+        const uint32_t sa = ring.stage(k), sb = sa + A_BYTES;
         const int dh = d.dh[tap], dw = d.dw[tap];
         const long long toff = (long long)dh * d.a_sH + (long long)dw * d.a_sW + c;
 #pragma unroll
@@ -283,17 +250,10 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
           const char* src = static_cast<const char*>(d.w) + (ok ? (d.w_off[tap] + (long long)(n0 + n) * d.Cin + c) * ESZ : 0);
           cp_async16(sb + sw128_offset(n, chunk), src, ok);
         }
-        cp_async_commit();
-        if (k >= (uint32_t)AHEAD) {
-          cp_async_wait<AHEAD>();                     // this thread's chunks of slice k - AHEAD have landed
-          fence_proxy_async();                        // ... and are visible to the tensor core's (async-proxy) reads
-          mbar_arrive(full0 + 8 * ((k - AHEAD) % S));
-        }
+        ring.cp_async_handoff(k);
       }
     }
-    cp_async_wait<0>();
-    fence_proxy_async();
-    for (uint32_t j = k > (uint32_t)AHEAD ? k - AHEAD : 0; j < k; ++j) mbar_arrive(full0 + 8 * (j % S));
+    ring.cp_async_drain(k);
     return;
   }
 
@@ -303,38 +263,18 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
 #undef VFX_TILE_WALK
   const int ct = tid - 128, cw = ct >> 7, w = (ct >> 5) & 3, l = tid & 31;
   T* out_act = reinterpret_cast<T*>(d.out_act);
-  float acc[BN / 2], p0[BN / 2], p1[BN / 2];
-  // issue slice kk's 4 wgmma into p (zeroed: the tensor core's accumulator adds truncate, see retire)
-  auto issue = [&](float (&p)[BN / 2], uint32_t kk) {
-    const uint32_t s = kk % S;
-    mbar_wait(full0 + 8 * s, (kk / S) & 1);
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) p[i] = 0.f;
-    const uint32_t sa = sbase + s * STAGE;
-    const uint64_t da = sw128_desc(sa + cw * 64 * 128), db = sw128_desc(sa + A_BYTES);
-    wgmma_fence();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) Wgmma<BN, KIND>::mma(p, da + 2 * q, db + 2 * q);   // 32 bytes of K each
-    wgmma_commit();
-  };
-  // slice kk's group has completed: free its stage and add it.  Summing the K slices here rounds to nearest, so the
-  // error of long reductions (9 taps x 768 channels) does not build up as a bias.
+  float acc[BN / 2];
   uint32_t k = 0;                                     // K slices consumed by this CTA
   int ti = 0;                                         // tiles begun by this CTA
-  const uint32_t rel = niter > 3 ? 2 : niter - 1;     // (the producer waits for it after slice S > rel + 1)
-  auto retire = [&](float (&p)[BN / 2], uint32_t kk) {
-    wgmma_fence_operand(p);                           // the reads of p below stay after the wgmma_wait that precedes
-    __syncwarp();
-    if (l == 0) mbar_arrive(empty0 + 8 * (kk % S));
-    // TST: after the tile's slice `rel`, the thread that issued the previous tile's stores hands the buffer back to the
-    // producer once they have read it, early enough for the residual load to hide behind the rest of the K loop and late
-    // enough for the stores to have read it (waiting stalls that thread's warpgroup)
-    if (TST && ct == 0 && kk == k + rel && ti > 0) {
+  const int rel = niter > 3 ? 2 : niter - 1;          // (the producer waits for it after slice S > rel + 1)
+  // TST: after the tile's slice `rel`, the thread that issued the previous tile's stores hands the buffer back to the
+  // producer once they have read it, early enough for the residual load to hide behind the rest of the K loop and late
+  // enough for the stores to have read it (waiting stalls that thread's warpgroup)
+  auto released = [&](int it) {
+    if (TST && ct == 0 && it == rel && ti > 0) {
       bulk_wait_read<0>();
       mbar_arrive(eempty);
     }
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] += p[i];
   };
 
   for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++ti) {
@@ -345,29 +285,7 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       const bool live = tile_row<TMA>(d, tp, M, mt, ct & 127, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw);
       if (!named_sync_or(2, 256, live)) continue;
     }
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    // slice it goes to p[it & 1]; slice it - 1 is added while slice it is in flight
-    issue(p0, k);
-    int it = 1;
-    for (; it + 1 < niter; it += 2) {
-      issue(p1, k + it);
-      wgmma_wait<1>();
-      retire(p0, k + it - 1);
-      issue(p0, k + it + 1);
-      wgmma_wait<1>();
-      retire(p1, k + it);
-    }
-    if (it < niter) {
-      issue(p1, k + it);
-      wgmma_wait<1>();
-      retire(p0, k + it - 1);
-      wgmma_wait<0>();
-      retire(p1, k + it);
-    } else {
-      wgmma_wait<0>();
-      retire(p0, k + it - 1);
-    }
+    k_loop<BN, KIND>(ring, acc, k, niter, cw, l, [](int, uint32_t sa) { return sa; }, released);
     k += niter;
 
     // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is
@@ -472,7 +390,6 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       }
       continue;
     }
-    named_sync(2, 256);                               // the previous tile's epilogue has finished reading epi / crow
     named_sync(2, 256);                               // the previous tile's epilogue has finished reading epi / crow
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
@@ -584,12 +501,6 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
 // Weights: the taps' [N][Cin] matrices start at arbitrary offsets (the ConvTranspose phase groups use some taps of a
 // larger array), so the third dimension counts in units of the greatest common divisor of the offsets' differences,
 // from the lowest offset.  Rows n >= N of a box are then zeros, not the next matrix.
-CUtensorMapDataType map_dtype(int precision) {
-  return precision == VFX_PREC_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-         : precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-}
-
 int tma_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
   const long long esz = (long long)prec_esz(precision), LIM = 1LL << 40;          // tensor-map strides are below 2^40 bytes
   if (d.W <= 0 || d.H <= 0) return 0;
@@ -693,26 +604,13 @@ int tma_store_plan(int precision, const vfx_conv_desc& d, int bn, TmaPlan& tp) {
 
 template <int BN, int KIND, bool TMA, bool TST>
 int launch(const vfx_conv_desc& d, const TmaPlan& tp, int vec, cudaStream_t st) {
-  constexpr int smem = Cfg<BN, TMA, TST>::SMEM;
-  static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
-  int dev = 0;
-  VFX_CUDA_CHECK(cudaGetDevice(&dev));
-  if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_wgmma_kernel<BN, KIND, TMA, TST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    if (dev < 64) attr_set |= 1ull << dev;
-  }
-  const int sms = sm_count(dev);
-  VFX_REQUIRE(sms > 0, "conv_gemm_tc: cannot read the SM count of device %d", dev);
   const int nkc = ceil_div(d.Cin, 128 / OpT<KIND>::ESZ);
   const long long mtiles = TMA ? tp.mtiles : ((long long)d.B * d.Hq * d.Wq + BM - 1) / BM;
-  const long long tiles = mtiles * ceil_div(d.N, BN);
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
-  conv_gemm_wgmma_kernel<BN, KIND, TMA, TST><<<grid, NT, smem, st>>>(d, tp, nkc, vec);
-  VFX_LAUNCH_CHECK();
-  if (TMA) ++g_conv_tma_launches;
-  if (TST) ++g_conv_tma_store_launches;
-  return VFX_OK;
+  const int r = launch_persistent<conv_gemm_wgmma_kernel<BN, KIND, TMA, TST>>(
+      "conv_gemm_tc", Cfg<BN, TMA, TST>::Plan::SMEM, mtiles * ceil_div(d.N, BN), st, d, tp, nkc, vec);
+  if (r == VFX_OK && TMA) ++g_conv_tma_launches;
+  if (r == VFX_OK && TST) ++g_conv_tma_store_launches;
+  return r;
 }
 
 // Launches without per-item extents go through TMA where tma_plan can express them, and among those, the ones whose

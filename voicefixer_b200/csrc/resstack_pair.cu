@@ -1,22 +1,21 @@
 // ResStack pair x' = x + conv2_{k3,d=1}(lrelu_0.01(conv1_{k3,dilation}(a) + b1)) + b2 (include/vfx_b200.h,
 // vfx_resstack_pair), ResStack.forward voicefixer/vocoder/model/modules.py:592-595.
 //
-// Fused form (VFX_PAIR_FUSED; the engine's fused pairs): a persistent, warp-specialised kernel.  grid = min(tiles, SMs);
-// a tile is 126 output rows of one item, and each CTA walks a static stride over the (item, row block) tiles with the
-// row block fastest, so that neighbouring CTAs work on neighbouring rows and the dilation halo comes from L2.
-//  - Producer warpgroup: per tile, conv1's 3 x NKS K slices (the 128 a rows [r0 - 1, r0 + 127) shifted by the tap, and
-//    the tap's W1 rows), then conv2's 3 x NKS slices (W2 rows only), into a ring of 128-byte-swizzled K-major tiles handed
-//    over through full / empty mbarriers.  It runs ahead into the next tile's conv1 while the consumers finish conv2 and
-//    the epilogue of this one.  Two forms:
-//      TMA (launches without lens): one thread issues a box of the (C, L, B) operand map at row r0 - 1 + (tap - 1) *
-//      dilation and a box of the [3][C][C] weight map per slice; the out-of-bounds fill is conv1's zero padding.
-//      cp.async (ragged batches): the warpgroup stages 16-byte chunks with zero fill beyond the item's own length.
-//  - Two consumer warpgroups, 64 rows each: conv1 with one wgmma group in flight into one of two partials while the
-//    previous slice's partial is added to the fp32 accumulator (conv_gemm_tc.cu's K loop); its epilogue writes lrelu(h +
-//    b1) in the operand format into shared memory three times, copy t shifted up by t rows, so that conv2's tap t reads
-//    copy t as an ordinary K-major A tile (rows outside [0, L) are zero: conv2's padding).  The h copies are one buffer:
-//    a named barrier keeps the next tile's h writes behind this tile's last conv2 wgmma.  conv2 runs the same K loop
-//    from the h copies and its epilogue adds b2 and the residual and writes x' / act(x').
+// Fused form (VFX_PAIR_FUSED; the engine's fused pairs): a persistent, warp-specialised kernel on the pipeline of
+// tc_pipeline.cuh (ring, feed and K loop).  grid = min(tiles, SMs); a tile is 126 output rows of one item, and each CTA
+// walks a static stride over the (item, row block) tiles with the row block fastest, so that neighbouring CTAs work on
+// neighbouring rows and the dilation halo comes from L2.
+//  - Producer: per tile, conv1's 3 x NKS K slices (the 128 a rows [r0 - 1, r0 + 127) shifted by the tap, and the tap's
+//    W1 rows), then conv2's 3 x NKS slices (W2 rows only).  It runs ahead into the next tile's conv1 while the consumers
+//    finish conv2 and the epilogue of this one.  Two forms:
+//      TMA (launches without lens): a box of the (C, L, B) operand map at row r0 - 1 + (tap - 1) * dilation and a box of
+//      the [3][C][C] weight map per slice; the out-of-bounds fill is conv1's zero padding.
+//      cp.async (ragged batches): zero fill beyond the item's own length.
+//  - Consumers: conv1's K loop; its epilogue writes lrelu(h + b1) in the operand format into shared memory three times,
+//    copy t shifted up by t rows, so that conv2's tap t reads copy t as an ordinary K-major A tile (rows outside [0, L)
+//    are zero: conv2's padding).  The h copies are one buffer: a named barrier keeps the next tile's h writes behind this
+//    tile's last conv2 wgmma.  conv2's K loop reads its A tiles from the h copies, and its epilogue adds b2 and the
+//    residual and writes x' / act(x').
 //  - Nothing global in the epilogues' critical path: b1 and b2 are staged in shared memory once per CTA.  In tf32 the
 //    residual (the encoded stream, a == x) is rows 1 ... 126 of conv1's centre-tap A tiles, which are kept out of the
 //    ring for that, read into registers in the h epilogue and then released to the producer (one mbarrier).  In the
@@ -29,37 +28,23 @@
 // Every sum is in the order of the blocked form: per K slice 4 wgmma into a zeroed partial, partials added in (tap,
 // channel slice) order with round-to-nearest fp32 adds, then (acc + b) + residual.
 //
-// Blocked form (VFX_PAIR_BLOCKED, the tests' reference): conv_gemm_tc.cu's two convolutions per row block, h in a scratch.
+// Blocked form (VFX_PAIR_BLOCKED, the tests' reference): two conv_gemm_tc launches per row block, h in a scratch.
 #include <string.h>
-#include "tc_ptx.cuh"
-#include "wgmma_ptx.cuh"
+#include "tc_pipeline.cuh"
 
 namespace vfx {
 
 namespace {
 constexpr size_t PAIR_SCRATCH_BYTES = 32u << 20;
 
-template <int KIND> struct PairT;
-template <> struct PairT<0> { using T = tf32_t; static constexpr int ESZ = 4; };
-template <> struct PairT<1> { using T = __nv_bfloat16; static constexpr int ESZ = 2; };
-template <> struct PairT<2> { using T = __half; static constexpr int ESZ = 2; };
+constexpr int P_ROWS = 126;                       // output rows of a tile (of the 128 rows of its A tiles)
 
-constexpr int P_ROWS = 126, P_NT = 384, P_A_BYTES = 128 * 128;   // warpgroup 0 produces, warpgroups 1 and 2 consume
-constexpr int P_SMEM_MAX = 227 * 1024;
-constexpr int P_PROD_REGS = 56, P_CONS_REGS = 224;               // 128 x 56 + 256 x 224 <= 384 x 168
-
+// Shared memory beside the ring: the h copies, the tf32 centre tiles, b1 / b2 and the centre tiles' mbarrier
 template <int C, int KIND> struct PairCfg {
-  static constexpr int ESZ = PairT<KIND>::ESZ, NKS = C * ESZ / 128, NITER = 3 * NKS;   // K slices per convolution
-  static constexpr int STAGE = P_A_BYTES + C * 128;
+  static constexpr int ESZ = OpT<KIND>::ESZ, NKS = C * ESZ / 128, NITER = 3 * NKS;   // K slices per convolution
   static constexpr int H = 3 * NKS * 16384;                       // the three h copies
   static constexpr int CTR = KIND == 0 ? NKS * 16384 : 0;         // tf32: conv1's centre-tap A tiles (the residual)
-  static constexpr int FIXED = 1024 + H + CTR + 2 * C * 4 + 8;    // + ring alignment, b1 / b2, the centre's barrier
-  static constexpr int FIT = (P_SMEM_MAX - FIXED) / (STAGE + 16);
-  static constexpr int STAGES = FIT < 8 ? FIT : 8;
-  // cp.async: slice k is signalled full after slice k + AHEAD is issued (conv_gemm_tc.cu's Cfg::AHEAD)
-  static constexpr int AHEAD = STAGES - 2;
-  static constexpr int SMEM = FIXED + STAGES * (STAGE + 16);
-  static_assert(STAGES >= 3 && SMEM <= P_SMEM_MAX, "resstack_pair: shared-memory plan");
+  using Plan = RingPlan<A_BYTES + C * 128, H + CTR + 2 * C * 4 + 8, 3>;   // 4 stages tf32, 7 16-bit C = 64, 4 C = 128
 };
 
 // What a TMA launch carries beside the descriptor: the operand (C, L, B), box (128 bytes, 128 rows, 1), and the two
@@ -83,38 +68,34 @@ __device__ __forceinline__ bool pair_tile(const vfx_pair_desc& d, int nrb, int t
 }
 
 template <int C, int KIND, bool TMA>
-__global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_constant__ vfx_pair_desc d,
+__global__ void __launch_bounds__(NT, 1) pair_fused_kernel(const __grid_constant__ vfx_pair_desc d,
                                                              const __grid_constant__ PairMaps m, const int niter) {
-  using T = typename PairT<KIND>::T;
+  using T = typename OpT<KIND>::T;
   using G = PairCfg<C, KIND>;
   constexpr int ESZ = G::ESZ, AL = 16 / ESZ, BK = 128 / ESZ, NKS = G::NKS, NITER = G::NITER;
-  constexpr int S = G::STAGES, STAGE = G::STAGE, AHEAD = G::AHEAD;
+  constexpr int S = G::Plan::STAGES, STAGE = G::Plan::STAGE;
   constexpr bool EARLY = KIND != 0 && C == 64;    // 16-bit C = 64: the residual goes to registers before conv2
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* const gbase = smem_raw + (sbase - smem_u32(smem_raw));
-  const uint32_t hbase = sbase + S * STAGE, cbase = hbase + G::H;
+  const Ring<typename G::Plan> ring{(smem_u32(smem_raw) + 1023u) & ~1023u};
+  uint8_t* const gbase = smem_raw + (ring.base - smem_u32(smem_raw));
+  const uint32_t hbase = ring.base + S * STAGE, cbase = hbase + G::H, cempty = cbase + G::CTR + 2 * C * 4;
   uint8_t* const hgen = gbase + S * STAGE;
   const uint8_t* const cgen = hgen + G::H;
   float* const bias = reinterpret_cast<float*>(hgen + G::H + G::CTR);          // b1[C], b2[C]
-  const uint32_t full0 = cbase + G::CTR + 2 * C * 4, empty0 = full0 + 8 * S, cempty = empty0 + 8 * S;
 
   const int tid = threadIdx.x;
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(full0 + 8 * s, TMA ? 1 : 128);      // the issuing thread's expect_tx + the bytes, or every producer thread
-      mbar_init(empty0 + 8 * s, 8);                 // every consumer warp, after its wgmma group has read the stage
-    }
+    ring.init(TMA);
     mbar_init(cempty, 8);                           // every consumer warp, after it has read its residual rows
   }
-  for (int i = tid; i < 2 * C; i += P_NT) bias[i] = i < C ? d.b1[i] : d.b2[i - C];
+  for (int i = tid; i < 2 * C; i += NT) bias[i] = i < C ? d.b1[i] : d.b2[i - C];
   __syncthreads();
   // derived after each role's setmaxnreg, so that nothing stays live across it
 #define VFX_PAIR_WALK const int nrb = (d.L + P_ROWS - 1) / P_ROWS, ntiles = d.B * nrb;
 
   if (tid < 128) {
     // ================================================================ producer
-    setmaxnreg_dec<P_PROD_REGS>();
+    setmaxnreg_dec<PROD_REGS>();
     VFX_PAIR_WALK
     uint32_t k = 0, u = 0;                          // K slices issued, tiles staged by this CTA
     if constexpr (TMA) {
@@ -123,20 +104,19 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
         int b, r0, L;
         pair_tile(d, nrb, t, b, r0, L);
         for (int it = 0; it < 2 * NITER; ++it, ++k) {
-          const int s = k % S;
-          if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+          ring.acquire(k);
           const bool p2 = it >= NITER;
           const int kk = p2 ? it - NITER : it, tap = kk / NKS, ks = kk - tap * NKS;
-          const uint32_t sa = sbase + s * STAGE, full = full0 + 8 * s;
+          const uint32_t sa = ring.stage(k), full = ring.full(k);
           if (!p2) {
             const bool ctr = KIND == 0 && tap == 1;
             if (ctr && ks == 0 && u > 0) mbar_wait(cempty, (u - 1) & 1);   // the last tile's residual has been read
-            mbar_expect_tx(full, P_A_BYTES + C * 128);
+            mbar_expect_tx(full, A_BYTES + C * 128);
             tma_load_3d(ctr ? cbase + ks * 16384 : sa, &m.a, full, ks * BK, r0 - 1 + (tap - 1) * d.dilation, b);
           } else {
             mbar_expect_tx(full, C * 128);
           }
-          tma_load_3d(sa + P_A_BYTES, p2 ? &m.w2 : &m.w1, full, ks * BK, 0, tap);
+          tma_load_3d(sa + A_BYTES, p2 ? &m.w2 : &m.w1, full, ks * BK, 0, tap);
         }
       }
       return;
@@ -148,11 +128,10 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
       if (!pair_tile(d, nrb, t, b, r0, L)) continue;
       const char* A = static_cast<const char*>(d.a) + (long long)b * d.L * C * ESZ;
       for (int it = 0; it < 2 * NITER; ++it, ++k) {
-        const int s = k % S;
-        if (k >= (uint32_t)S) mbar_wait(empty0 + 8 * s, ((k / S) & 1) ^ 1);
+        ring.acquire(k);
         const bool p2 = it >= NITER;
         const int kk = p2 ? it - NITER : it, tap = kk / NKS, ks = kk - tap * NKS, c = ks * BK + chunk * AL;
-        const uint32_t sa = sbase + s * STAGE;
+        const uint32_t sa = ring.stage(k);
         if (!p2) {
           const bool ctr = KIND == 0 && tap == 1;
           if (ctr && ks == 0 && u > 0) mbar_wait(cempty, (u - 1) & 1);
@@ -168,25 +147,18 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
 #pragma unroll
         for (int i = 0; i < C / 16; ++i) {
           const int n = lrow + 16 * i;
-          cp_async16(sa + P_A_BYTES + sw128_offset(n, chunk), W + (long long)n * C * ESZ, true);
+          cp_async16(sa + A_BYTES + sw128_offset(n, chunk), W + (long long)n * C * ESZ, true);
         }
-        cp_async_commit();
-        if (k >= (uint32_t)AHEAD) {
-          cp_async_wait<AHEAD>();                   // this thread's chunks of slice k - AHEAD have landed
-          fence_proxy_async();                      // ... and are visible to the tensor core's (async-proxy) reads
-          mbar_arrive(full0 + 8 * ((k - AHEAD) % S));
-        }
+        ring.cp_async_handoff(k);
       }
       ++u;
     }
-    cp_async_wait<0>();
-    fence_proxy_async();
-    for (uint32_t j = k > (uint32_t)AHEAD ? k - AHEAD : 0; j < k; ++j) mbar_arrive(full0 + 8 * (j % S));
+    ring.cp_async_drain(k);
     return;
   }
 
   // ================================================================== consumers
-  setmaxnreg_inc<P_CONS_REGS>();
+  setmaxnreg_inc<CONS_REGS>();
   VFX_PAIR_WALK
 #undef VFX_PAIR_WALK
   const int ct = tid - 128, cw = ct >> 7, w = (ct >> 5) & 3, l = tid & 31;
@@ -194,59 +166,13 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
   T* const out_act = reinterpret_cast<T*>(d.out_act);
   const float* const b1 = bias;
   const float* const b2 = bias + C;
-  float acc[C / 2], p0[C / 2], p1[C / 2], xr[C / 2];
-  // issue slice kk (slice it of the tile: conv1 for it < NITER, conv2 after) as 4 wgmma into p, zeroed
-  auto issue = [&](float (&p)[C / 2], uint32_t kk, int it) {
-    const uint32_t s = kk % S;
-    mbar_wait(full0 + 8 * s, (kk / S) & 1);
-#pragma unroll
-    for (int i = 0; i < C / 2; ++i) p[i] = 0.f;
-    const uint32_t sa = sbase + s * STAGE;
-    const uint32_t a_tile = it >= NITER ? hbase + (uint32_t)(it - NITER) * 16384
-                            : KIND == 0 && it / NKS == 1 ? cbase + (uint32_t)(it - NKS) * 16384 : sa;
-    const uint64_t da = sw128_desc(a_tile + cw * 64 * 128), db = sw128_desc(sa + P_A_BYTES);
-    wgmma_fence();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) Wgmma<C, KIND>::mma(p, da + 2 * q, db + 2 * q);
-    wgmma_commit();
+  float acc[C / 2], xr[C / 2];
+  // the A tile of K slice it (of the niter = NITER slices, a kernel argument: see k_loop): conv1's come from the ring,
+  // except in tf32 the centre tap's, which are the centre tiles; conv2's are the h copies
+  const auto conv1_a = [&](int it, uint32_t sa) {
+    return KIND == 0 && it / NKS == 1 ? cbase + (uint32_t)(it - NKS) * 16384 : sa;
   };
-  // slice kk's group has completed: free its stage and add it (round to nearest, in slice order)
-  auto retire = [&](float (&p)[C / 2], uint32_t kk) {
-    wgmma_fence_operand(p);
-    __syncwarp();
-    if (l == 0) mbar_arrive(empty0 + 8 * (kk % S));
-#pragma unroll
-    for (int i = 0; i < C / 2; ++i) acc[i] += p[i];
-    wgmma_fence_operand(acc);                       // the adds stay here, before the next slice is issued: p is reused
-  };
-  // one convolution: the niter (= NITER) slices from ring slice k0, tile slice it0; slice it goes to p[it & 1] and
-  // slice it - 1 is added while slice it is in flight.  The count is a kernel argument, as in conv_gemm_tc.cu: with
-  // the compile-time NITER, ptxas peels the loop and serialises its wgmma groups (C7514).
-  auto conv = [&](uint32_t k0, int it0) {
-#pragma unroll
-    for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
-    issue(p0, k0, it0);
-    int it = 1;
-#pragma unroll 1
-    for (; it + 1 < niter; it += 2) {
-      issue(p1, k0 + it, it0 + it);
-      wgmma_wait<1>();
-      retire(p0, k0 + it - 1);
-      issue(p0, k0 + it + 1, it0 + it + 1);
-      wgmma_wait<1>();
-      retire(p1, k0 + it);
-    }
-    if (it < niter) {
-      issue(p1, k0 + it, it0 + it);
-      wgmma_wait<1>();
-      retire(p0, k0 + it - 1);
-      wgmma_wait<0>();
-      retire(p1, k0 + it);
-    } else {
-      wgmma_wait<0>();
-      retire(p0, k0 + it - 1);
-    }
-  };
+  const auto conv2_a = [&](int it, uint32_t) { return hbase + (uint32_t)it * 16384; };
   // accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is row cw*64 + w*16 + l/4 + 8h,
   // column 8j + 2(l%4) + e
   const int row0 = cw * 64 + w * 16 + (l >> 2);
@@ -273,7 +199,7 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
     };
 
     // ---- conv1 -> h copies
-    conv(k, 0);
+    k_loop<C, KIND>(ring, acc, k, niter, cw, l, conv1_a, [](int) {});
     k += NITER;
     named_sync(1, 256);                             // every consumer's conv2 of the last tile has read the h copies
 #pragma unroll
@@ -328,7 +254,7 @@ __global__ void __launch_bounds__(P_NT, 1) pair_fused_kernel(const __grid_consta
     named_sync(1, 256);
 
     // ---- conv2 from the h copies, residual, outputs
-    conv(k, NITER);
+    k_loop<C, KIND>(ring, acc, k, niter, cw, l, conv2_a, [](int) {});
     k += NITER;
     if constexpr (KIND != 0 && !EARLY) load_res();
 #pragma unroll
@@ -365,9 +291,7 @@ int pair_maps(const vfx_pair_desc& d, PairMaps& m) {
   const long long esz = (long long)prec_esz(d.precision), C = d.C;
   const EncodeTiled encode = tensor_map_encoder();
   VFX_REQUIRE(encode, "resstack_pair: this CUDA driver has no cuTensorMapEncodeTiled");
-  const CUtensorMapDataType dt = d.precision == VFX_PREC_TF32   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                 : d.precision == VFX_PREC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                                : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = map_dtype(d.precision);
   const cuuint32_t bk = (cuuint32_t)(128 / esz), ones[3] = {1, 1, 1};
   const cuuint64_t adim[3] = {(cuuint64_t)C, (cuuint64_t)d.L, (cuuint64_t)d.B};
   const cuuint64_t astr[2] = {(cuuint64_t)(C * esz), (cuuint64_t)(d.L * C * esz)};
@@ -390,22 +314,9 @@ int pair_maps(const vfx_pair_desc& d, PairMaps& m) {
 
 template <int C, int KIND, bool TMA>
 int launch_pair(const vfx_pair_desc& d, const PairMaps& m, cudaStream_t st) {
-  constexpr int smem = PairCfg<C, KIND>::SMEM;
-  static unsigned long long attr_set = 0;      // devices on which the shared-memory limit has been raised
-  int dev = 0;
-  VFX_CUDA_CHECK(cudaGetDevice(&dev));
-  if (dev >= 64 || !(attr_set >> dev & 1)) {
-    VFX_CUDA_CHECK(cudaFuncSetAttribute(pair_fused_kernel<C, KIND, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    if (dev < 64) attr_set |= 1ull << dev;
-  }
-  const int sms = sm_count(dev);
-  VFX_REQUIRE(sms > 0, "resstack_pair: cannot read the SM count of device %d", dev);
-  const long long tiles = (long long)d.B * ceil_div(d.L, P_ROWS);
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  if (tiles + grid >= (1LL << 31)) return VFX_ERR_UNSUPPORTED;      // the tile walk t += gridDim.x stays inside int
-  pair_fused_kernel<C, KIND, TMA><<<grid, P_NT, smem, st>>>(d, m, PairCfg<C, KIND>::NITER);
-  VFX_LAUNCH_CHECK();
-  return VFX_OK;
+  return launch_persistent<pair_fused_kernel<C, KIND, TMA>>("resstack_pair", PairCfg<C, KIND>::Plan::SMEM,
+                                                            (long long)d.B * ceil_div(d.L, P_ROWS), st, d, m,
+                                                            PairCfg<C, KIND>::NITER);
 }
 
 // launches without per-item lengths are fed by TMA, ragged ones by cp.async
