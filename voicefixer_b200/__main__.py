@@ -1,11 +1,13 @@
 """Command line mirror of the reference's `voicefixer` entry point (voicefixer/__main__.py:13-219):
 
     python -m voicefixer_b200 --infile in.wav --outfile out.wav [--mode 0|1|2|all]
-    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...]
+    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...] [--batch]
 
 Same flags, same output naming (`--mode all` writes `<name>-mode<k><ext>` for k = 0,1,2), same
 `.wav`-only input rule, same messages.  The work is planned first (`plan_jobs`, a pure function) and
-then executed with one VoiceFixer instance as a reader -> GPU -> writer pipeline (`run_jobs`)."""
+then executed with one VoiceFixer instance as a reader -> GPU -> writer pipeline (`run_jobs`), one
+file at a time; with `--batch` the same jobs run through `VoiceFixer.restore_files`, many files per
+batch (`execute`)."""
 import argparse
 import os
 import re
@@ -32,6 +34,8 @@ def build_parser():
     p.add_argument("--silent", default=False, action="store_true", help="Set this flag if you do not want to see any message.")
     p.add_argument("--weight_prepare", default=False, action="store_true",
                    help="Only check that the checkpoints are present (the reference uses it to trigger the download).")
+    p.add_argument("--batch", default=False, action="store_true",
+                   help="Restore many files at once (VoiceFixer.restore_files): the same outputs, batched across files.")
     return p
 
 
@@ -148,6 +152,22 @@ def run_jobs(jobs, load, restore, save, say=print, depth=2):
     return took
 
 
+def execute(vf, jobs, batch=False, cuda=True, say=print):
+    """Runs [(src, dst, mode)] with the VoiceFixer vf: one file at a time through run_jobs, or with batch through
+    vf.restore_files, which prints the same `Processing` line per job as its wave starts and one `Restoration took`
+    line per wave."""
+    from . import wavio
+    if not batch:
+        run_jobs(jobs,                                                        # = vf.restore(input, output, ...) per job
+                 load=lambda src: vf._load_wav(src, sample_rate=44100),      # base.py:141-146, staged
+                 restore=lambda wav, mode: vf.restore_inmem(wav, cuda=cuda, mode=mode),
+                 save=lambda out, dst: wavio.save_wave(out, fname=dst, sample_rate=44100), say=say)
+    elif jobs:
+        vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda,
+                         _on_wave=lambda ids: [say("Processing {}, mode={}".format(jobs[i][0], jobs[i][2])) for i in ids],
+                         _on_wave_done=lambda ids, s: print("Restoration took {} s".format(round(s, 1))))
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.weight_prepare:
@@ -167,12 +187,8 @@ def main(argv=None):
     from .api import VoiceFixer
     vf = VoiceFixer()
     say("Start processing %d job(s)." % len(jobs))
-    from . import wavio
     t0 = time.time()
-    run_jobs(jobs,                                                            # = vf.restore(input, output, ...) per job
-             load=lambda src: vf._load_wav(src, sample_rate=44100),          # base.py:141-146, staged
-             restore=lambda wav, mode: vf.restore_inmem(wav, cuda=not args.disable_cuda, mode=mode),
-             save=lambda out, dst: wavio.save_wave(out, fname=dst, sample_rate=44100), say=say)
+    execute(vf, jobs, batch=args.batch, cuda=not args.disable_cuda, say=say)
     say("Done: {} job(s) in {} s".format(len(jobs), round(time.time() - t0, 3)))
     return 0
 

@@ -125,6 +125,110 @@ def plan_many(lengths, mode, max_items, what="restore_many"):
     return [(L_cap, [segs[j] for j in idx]) for L_cap, idx in _pack([b - a for _, a, b in segs], max_items)]
 
 
+def plan_waves(lengths, budget):
+    """The waves VoiceFixer.restore_files runs files in: consecutive runs of indices into lengths (the files' lengths at
+    44.1 kHz), in input order, every index in exactly one.  A wave takes the next file while the lengths in it still sum
+    to at most budget samples; a file longer than budget is a wave of its own (restore_many cuts it into batches).
+    A generator that reads lengths lazily: each wave is yielded once the first length past it is known, so a reader can
+    decode the files as it goes."""
+    wave, total = [], 0
+    for i, n in enumerate(lengths):
+        if wave and total + int(n) > budget:
+            yield wave
+            wave, total = [], 0
+        wave.append(i)
+        total += int(n)
+    if wave:
+        yield wave
+
+
+def run_waves(srcs, budget, load, restore, write, depth=2):
+    """The pipeline of VoiceFixer.restore_files over jobs 0 .. len(srcs) - 1, srcs[i] being job i's input file:
+
+    a reader thread calls load(i, prev) -> (item, length at 44.1 kHz) for each job in order and groups the jobs into
+    waves by plan_waves(lengths, budget).  prev is the item load returned for an earlier job of the same wave with the
+    same source, or None: load then checks that item for job i rather than reading the file again.
+    The calling thread calls restore(wave) -> result for each wave [(i, item), ...]; it may return before the GPU is done.
+    A writer thread calls write([i, ...], result) for each wave, which writes the wave's outputs in order.
+
+    At most `depth` loaded and `depth` restored waves are in flight.  Errors follow run_jobs's order rule: a failing load
+    cuts its wave short (the jobs before it in the wave are restored and written), a failing restore fails its wave,
+    every job before the failure is written and nothing after it is started, and the exception is re-raised once the
+    threads have drained.  Returns the number of waves restored."""
+    import queue
+    import threading
+    loaded, finished = queue.Queue(maxsize=depth), queue.Queue(maxsize=depth)
+    stop, write_errors = threading.Event(), []
+
+    def reader():
+        pending = {}                                     # job -> item: loaded and not yet handed on
+
+        def lengths():
+            for i, src in enumerate(srcs):
+                if stop.is_set():
+                    return
+                prev = next((pending[j] for j in pending if srcs[j] == src), None)
+                pending[i], n = load(i, prev)
+                yield n
+
+        try:
+            for wave in plan_waves(lengths(), budget):
+                loaded.put([(i, pending.pop(i)) for i in wave])
+        except BaseException as e:                       # noqa: BLE001 - re-raised by the caller's thread
+            if pending:                                  # the jobs before the failing one
+                loaded.put(sorted(pending.items()))
+            loaded.put(e)
+        finally:
+            loaded.put(None)
+
+    def writer():
+        while True:
+            item = finished.get()
+            if item is None:
+                return
+            if write_errors:
+                continue                                 # drain
+            try:
+                write(*item)
+            except BaseException as e:                   # noqa: BLE001
+                write_errors.append(e)
+                stop.set()
+
+    threads = [threading.Thread(target=reader, name="vfx-wave-reader", daemon=True),
+               threading.Thread(target=writer, name="vfx-wave-writer", daemon=True)]
+    for t in threads:
+        t.start()
+    failure, waves = None, 0
+    try:
+        while True:
+            item = loaded.get()
+            if item is None:
+                break
+            if failure is not None or stop.is_set():
+                continue                                 # keep draining so the reader can finish
+            if isinstance(item, BaseException):
+                failure = item
+                stop.set()
+                continue
+            try:
+                result = restore(item)
+            except BaseException as e:                   # noqa: BLE001
+                failure = e
+                stop.set()
+                continue
+            waves += 1
+            finished.put(([i for i, _ in item], result))
+    finally:
+        finished.put(None)
+        for t in threads:
+            t.join()
+    if write_errors:
+        raise write_errors[0]
+    if failure is not None:
+        raise failure
+    return waves
+
+
 def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
     """Packs the items of Vocoder.forward_many (kind "mel": [1, 1, T, 128] mels) or Vocoder.oracle_many (kind "wav": 1-D
     float32 recordings) into ragged batches by length with _pack, cap being a batch's longest item in frames (mels) or
@@ -1443,3 +1547,119 @@ class VoiceFixer:
         wav_10k = self._load_wav(input, sample_rate=44100)               # base.py:141-146
         out_np_wav = self.restore_inmem(wav_10k, cuda=cuda, mode=mode, your_vocoder_func=your_vocoder_func)
         wavio.save_wave(out_np_wav, fname=output, sample_rate=44100)
+
+    @torch.no_grad()
+    def restore_files(self, inputs, outputs, mode=0, cuda=True, dropout_seed=None, _budget=None, _on_wave=None,
+                      _on_wave_done=None):
+        """Extension of the reference API: restore(inputs[i], outputs[i]) for many files, the files batched across each
+        other.  Output file i is byte for byte what restore(inputs[i], outputs[i], mode=mode_i) writes in modes 0 and 1,
+        for .wav and .flac at every rate and channel count the readers take.  In mode 2 with dropout_seed it is what
+        save_wave(restore_inmem(load_mono(inputs[i]), mode=2, dropout_seed=seed_i), outputs[i]) writes; without a seed the
+        masks are random, with restore()'s distribution.
+
+        mode: one of 0, 1, 2 for every file, or one per file (so an input may be listed several times with different
+        outputs and modes).  dropout_seed: one int in [0, 2^64) or one per file, as in restore_many; it is the dropout of
+        the files restored in mode 2, and refused when there is none.  A length mismatch, an empty list, a bad mode or a
+        bad seed raises ValueError before anything is read.  Output directories are not created, as with restore().
+
+        The files run in waves of consecutive files (plan_waves), about twice the audio of the largest 30 s batch the
+        free device memory holds, through three stages (run_waves): a reader thread decodes each file at its own rate
+        (wavio.load_mono_native, the next files ahead in a four-thread pool) into pinned memory and checks it as restore_many would; the calling thread uploads the
+        wave, runs one device-resident restore_many(..., sample_rate=) per mode present (an input listed several times
+        in a wave is decoded and uploaded once), queues one copy of all the wave's outputs into pinned memory and an
+        event, and goes on to the next wave without waiting; a writer thread waits for that event and writes each output
+        with wavio.save_wave.  The GPU never waits for the host between waves.
+
+        Errors: every file before a failing one, in input order, is written and none after it is started; the exception
+        is re-raised once the threads have drained.  A file that cannot be read or written raises RuntimeError, and one
+        too short for its mode or at a bad rate ValueError, each naming the file; such a file cuts its wave short, the
+        files before it in that wave still being restored and written.
+
+        _budget (samples at 44.1 kHz per wave), _on_wave(jobs) (called as a wave starts) and _on_wave_done(jobs,
+        seconds) (called as its outputs reach the host, with the GPU time from its upload to its copy back) are for the
+        command line and the tests."""
+        _check_cuda(cuda)
+        inputs, outputs = [str(p) for p in inputs], [str(p) for p in outputs]
+        n = len(inputs)
+        if n == 0 or len(outputs) != n:
+            raise ValueError(f"restore_files takes a non-empty list of inputs and as many outputs; got {n} inputs and "
+                             f"{len(outputs)} outputs")
+        modes = list(mode) if isinstance(mode, (list, tuple, np.ndarray)) else [mode] * n
+        if len(modes) != n:
+            raise ValueError(f"restore_files: mode has {len(modes)} entries for {n} files; give one mode, or one per file")
+        for i, m in enumerate(modes):
+            if isinstance(m, (bool, np.bool_)) or m not in (0, 1, 2):
+                raise ValueError(f"restore_files: file {i} has mode {m!r}; mode must be 0, 1 or 2")
+        modes = [int(m) for m in modes]
+        seeds = None
+        if dropout_seed is not None:
+            if 2 not in modes:
+                raise ValueError("restore_files: dropout_seed is mode 2's dropout; no file is restored in mode 2")
+            seeds = dropout_seeds(dropout_seed, 2, None, n, "restore_files")
+        eng = self._engine
+        dev = f"cuda:{eng.device}"
+        budget = _budget if _budget is not None else 2 * eng.max_batch(SEG_LENGTH) * SEG_LENGTH
+        from concurrent.futures import ThreadPoolExecutor
+        pool = ThreadPoolExecutor(max_workers=4, thread_name_prefix="vfx-decode")
+        ahead = {}                                                       # input -> its decode, started ahead of use
+
+        def decode(path):
+            x, sr = wavio.load_mono_native(path)
+            return torch.from_numpy(x).pin_memory(), sr
+
+        def load(i, prev):
+            if prev is None:
+                for j in range(i, min(n, i + 8)):        # the next inputs decode in the background, each path once
+                    if j not in ahead and inputs[j] not in inputs[i:j]:
+                        ahead[j] = pool.submit(decode, inputs[j])
+                try:
+                    x, sr = (ahead.pop(i, None) or pool.submit(decode, inputs[i])).result()
+                except Exception as e:
+                    raise RuntimeError(f"restore_files: {inputs[i]}: {e}") from e
+                prev = (x, resample.check_rate(sr, f"restore_files: {inputs[i]}"))
+            x, sr = prev
+            n44 = resample.out_len(x.shape[0], sr)
+            plan_many([n44], modes[i], lambda L: 1, what=f"restore_files: {inputs[i]}")     # restore_many's refusals
+            return prev, n44
+
+        def restore(wave):
+            ids = [i for i, _ in wave]
+            if _on_wave is not None:
+                _on_wave(ids)
+            start, done = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            start.record()
+            up = {}                                                      # id(item) -> the input on the device
+            for _, item in wave:
+                if id(item) not in up:
+                    up[id(item)] = item[0].to(dev, non_blocking=True)
+            outs = {}
+            for m in sorted(set(modes[i] for i in ids)):
+                run = [(i, item) for i, item in wave if modes[i] == m]
+                ys = self.restore_many([up[id(item)] for _, item in run], cuda=True, mode=m,
+                                       sample_rate=[item[1] for _, item in run],
+                                       dropout_seed=[seeds[i] for i, _ in run] if seeds is not None and m == 2 else None)
+                outs.update((i, y.view(-1)) for (i, _), y in zip(run, ys))
+            flat = torch.cat([outs[i] for i in ids])
+            host = torch.empty(flat.shape, pin_memory=True)
+            host.copy_(flat, non_blocking=True)
+            done.record()
+            offs = np.cumsum([0] + [outs[i].shape[0] for i in ids])
+            return host, {i: (int(offs[k]), int(offs[k + 1])) for k, i in enumerate(ids)}, start, done
+
+        def write(ids, result):
+            host, spans, start, done = result
+            done.synchronize()
+            if _on_wave_done is not None:
+                _on_wave_done(ids, start.elapsed_time(done) / 1e3)
+            y = host.numpy()
+            for i in ids:
+                a, b = spans[i]
+                try:
+                    wavio.save_wave(y[None, a:b], fname=outputs[i], sample_rate=44100)
+                except Exception as e:
+                    raise RuntimeError(f"restore_files: {outputs[i]}: {e}") from e
+
+        try:
+            run_waves(inputs, budget, load, restore, write)
+        finally:
+            pool.shutdown(wait=True, cancel_futures=True)

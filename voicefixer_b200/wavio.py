@@ -81,10 +81,15 @@ def _resample(x, sr_in, sr_out):
     return resample_poly(x, sr_out // g, sr_in // g, axis=0).astype(np.float32)
 
 
+def load_mono_native(path):
+    """(x, sr): the file's mono mix (mean over channels), float32, at its own rate sr."""
+    x, sr = _read_pcm(path)
+    return x.mean(axis=1).astype(np.float32), sr
+
+
 def load_mono(path, sample_rate=44100):
     """librosa.load(path, sr=sample_rate): mono mix (mean over channels), float32."""
-    x, sr = _read_pcm(path)
-    return _resample(x.mean(axis=1).astype(np.float32), sr, sample_rate)
+    return _resample(*load_mono_native(path), sample_rate)
 
 
 def read_wave(path, sample_rate):
