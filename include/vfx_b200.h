@@ -312,6 +312,30 @@ int vfx_scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_ite
                      size_t workspace_bytes, void* stream);
 size_t vfx_scatter_rows_workspace_bytes(int B);
 
+/* The most channels one file of vfx_pack_pcm16 may have (also the most a FLAC stream holds). */
+#define VFX_PCM16_MAX_CHANNELS 8
+
+/* One file of vfx_pack_pcm16: its C channels are the float32 device rows rows[0 .. C), n samples each; its interleaved
+ * int16 samples [n][C] go to y[dst_off .. dst_off + n * C). */
+typedef struct vfx_pcm16_item {
+  const float* rows[VFX_PCM16_MAX_CHANNELS];
+  long long n, dst_off;
+  int C;
+} vfx_pcm16_item;
+
+/* 16-bit PCM of B files in two launches (a per-file maximum, then the packing), with the arithmetic of the host
+ * quantiser (wavio.pcm16, tools/wav.py's save_wave) bit for bit: a file whose maximum over all its samples is <= 1 is
+ * scaled by 32768 (a NaN anywhere makes the maximum NaN, and the file is not scaled); each value is truncated toward
+ * zero to int32 and its low 16 bits kept, a value outside int32's range, +-inf and NaN giving 0 (what the x86 C cast
+ * numpy uses gives).  y: a device buffer of y_elems int16.  The library validates every item before any launch: C in
+ * [1, VFX_PCM16_MAX_CHANNELS]; rows[0 .. C) non-null; n >= 1; 0 <= dst_off and dst_off + n * C <= y_elems; and no two
+ * items' destination ranges overlap.  A bad item returns VFX_ERR_INVALID naming it, and nothing is launched or
+ * written.  The table and the per-file maxima are staged into the workspace: vfx_pack_pcm16_workspace_bytes(B) bytes
+ * (0 for B <= 0).  B <= 65535. */
+int vfx_pack_pcm16(const vfx_pcm16_item* items_host, int B, short* y, long long y_elems, void* workspace,
+                   size_t workspace_bytes, void* stream);
+size_t vfx_pack_pcm16_workspace_bytes(int B);
+
 /* ---- per-kernel test entry points (tests/ call the kernels through these) --------------- */
 
 /* Generic channels-last "shifted-window" convolution GEMM; the one kernel family behind every

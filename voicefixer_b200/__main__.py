@@ -1,13 +1,14 @@
 """Command line mirror of the reference's `voicefixer` entry point (voicefixer/__main__.py:13-219):
 
     python -m voicefixer_b200 --infile in.wav --outfile out.wav [--mode 0|1|2|all]
-    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...] [--batch]
+    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...] [--batch] [--keep-channels]
 
 Same flags, same output naming (`--mode all` writes `<name>-mode<k><ext>` for k = 0,1,2), same
 `.wav`-only input rule, same messages.  The work is planned first (`plan_jobs`, a pure function) and
 then executed with one VoiceFixer instance as a reader -> GPU -> writer pipeline (`run_jobs`), one
 file at a time; with `--batch` the same jobs run through `VoiceFixer.restore_files`, many files per
-batch (`execute`)."""
+batch (`execute`).  With `--keep-channels` every channel of a file is restored and written (restore(...,
+channels="keep")), on either path, with the same bytes."""
 import argparse
 import os
 import re
@@ -36,6 +37,8 @@ def build_parser():
                    help="Only check that the checkpoints are present (the reference uses it to trigger the download).")
     p.add_argument("--batch", default=False, action="store_true",
                    help="Restore many files at once (VoiceFixer.restore_files): the same outputs, batched across files.")
+    p.add_argument("--keep-channels", default=False, action="store_true",
+                   help="Restore every channel of a multichannel file and write them all, instead of its mono mix.")
     return p
 
 
@@ -152,18 +155,23 @@ def run_jobs(jobs, load, restore, save, say=print, depth=2):
     return took
 
 
-def execute(vf, jobs, batch=False, cuda=True, say=print):
+def execute(vf, jobs, batch=False, cuda=True, say=print, channels="mix"):
     """Runs [(src, dst, mode)] with the VoiceFixer vf: one file at a time through run_jobs, or with batch through
     vf.restore_files, which prints the same `Processing` line per job as its wave starts and one `Restoration took`
-    line per wave."""
+    line per wave.  channels: restore()'s ("mix" or "keep")."""
     from . import wavio
     if not batch:
-        run_jobs(jobs,                                                        # = vf.restore(input, output, ...) per job
-                 load=lambda src: vf._load_wav(src, sample_rate=44100),      # base.py:141-146, staged
-                 restore=lambda wav, mode: vf.restore_inmem(wav, cuda=cuda, mode=mode),
+        if channels == "keep":                                            # = vf.restore(..., channels="keep") per job
+            load = lambda src: wavio.read_wave(src, 44100)                # noqa: E731
+            restore = lambda wav, mode: vf.restore_columns(wav, cuda=cuda, mode=mode)   # noqa: E731
+        else:                                                             # = vf.restore(input, output, ...) per job
+            load = lambda src: vf._load_wav(src, sample_rate=44100)       # noqa: E731  base.py:141-146, staged
+            restore = lambda wav, mode: vf.restore_inmem(wav, cuda=cuda, mode=mode)     # noqa: E731
+        run_jobs(jobs, load=load, restore=restore,
                  save=lambda out, dst: wavio.save_wave(out, fname=dst, sample_rate=44100), say=say)
     elif jobs:
-        vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda,
+        kw = {"channels": channels} if channels != "mix" else {}        # "mix" is restore_files' default
+        vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda, **kw,
                          _on_wave=lambda ids: [say("Processing {}, mode={}".format(jobs[i][0], jobs[i][2])) for i in ids],
                          _on_wave_done=lambda ids, s: print("Restoration took {} s".format(round(s, 1))))
 
@@ -188,7 +196,8 @@ def main(argv=None):
     vf = VoiceFixer()
     say("Start processing %d job(s)." % len(jobs))
     t0 = time.time()
-    execute(vf, jobs, batch=args.batch, cuda=not args.disable_cuda, say=say)
+    execute(vf, jobs, batch=args.batch, cuda=not args.disable_cuda, say=say,
+            channels="keep" if args.keep_channels else "mix")
     say("Done: {} job(s) in {} s".format(len(jobs), round(time.time() - t0, 3)))
     return 0
 

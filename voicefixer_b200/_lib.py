@@ -12,6 +12,7 @@ VFX_OK = 0
 PREC = {"fp32": 0, "bf16": 1, "tf32": 2, "fp16": 3}
 ACT = {"none": 0, "lrelu": 1, "elu": 2, "lrelu_xsinx": 3, "sigmoid": 4}
 PAIR_FORM = {"fused": 0, "blocked": 1}
+PCM16_MAX_CHANNELS = 8                 # VFX_PCM16_MAX_CHANNELS
 
 _c = ctypes
 _vp, _i, _f, _sz, _ll = _c.c_void_p, _c.c_int, _c.c_float, _c.c_size_t, _c.c_longlong
@@ -60,6 +61,11 @@ class ScatterItem(ctypes.Structure):
     _fields_ = [("dst", _vp), ("dst_elems", _ll), ("dst_off", _ll), ("len", _i), ("src_off", _i)]
 
 
+class Pcm16Item(ctypes.Structure):
+    """struct vfx_pcm16_item (include/vfx_b200.h)."""
+    _fields_ = [("rows", _vp * PCM16_MAX_CHANNELS), ("n", _ll), ("dst_off", _ll), ("C", _i)]
+
+
 # name -> (restype, argtypes); must list every symbol include/vfx_b200.h declares
 SIGNATURES = {
     "vfx_last_error": (_c.c_char_p, []),
@@ -104,6 +110,8 @@ SIGNATURES = {
     "vfx_resample_src_workspace_bytes": (_sz, [_i]),
     "vfx_scatter_rows": (_i, [_vp, _i, _ll, _c.POINTER(ScatterItem), _vp, _sz, _vp]),
     "vfx_scatter_rows_workspace_bytes": (_sz, [_i]),
+    "vfx_pack_pcm16": (_i, [_c.POINTER(Pcm16Item), _i, _vp, _ll, _vp, _sz, _vp]),
+    "vfx_pack_pcm16_workspace_bytes": (_sz, [_i]),
     "vfx_bn_stats": (_i, [_vp, _ll, _ll, _i, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "vfx_bn_act": (_i, [_i, _vp, _ll, _ll, _i, _ll, _i, _vp, _vp, _i, _i, _i, _f, _vp, _ll, _ll, _vp]),
     "vfx_dropout_apply": (_i, [_vp, _vp, _ll, _vp]),

@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from .engine import Engine, default_precision
+from ._lib import PCM16_MAX_CHANNELS
 from . import resample, wavio
 
 SEG_LENGTH = 44100 * 30                      # voicefixer/base.py:116
@@ -140,6 +141,20 @@ def plan_waves(lengths, budget):
         total += int(n)
     if wave:
         yield wave
+
+
+def file_samples(shape, sr, mode, src):
+    """The samples a file counts against VoiceFixer.restore_files' wave budget (plan_waves): its length at 44.1 kHz
+    times the channels restored, shape being the decoded file's, (L,) for a mono mix or (L, C) with every channel kept.
+    Raises ValueError naming src for what restore_many would refuse (plan_many) and for more than PCM16_MAX_CHANNELS
+    channels, the most one file of the device packer (Engine.pack_pcm16) and one FLAC stream hold."""
+    C = shape[1] if len(shape) == 2 else 1
+    if C > PCM16_MAX_CHANNELS:
+        raise ValueError(f"restore_files: {src} has {C} channels; channels=\"keep\" restores at most "
+                         f"{PCM16_MAX_CHANNELS} per file (the device packer's bound, and the most a FLAC stream holds)")
+    n44 = resample.out_len(shape[0], sr)
+    plan_many([n44], mode, lambda L: 1, what=f"restore_files: {src}")             # restore_many's refusals
+    return n44 * C
 
 
 def run_waves(srcs, budget, load, restore, write, depth=2):
@@ -1021,11 +1036,21 @@ def prefilter_bytes(eng, L):
     return eng.hf_cut_workspace_bytes(2, L) - eng.hf_cut_workspace_bytes(1, L) + 4 * L
 
 
-def drop_key_rows(segs, seeds):
+def check_channels(channels, who):
+    """Refuses a channels argument other than "mix" (the mono mix, as the reference reads files) or "keep" (every
+    channel restored on its own)."""
+    if not isinstance(channels, str) or channels not in ("mix", "keep"):
+        raise ValueError(f'{who}: channels is {channels!r}; it must be "mix" or "keep"')
+
+
+def drop_key_rows(segs, seeds, bases=None):
     """The seeded dropout keys of a batch (vfx_drop_key): segs = [(recording, a, b), ...] (plan_many's segments, a the
-    first sample of a 30 s segment), seeds one per recording -> uint64 (B, 2) rows (seed of the recording, a // SEG_LENGTH):
-    segment k of a recording draws its masks from stream k of its seed, whatever batch it runs in."""
-    return np.array([(seeds[i], a // SEG_LENGTH) for i, a, _ in segs], dtype=np.uint64).reshape(-1, 2)
+    first sample of a 30 s segment), seeds one per recording -> uint64 (B, 2) rows (seed of the recording,
+    base of the recording + a // SEG_LENGTH): segment k of a recording draws its masks from stream base + k of its seed,
+    whatever batch it runs in.  bases: one stream base per recording, 0 for each without it (restore_files gives
+    channel c of a file the base c << 32, so that the channels of one file never share masks)."""
+    return np.array([(seeds[i], (int(bases[i]) if bases is not None else 0) + a // SEG_LENGTH) for i, a, _ in segs],
+                    dtype=np.uint64).reshape(-1, 2)
 
 
 def _upload_keys(rows, dev):
@@ -1068,12 +1093,14 @@ def _many_inputs(eng, wavs, sample_rate, mode, drop_masks_fn, dropout_seed, what
     return on_dev, items, rates, seeds, lengths
 
 
-def _segment_batches(eng, items, rates, lengths, mode, drop_masks_fn, seeds, on_dev, what, sizing="restore"):
+def _segment_batches(eng, items, rates, lengths, mode, drop_masks_fn, seeds, on_dev, what, sizing="restore",
+                     bases=None):
     """The batch loop of restore_many and analysis_many: plan_many's batches as (segs, x, lens, masks, keys): the rows
     (mode 1: after the ragged pre-filter) and lengths of the batch's segments on the device, and mode 2's dropout masks
     or seeded keys (None otherwise).  Each batch is sized to the device memory that is free (Engine.max_batch) for
     `sizing`: "restore", a restore; "analysis", analysis_ragged and the batch's two mel tensors; "hook", the same calls
-    sized as a restore, so that the memory the engine's own vocoder would take is left to the caller's vocoder."""
+    sized as a restore, so that the memory the engine's own vocoder would take is left to the caller's vocoder.
+    bases: the recordings' seeded dropout stream bases (drop_key_rows), or None."""
     dev = f"cuda:{eng.device}"
 
     def max_items(L_cap):
@@ -1090,7 +1117,7 @@ def _segment_batches(eng, items, rates, lengths, mode, drop_masks_fn, seeds, on_
             x, _, lens = eng.hf_cut(x, lens=lens)
         masks = keys = None
         if seeds is not None:
-            keys = _upload_keys(drop_key_rows(segs, seeds), dev)
+            keys = _upload_keys(drop_key_rows(segs, seeds, bases), dev)
         elif mode == 2:
             masks = _drop_masks(drop_masks_fn, len(segs), 1 + L_cap // 441)
             if on_dev:
@@ -1248,7 +1275,7 @@ class VoiceFixer:
 
     @torch.no_grad()
     def restore_many(self, wavs, cuda=True, mode=0, drop_masks_fn=None, sample_rate=44100, dropout_seed=None,
-                     your_vocoder_func=None):
+                     your_vocoder_func=None, _stream_base=None):
         """Extension of the reference API: restores a list of 1-D recordings of any lengths, in any mode, and returns a
         list of (1, L_i') arrays, element i what restore_inmem(wavs[i], cuda=True, mode=mode) returns -- bit-identical in
         modes 0 and 1 and in mode 2 with drop_masks_fn=False; in mode 2 with dropout, the same distribution.
@@ -1296,14 +1323,18 @@ class VoiceFixer:
         memory, without a host wait).  Element i depends on recording i and its seed only: it is bit-identical to
         restore_inmem(wavs[i], cuda=True, mode=2, dropout_seed=seed_i) and to restore_many([wavs[i]], mode=2,
         dropout_seed=seed_i)[0], whatever the other recordings, their order, the batch plan, host or CUDA input, or
-        sample_rate.  Recordings given the same seed share their masks segment by segment; distinct seeds avoid that."""
+        sample_rate.  Recordings given the same seed share their masks segment by segment; distinct seeds avoid that.
+
+        Channels: the list takes 1-D recordings.  The channels of a multichannel recording x (L, C) are restored as the
+        columns [x[:, c] for c in range(C)]; for a CUDA tensor those are strided views, read in place without a copy.
+        _stream_base (restore_files' channels): one seeded dropout stream base per recording (drop_key_rows)."""
         _check_cuda(cuda)
         eng = self._engine
         dev = f"cuda:{eng.device}"
         on_dev, items, rates, seeds, lengths = _many_inputs(eng, wavs, sample_rate, mode, drop_masks_fn, dropout_seed,
                                                             "restore_many")
         batches = _segment_batches(eng, items, rates, lengths, mode, drop_masks_fn, seeds, on_dev, "restore_many",
-                                   sizing="restore" if your_vocoder_func is None else "hook")
+                                   sizing="restore" if your_vocoder_func is None else "hook", bases=_stream_base)
         if your_vocoder_func is not None:
             pieces = {}                                                  # (recording, start) -> vocoded segment
             for segs, x, lens, masks, keys in batches:
@@ -1543,37 +1574,61 @@ class VoiceFixer:
         _check_cuda(False)
         return StreamPool(self._engine, chunk_seconds, context_seconds, max_windows, mode=mode)
 
-    def restore(self, input, output, cuda=False, mode=0, your_vocoder_func=None):
-        wav_10k = self._load_wav(input, sample_rate=44100)               # base.py:141-146
-        out_np_wav = self.restore_inmem(wav_10k, cuda=cuda, mode=mode, your_vocoder_func=your_vocoder_func)
+    def restore(self, input, output, cuda=False, mode=0, your_vocoder_func=None, channels="mix"):
+        """base.py:141-146.  channels (extension): "mix" (the default) restores the file's mono mix, as the reference
+        does; "keep" restores each channel on its own and writes them all (restore_columns on wavio.read_wave), so a
+        stereo file stays stereo.  A mono file gives the same output either way."""
+        check_channels(channels, "restore")
+        if channels == "keep":
+            out_np_wav = self.restore_columns(wavio.read_wave(input, 44100), cuda=cuda, mode=mode,
+                                              your_vocoder_func=your_vocoder_func)
+        else:
+            wav_10k = self._load_wav(input, sample_rate=44100)           # base.py:141-146
+            out_np_wav = self.restore_inmem(wav_10k, cuda=cuda, mode=mode, your_vocoder_func=your_vocoder_func)
         wavio.save_wave(out_np_wav, fname=output, sample_rate=44100)
 
+    def restore_columns(self, x, cuda=False, mode=0, your_vocoder_func=None):
+        """Extension: the channels of x (L, C) float32 at 44.1 kHz, each restored on its own by restore_inmem, as a
+        (C, L') array (row c: restore_inmem(x[:, c])[0]), which save_wave writes as C channels."""
+        x = np.asarray(x, dtype=np.float32)
+        if x.ndim != 2 or x.shape[1] < 1:
+            raise ValueError(f"restore_columns takes an (L, C) array, one column per channel; got shape {x.shape}")
+        return np.concatenate([self.restore_inmem(x[:, c], cuda=cuda, mode=mode, your_vocoder_func=your_vocoder_func)
+                               for c in range(x.shape[1])])
+
     @torch.no_grad()
-    def restore_files(self, inputs, outputs, mode=0, cuda=True, dropout_seed=None, _budget=None, _on_wave=None,
-                      _on_wave_done=None):
+    def restore_files(self, inputs, outputs, mode=0, cuda=True, dropout_seed=None, channels="mix", _budget=None,
+                      _on_wave=None, _on_wave_done=None):
         """Extension of the reference API: restore(inputs[i], outputs[i]) for many files, the files batched across each
-        other.  Output file i is byte for byte what restore(inputs[i], outputs[i], mode=mode_i) writes in modes 0 and 1,
-        for .wav and .flac at every rate and channel count the readers take.  In mode 2 with dropout_seed it is what
-        save_wave(restore_inmem(load_mono(inputs[i]), mode=2, dropout_seed=seed_i), outputs[i]) writes; without a seed the
-        masks are random, with restore()'s distribution.
+        other.  Output file i is byte for byte what restore(inputs[i], outputs[i], mode=mode_i, channels=channels) writes
+        in modes 0 and 1, for .wav and .flac at every rate and channel count the readers take.  In mode 2 with
+        dropout_seed it is what save_wave(restore_inmem(load_mono(inputs[i]), mode=2, dropout_seed=seed_i), outputs[i])
+        writes (with channels="keep": channel c restored with masks from the Philox keys (seed_i, (c << 32) | k), k the
+        segment, so channel 0 has the mono call's masks and no two channels share theirs); without a seed the masks are
+        random, with restore()'s distribution.
 
         mode: one of 0, 1, 2 for every file, or one per file (so an input may be listed several times with different
         outputs and modes).  dropout_seed: one int in [0, 2^64) or one per file, as in restore_many; it is the dropout of
-        the files restored in mode 2, and refused when there is none.  A length mismatch, an empty list, a bad mode or a
-        bad seed raises ValueError before anything is read.  Output directories are not created, as with restore().
+        the files restored in mode 2, and refused when there is none.  channels: "mix" (the default) restores each file's
+        mono mix, "keep" each of its channels (at most PCM16_MAX_CHANNELS = 8 per file, the device packer's bound and
+        FLAC's).  A length mismatch, an empty list, a bad mode, seed or channels raises ValueError before anything is
+        read.  Output directories are not created, as with restore().
 
-        The files run in waves of consecutive files (plan_waves), about twice the audio of the largest 30 s batch the
-        free device memory holds, through three stages (run_waves): a reader thread decodes each file at its own rate
-        (wavio.load_mono_native, the next files ahead in a four-thread pool) into pinned memory and checks it as restore_many would; the calling thread uploads the
-        wave, runs one device-resident restore_many(..., sample_rate=) per mode present (an input listed several times
-        in a wave is decoded and uploaded once), queues one copy of all the wave's outputs into pinned memory and an
-        event, and goes on to the next wave without waiting; a writer thread waits for that event and writes each output
-        with wavio.save_wave.  The GPU never waits for the host between waves.
+        The files run in waves of consecutive files (plan_waves, every channel of a file counted), about twice the audio
+        of the largest 30 s batch the free device memory holds, through three stages (run_waves): a reader thread
+        decodes each file at its own rate (wavio.load_mono_native, or wavio.load_native's (L, C) with "keep"; the next
+        files ahead in a four-thread pool) into pinned memory and checks it as restore_many would; the calling thread
+        uploads the wave, runs one device-resident restore_many(..., sample_rate=) per mode present on the files (with
+        "keep", on the columns x[:, c] of each uploaded file, read in place; an input listed several times in a wave is
+        decoded and uploaded once), packs all the wave's outputs into 16-bit PCM on the device (Engine.pack_pcm16, the
+        quantiser of save_wave bit for bit), queues one copy of them into pinned memory and an event, and goes on to the
+        next wave without waiting; a writer thread waits for that event and writes each output with wavio.write_pcm16.
+        The GPU never waits for the host between waves.
 
         Errors: every file before a failing one, in input order, is written and none after it is started; the exception
         is re-raised once the threads have drained.  A file that cannot be read or written raises RuntimeError, and one
-        too short for its mode or at a bad rate ValueError, each naming the file; such a file cuts its wave short, the
-        files before it in that wave still being restored and written.
+        too short for its mode, at a bad rate or (with "keep") with more than 8 channels ValueError, each naming the
+        file; such a file cuts its wave short, the files before it in that wave still being restored and written.
 
         _budget (samples at 44.1 kHz per wave), _on_wave(jobs) (called as a wave starts) and _on_wave_done(jobs,
         seconds) (called as its outputs reach the host, with the GPU time from its upload to its copy back) are for the
@@ -1591,6 +1646,8 @@ class VoiceFixer:
             if isinstance(m, (bool, np.bool_)) or m not in (0, 1, 2):
                 raise ValueError(f"restore_files: file {i} has mode {m!r}; mode must be 0, 1 or 2")
         modes = [int(m) for m in modes]
+        check_channels(channels, "restore_files")
+        keep = channels == "keep"
         seeds = None
         if dropout_seed is not None:
             if 2 not in modes:
@@ -1604,7 +1661,7 @@ class VoiceFixer:
         ahead = {}                                                       # input -> its decode, started ahead of use
 
         def decode(path):
-            x, sr = wavio.load_mono_native(path)
+            x, sr = wavio.load_native(path) if keep else wavio.load_mono_native(path)
             return torch.from_numpy(x).pin_memory(), sr
 
         def load(i, prev):
@@ -1617,10 +1674,7 @@ class VoiceFixer:
                 except Exception as e:
                     raise RuntimeError(f"restore_files: {inputs[i]}: {e}") from e
                 prev = (x, resample.check_rate(sr, f"restore_files: {inputs[i]}"))
-            x, sr = prev
-            n44 = resample.out_len(x.shape[0], sr)
-            plan_many([n44], modes[i], lambda L: 1, what=f"restore_files: {inputs[i]}")     # restore_many's refusals
-            return prev, n44
+            return prev, file_samples(tuple(prev[0].shape), prev[1], modes[i], inputs[i])
 
         def restore(wave):
             ids = [i for i, _ in wave]
@@ -1632,19 +1686,21 @@ class VoiceFixer:
             for _, item in wave:
                 if id(item) not in up:
                     up[id(item)] = item[0].to(dev, non_blocking=True)
-            outs = {}
+            outs = {}                                                    # file -> its restored channels
             for m in sorted(set(modes[i] for i in ids)):
-                run = [(i, item) for i, item in wave if modes[i] == m]
-                ys = self.restore_many([up[id(item)] for _, item in run], cuda=True, mode=m,
-                                       sample_rate=[item[1] for _, item in run],
-                                       dropout_seed=[seeds[i] for i, _ in run] if seeds is not None and m == 2 else None)
-                outs.update((i, y.view(-1)) for (i, _), y in zip(run, ys))
-            flat = torch.cat([outs[i] for i in ids])
-            host = torch.empty(flat.shape, pin_memory=True)
-            host.copy_(flat, non_blocking=True)
+                run = [(i, item, c) for i, item in wave if modes[i] == m
+                       for c in range(up[id(item)].shape[1] if keep else 1)]
+                ys = self.restore_many([up[id(item)][:, c] if keep else up[id(item)] for _, item, c in run], cuda=True,
+                                       mode=m, sample_rate=[item[1] for _, item, _ in run],
+                                       dropout_seed=[seeds[i] for i, _, _ in run] if seeds is not None and m == 2 else None,
+                                       _stream_base=[c << 32 for _, _, c in run])
+                for (i, _, _), y in zip(run, ys):
+                    outs.setdefault(i, []).append(y.view(-1))
+            pcm, offs = eng.pack_pcm16([outs[i] for i in ids])
+            host = torch.empty(pcm.shape, dtype=torch.int16, pin_memory=True)
+            host.copy_(pcm, non_blocking=True)
             done.record()
-            offs = np.cumsum([0] + [outs[i].shape[0] for i in ids])
-            return host, {i: (int(offs[k]), int(offs[k + 1])) for k, i in enumerate(ids)}, start, done
+            return host, {i: (offs[k], offs[k + 1], len(outs[i])) for k, i in enumerate(ids)}, start, done
 
         def write(ids, result):
             host, spans, start, done = result
@@ -1653,9 +1709,9 @@ class VoiceFixer:
                 _on_wave_done(ids, start.elapsed_time(done) / 1e3)
             y = host.numpy()
             for i in ids:
-                a, b = spans[i]
+                a, b, C = spans[i]
                 try:
-                    wavio.save_wave(y[None, a:b], fname=outputs[i], sample_rate=44100)
+                    wavio.write_pcm16(y[a:b].reshape(-1, C), fname=outputs[i], sample_rate=44100)
                 except Exception as e:
                     raise RuntimeError(f"restore_files: {outputs[i]}: {e}") from e
 

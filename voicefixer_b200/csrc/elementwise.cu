@@ -415,6 +415,45 @@ __global__ void __launch_bounds__(256) scatter_rows_kernel(const float* __restri
   if (j < it.len) it.dst[it.dst_off + j] = __ldg(x + (long long)b * ldx + it.src_off + j);
 }
 
+// vfx_pack_pcm16.  A float's key orders as the float does (NaN above +inf), so that one atomicMax per warp gives a
+// file's np.max: the key of a NaN is the largest, and a NaN anywhere makes the maximum NaN.  Key 0 is below every float.
+__device__ __forceinline__ unsigned pcm16_key(float v) {
+  const unsigned u = __float_as_uint(v);
+  return isnan(v) ? 0xFFFFFFFFu : (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// vmax[b] <- the key of file b's maximum over its n * C samples (vmax zeroed before); grid (x, B), frames grid-strided
+__global__ void __launch_bounds__(256) pcm16_max_kernel(const vfx_pcm16_item* __restrict__ items,
+                                                        unsigned* __restrict__ vmax) {
+  const vfx_pcm16_item& it = items[blockIdx.y];
+  unsigned m = 0;
+  for (int c = 0; c < it.C; ++c)
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < it.n; t += (long long)gridDim.x * blockDim.x)
+      m = max(m, pcm16_key(__ldg(it.rows[c] + t)));
+  m = __reduce_max_sync(0xFFFFFFFFu, m);
+  if ((threadIdx.x & 31) == 0 && m != 0) atomicMax(vmax + blockIdx.y, m);
+}
+
+// numpy's float32 -> int16 cast on x86: truncation toward zero to int32 (cvttss2si, whose out-of-range result
+// 0x80000000 covers NaN and +-inf), then the low 16 bits.  cvt.rzi.s32.f32 saturates instead, so that range is explicit.
+__device__ __forceinline__ short pcm16_of(float v) {
+  if (!(v >= -2147483648.f && v < 2147483648.f)) return 0;
+  return (short)(unsigned short)((unsigned)__float2int_rz(v) & 0xFFFFu);
+}
+
+// file b's interleaved y[dst_off + t * C + c] <- its rows[c][t], scaled by 32768 iff its maximum is <= 1
+__global__ void __launch_bounds__(256) pcm16_pack_kernel(const vfx_pcm16_item* __restrict__ items,
+                                                         const unsigned* __restrict__ vmax, short* __restrict__ y) {
+  const vfx_pcm16_item& it = items[blockIdx.y];
+  const bool scale = vmax[blockIdx.y] <= pcm16_key(1.0f);
+  short* out = y + it.dst_off;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < it.n; t += (long long)gridDim.x * blockDim.x)
+    for (int c = 0; c < it.C; ++c) {
+      const float v = __ldg(it.rows[c] + t);
+      out[t * it.C + c] = pcm16_of(scale ? v * 32768.f : v);
+    }
+}
+
 inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
   if (g > 132LL * 32) g = 132LL * 32;      // 32 blocks per SM of an H100 SXM
@@ -604,6 +643,18 @@ int scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* i
               "scatter_rows: bad arguments (B %d, ldx %lld, max_len %d; B <= 65535)", B, ldx, max_len);
   dim3 grid(ceil_div(max_len, 256), B);
   scatter_rows_kernel<<<grid, 256, 0, st>>>(x, ldx, items);
+  VFX_LAUNCH_CHECK();
+  return VFX_OK;
+}
+
+int pack_pcm16(const vfx_pcm16_item* items, int B, long long max_n, unsigned* vmax, short* y, cudaStream_t st) {
+  VFX_REQUIRE(items && vmax && y && B > 0 && B <= 65535 && max_n > 0,
+              "pack_pcm16: bad arguments (B %d, max_n %lld; B <= 65535)", B, max_n);
+  VFX_CUDA_CHECK(cudaMemsetAsync(vmax, 0, sizeof(unsigned) * B, st));
+  dim3 grid(ceil_div(std::min(max_n, 1024LL * 256), 256), B);
+  pcm16_max_kernel<<<grid, 256, 0, st>>>(items, vmax);
+  VFX_LAUNCH_CHECK();
+  pcm16_pack_kernel<<<grid, 256, 0, st>>>(items, vmax, y);
   VFX_LAUNCH_CHECK();
   return VFX_OK;
 }

@@ -894,6 +894,40 @@ int check_scatter_items(const vfx_scatter_item* items, int B, long long ldx, int
   return VFX_OK;
 }
 
+// vfx_pack_pcm16: the item table and the per-file maxima are staged into the workspace, then two launches
+int pack_pcm16_forward(Ctx& c, const vfx_pcm16_item* items_host, int B, short* y, long long max_n) {
+  vfx_pcm16_item* items = c.ws->alloc<vfx_pcm16_item>(B);
+  unsigned* vmax = c.ws->alloc<unsigned>(B);
+  if (c.dry) return VFX_OK;
+  VFX_CUDA_CHECK(cudaMemcpyAsync(items, items_host, sizeof(vfx_pcm16_item) * B, cudaMemcpyHostToDevice, c.st));
+  return pack_pcm16(items, B, max_n, vmax, y, c.st);
+}
+
+// The items of vfx_pack_pcm16 (include/vfx_b200.h): each on its own, then no two destination ranges overlapping.
+// Sets *max_n to the longest item.
+int check_pcm16_items(const vfx_pcm16_item* items, int B, long long y_elems, long long* max_n) {
+  std::vector<std::pair<long long, int>> ranges;        // (first element, item) of each destination range
+  *max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    const vfx_pcm16_item& it = items[b];
+    VFX_REQUIRE(it.C >= 1 && it.C <= VFX_PCM16_MAX_CHANNELS, "pack_pcm16: item %d: %d channels (1 .. %d are packed)", b,
+                it.C, VFX_PCM16_MAX_CHANNELS);
+    for (int ch = 0; ch < it.C; ++ch) VFX_REQUIRE(it.rows[ch], "pack_pcm16: item %d: channel %d's row is null", b, ch);
+    VFX_REQUIRE(it.n >= 1 && it.n <= (1LL << 40), "pack_pcm16: item %d: length %lld is not in [1, 2^40]", b, it.n);
+    VFX_REQUIRE(it.dst_off >= 0 && it.dst_off <= y_elems - it.n * it.C, "pack_pcm16: item %d: destination [%lld, %lld) "
+                "is not inside the %lld given", b, it.dst_off, it.dst_off + it.n * it.C, y_elems);
+    ranges.push_back({it.dst_off, b});
+    *max_n = std::max(*max_n, it.n);
+  }
+  std::sort(ranges.begin(), ranges.end());
+  for (size_t k = 1; k < ranges.size(); ++k) {
+    const vfx_pcm16_item& p = items[ranges[k - 1].second];
+    VFX_REQUIRE(ranges[k - 1].first + p.n * p.C <= ranges[k].first, "pack_pcm16: item %d: its destination overlaps "
+                "item %d's", ranges[k].second, ranges[k - 1].second);
+  }
+  return VFX_OK;
+}
+
 // Vocoder.oracle's mel basis: librosa.filters.mel(sr=44100, n_fft=2048, n_mels=128, fmin=0, fmax=22050, htk=True) with
 // its default norm="slaney" (vocoder/model/util.py:115-123), built in float64 as librosa builds it and cast to float32
 // (wavio.slaney_htk_mel_basis is the same formula on the host).  band: start[128] ++ len[128] of each row's non-zeros.
@@ -1422,6 +1456,24 @@ int vfx_scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_ite
   if (max_len == 0) return VFX_OK;
   return planned_call(nullptr, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
                       [&](Ctx& c) { return scatter_rows_forward(c, x, B, ldx, items_host, max_len); });
+}
+
+size_t vfx_pack_pcm16_workspace_bytes(int B) {
+  if (B <= 0) return 0;
+  int rc;
+  const size_t peak = dry_peak(nullptr, VFX_MODE_EVAL, [&](Ctx& c) {
+    return pack_pcm16_forward(c, nullptr, B, nullptr, 1);
+  }, &rc);
+  return rc == VFX_OK ? peak : 0;
+}
+
+int vfx_pack_pcm16(const vfx_pcm16_item* items_host, int B, short* y, long long y_elems, void* workspace,
+                   size_t workspace_bytes, void* stream) {
+  VFX_REQUIRE(items_host && y && B > 0 && B <= 65535 && y_elems > 0 && workspace, "pack_pcm16: bad arguments");
+  long long max_n;
+  VFX_TRY(check_pcm16_items(items_host, B, y_elems, &max_n));
+  return planned_call(nullptr, VFX_MODE_EVAL, workspace, workspace_bytes, stream,
+                      [&](Ctx& c) { return pack_pcm16_forward(c, items_host, B, y, max_n); });
 }
 
 int vfx_conv_gemm(int precision, int impl, const vfx_conv_desc* d, void* stream) {

@@ -183,5 +183,8 @@ int resample_src(const float* h, const vfx_resample_src_item* items, int B, int 
 // row b of x[B][ldx] -> items[b]'s destination (items: the device copy of a table vfx_scatter_rows has validated);
 // max_len: the longest item
 int scatter_rows(const float* x, int B, long long ldx, const vfx_scatter_item* items, int max_len, cudaStream_t st);
+// vfx_pack_pcm16's two launches (items: the device copy of a table vfx_pack_pcm16 has validated; vmax[B]: scratch for
+// the per-file maxima); max_n: the most frames (n) of any item
+int pack_pcm16(const vfx_pcm16_item* items, int B, long long max_n, unsigned* vmax, short* y, cudaStream_t st);
 
 }  // namespace vfx

@@ -572,6 +572,46 @@ class Engine(_WorkspaceQueries):
         _lib.check(self.lib.vfx_scatter_rows(_ptr(x), B, x.stride(0), table, _ptr(ws), ws.numel(), _stream()),
                    "vfx_scatter_rows")
 
+    @staticmethod
+    def pack_pcm16_workspace_bytes(B):
+        """Workspace of pack_pcm16() on B files (vfx_pack_pcm16_workspace_bytes; no engine needed)."""
+        return int(_lib.load().vfx_pack_pcm16_workspace_bytes(int(B)))
+
+    def pack_pcm16(self, files, y=None):
+        """16-bit PCM of many files in one call (vfx_pack_pcm16): files is a list of lists of channels, each channel a
+        float32 CUDA tensor on this device with n_i elements (contiguous), the same n_i for every channel of file i, 1 to
+        PCM16_MAX_CHANNELS channels.  Returns (y, offsets): y an int16 CUDA tensor holding file i's interleaved (n_i, C_i)
+        samples at y[offsets[i]:offsets[i + 1]], each file quantised as wavio.pcm16 quantises its (C_i, n_i) array, bit
+        for bit.  y (optional): a contiguous int16 CUDA tensor of exactly sum n_i * C_i elements to write into."""
+        dev = torch.device(f"cuda:{self.device}")
+        B = len(files)
+        if B == 0:
+            raise ValueError("pack_pcm16 takes a non-empty list of files")
+        table, offs = (_lib.Pcm16Item * B)(), [0]
+        for b, rows in enumerate(files):
+            rows = list(rows)
+            if not 1 <= len(rows) <= _lib.PCM16_MAX_CHANNELS:
+                raise ValueError(f"pack_pcm16: file {b} has {len(rows)} channels; 1 .. {_lib.PCM16_MAX_CHANNELS} are packed")
+            n = rows[0].numel()
+            for r in rows:
+                if not (r.is_cuda and r.device == dev and r.dtype == torch.float32 and r.is_contiguous()
+                        and r.numel() == n):
+                    raise ValueError(f"pack_pcm16: file {b}: every channel must be a contiguous float32 tensor on {dev} "
+                                     f"of the same length")
+            t = table[b]
+            for c, r in enumerate(rows):
+                t.rows[c] = r.data_ptr()
+            t.n, t.dst_off, t.C = n, offs[-1], len(rows)
+            offs.append(offs[-1] + n * len(rows))
+        if y is None:
+            y = torch.empty(offs[-1], dtype=torch.int16, device=dev)
+        elif not (y.is_cuda and y.device == dev and y.dtype == torch.int16 and y.is_contiguous() and y.numel() == offs[-1]):
+            raise ValueError(f"pack_pcm16: y must be a contiguous int16 tensor of {offs[-1]} elements on {dev}")
+        ws = self._workspace(self.pack_pcm16_workspace_bytes(B))
+        _lib.check(self.lib.vfx_pack_pcm16(table, B, _ptr(y), y.numel(), _ptr(ws), ws.numel(), _stream()),
+                   "vfx_pack_pcm16")
+        return y, offs
+
     def hf_cut(self, wav, ratio=0.95, lens=None, out=None, lens_out=None, ws=None):
         """Mode-1 pre-filter: wav (B, L) -> (out (B, 512 * (L // 512)), cut bins (B,)).
 

@@ -81,9 +81,14 @@ def _resample(x, sr_in, sr_out):
     return resample_poly(x, sr_out // g, sr_in // g, axis=0).astype(np.float32)
 
 
+def load_native(path):
+    """(x, sr): the file's samples as float32 (L, C), one column per channel, at its own rate sr."""
+    return _read_pcm(path)
+
+
 def load_mono_native(path):
     """(x, sr): the file's mono mix (mean over channels), float32, at its own rate sr."""
-    x, sr = _read_pcm(path)
+    x, sr = load_native(path)
     return x.mean(axis=1).astype(np.float32), sr
 
 
@@ -98,9 +103,11 @@ def read_wave(path, sample_rate):
     return _resample(x, sr, sample_rate)
 
 
-def save_wave(frames, fname, sample_rate=44100):
-    """tools/wav.py:9-37 semantics: float frames with max <= 1 are scaled by 2^15, then cast to
-    int16 with C truncation toward zero; (1, N) or (1, 1, N) arrays are written as mono."""
+def pcm16(frames):
+    """tools/wav.py:9-37's quantiser: float frames -> int16 (L, C).  A last axis of 3 or more is the samples axis
+    ((C, L) and (1, C, L) arrays are transposed); float32 frames with max <= 1 over every sample (NaN: not <= 1) are
+    scaled by 2^15, float16 / float64 frames always; then cast to int16 as C truncates on x86 (toward zero, to int32,
+    the low 16 bits kept; 0 outside int32's range).  (1, N) or (1, 1, N) arrays give one channel."""
     frames = np.array(frames, copy=True)
     shape = list(frames.shape)
     if len(shape) == 1:
@@ -119,16 +126,27 @@ def save_wave(frames, fname, sample_rate=44100):
         frames = frames[0, ...]
     if frames.ndim == 1:
         frames = frames[:, None]
+    return frames
+
+
+def write_pcm16(pcm, fname, sample_rate=44100):
+    """Writes int16 (L, C) samples to fname: FLAC for a .flac name (at most 8 channels), WAV otherwise."""
     if str(fname).lower().endswith(".flac"):         # soundfile.write picks the container from the extension
         from . import _hostio
         with open(str(fname), "wb") as f:
-            f.write(_hostio.flac_encode_int16(frames, sample_rate))
+            f.write(_hostio.flac_encode_int16(pcm, sample_rate))
         return
     with wave.open(str(fname), "wb") as f:
-        f.setnchannels(frames.shape[1])
+        f.setnchannels(pcm.shape[1])
         f.setsampwidth(2)
         f.setframerate(sample_rate)
-        f.writeframes(np.ascontiguousarray(frames, dtype="<i2").tobytes())
+        f.writeframes(np.ascontiguousarray(pcm, dtype="<i2").tobytes())
+
+
+def save_wave(frames, fname, sample_rate=44100):
+    """tools/wav.py:9-37 semantics: write_pcm16(pcm16(frames)); (1, N) or (1, 1, N) arrays are written as mono, (C, N)
+    arrays (N >= 3) as C channels."""
+    write_pcm16(pcm16(frames), fname, sample_rate)
 
 
 _MEL_BASIS = None
