@@ -1,14 +1,15 @@
 """Command line mirror of the reference's `voicefixer` entry point (voicefixer/__main__.py:13-219):
 
     python -m voicefixer_b200 --infile in.wav --outfile out.wav [--mode 0|1|2|all]
-    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...] [--batch] [--keep-channels]
+    python -m voicefixer_b200 --infolder wavs/ --outfolder restored/ [--mode ...] [--batch] [--keep-channels] [--gpus N]
 
 Same flags, same output naming (`--mode all` writes `<name>-mode<k><ext>` for k = 0,1,2), same
 `.wav`-only input rule, same messages.  The work is planned first (`plan_jobs`, a pure function) and
 then executed with one VoiceFixer instance as a reader -> GPU -> writer pipeline (`run_jobs`), one
 file at a time; with `--batch` the same jobs run through `VoiceFixer.restore_files`, many files per
 batch (`execute`).  With `--keep-channels` every channel of a file is restored and written (restore(...,
-channels="keep")), on either path, with the same bytes."""
+channels="keep")), on either path, with the same bytes.  With `--gpus N` (N > 1) the jobs run as with `--batch`,
+spread over N GPUs by `VoiceFixer.restore_files(..., gpus=N)`, again with the same bytes."""
 import argparse
 import os
 import re
@@ -39,6 +40,8 @@ def build_parser():
                    help="Restore many files at once (VoiceFixer.restore_files): the same outputs, batched across files.")
     p.add_argument("--keep-channels", default=False, action="store_true",
                    help="Restore every channel of a multichannel file and write them all, instead of its mono mix.")
+    p.add_argument("--gpus", type=int, default=1,
+                   help="Spread the files over this many GPUs, one process each (as --batch, with the same outputs).")
     return p
 
 
@@ -155,12 +158,17 @@ def run_jobs(jobs, load, restore, save, say=print, depth=2):
     return took
 
 
-def execute(vf, jobs, batch=False, cuda=True, say=print, channels="mix"):
+def execute(vf, jobs, batch=False, cuda=True, say=print, channels="mix", gpus=1):
     """Runs [(src, dst, mode)] with the VoiceFixer vf: one file at a time through run_jobs, or with batch through
     vf.restore_files, which prints the same `Processing` line per job as its wave starts and one `Restoration took`
-    line per wave.  channels: restore()'s ("mix" or "keep")."""
+    line per wave.  channels: restore()'s ("mix" or "keep").  gpus > 1 runs the jobs through
+    vf.restore_files(..., gpus=gpus) whatever batch is; each device then prints its own lines, the `Processing` ones
+    only when say is print, and lines from different devices interleave."""
     from . import wavio
-    if not batch:
+    if gpus != 1 and jobs:
+        vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda,
+                         channels=channels, gpus=gpus, _messages=("processing", "took") if say is print else ("took",))
+    elif not batch:
         if channels == "keep":                                            # = vf.restore(..., channels="keep") per job
             load = lambda src: wavio.read_wave(src, 44100)                # noqa: E731
             restore = lambda wav, mode: vf.restore_columns(wav, cuda=cuda, mode=mode)   # noqa: E731
@@ -197,7 +205,7 @@ def main(argv=None):
     say("Start processing %d job(s)." % len(jobs))
     t0 = time.time()
     execute(vf, jobs, batch=args.batch, cuda=not args.disable_cuda, say=say,
-            channels="keep" if args.keep_channels else "mix")
+            channels="keep" if args.keep_channels else "mix", gpus=args.gpus)
     say("Done: {} job(s) in {} s".format(len(jobs), round(time.time() - t0, 3)))
     return 0
 

@@ -169,7 +169,9 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
     At most `depth` loaded and `depth` restored waves are in flight.  Errors follow run_jobs's order rule: a failing load
     cuts its wave short (the jobs before it in the wave are restored and written), a failing restore fails its wave,
     every job before the failure is written and nothing after it is started, and the exception is re-raised once the
-    threads have drained.  Returns the number of waves restored."""
+    threads have drained.  The exception's `vfx_job` attribute is then the job it stopped at: the one whose load failed,
+    the first of a failed wave, or for a failed write the job write set it to (else the wave's first).  Returns the
+    number of waves restored."""
     import queue
     import threading
     loaded, finished = queue.Queue(maxsize=depth), queue.Queue(maxsize=depth)
@@ -177,11 +179,13 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
 
     def reader():
         pending = {}                                     # job -> item: loaded and not yet handed on
+        at = [0]                                         # the job being loaded
 
         def lengths():
             for i, src in enumerate(srcs):
                 if stop.is_set():
                     return
+                at[0] = i
                 prev = next((pending[j] for j in pending if srcs[j] == src), None)
                 pending[i], n = load(i, prev)
                 yield n
@@ -192,7 +196,7 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
         except BaseException as e:                       # noqa: BLE001 - re-raised by the caller's thread
             if pending:                                  # the jobs before the failing one
                 loaded.put(sorted(pending.items()))
-            loaded.put(e)
+            loaded.put(_stopped_at(e, at[0]))
         finally:
             loaded.put(None)
 
@@ -206,7 +210,7 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
             try:
                 write(*item)
             except BaseException as e:                   # noqa: BLE001
-                write_errors.append(e)
+                write_errors.append(_stopped_at(e, item[0][0]))
                 stop.set()
 
     threads = [threading.Thread(target=reader, name="vfx-wave-reader", daemon=True),
@@ -228,7 +232,7 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
             try:
                 result = restore(item)
             except BaseException as e:                   # noqa: BLE001
-                failure = e
+                failure = _stopped_at(e, item[0][0])
                 stop.set()
                 continue
             waves += 1
@@ -242,6 +246,85 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
     if failure is not None:
         raise failure
     return waves
+
+
+def _stopped_at(e, job):
+    """e, with `vfx_job` (the job run_waves stopped at) set to job unless a stage closer to the failure set it."""
+    if getattr(e, "vfx_job", None) is None:
+        e.vfx_job = job
+    return e
+
+
+def plan_devices(weights, sources, n):
+    """The files of VoiceFixer.restore_files(..., gpus=n) per device: n lists of indices into weights (each file's
+    samples against a wave, file_samples' count; 0 for a file that cannot be probed) that together hold every index
+    once, each in input order.  Every occurrence of one source (an input listed several times, as --mode all does) goes
+    to one device, so that it is decoded once; these groups are placed longest first, each on the least-loaded device
+    (ties: the lower index), so the largest load is at most the largest group's weight plus the mean load.  A device
+    gets no files when there are fewer groups than devices."""
+    groups = {}
+    for i, src in enumerate(sources):
+        groups.setdefault(src, []).append(i)
+    groups = sorted(groups.values(), key=lambda g: (-sum(int(weights[i]) for i in g), g[0]))
+    loads, shards = [0] * n, [[] for _ in range(n)]
+    for g in groups:
+        d = min(range(n), key=lambda k: (loads[k], k))
+        shards[d] += g
+        loads[d] += sum(int(weights[i]) for i in g)
+    return [sorted(s) for s in shards]
+
+
+def _probe_samples(inputs, modes, keep):
+    """plan_devices' weights: file_samples' count for each input from its headers (wavio.probe), 0 where that fails."""
+    probed, weights = {}, []
+    for src, m in zip(inputs, modes):
+        try:
+            if src not in probed:
+                probed[src] = wavio.probe(src)
+            frames, ch, sr = probed[src]
+            weights.append(file_samples((frames, ch) if keep else (frames,), sr, m, src))
+        except Exception:                                 # noqa: BLE001 - its error surfaces on its device, as today
+            weights.append(0)
+    return weights
+
+
+class _ShardArgs:
+    """What every device's shard of restore_files(..., gpus=N) shares: the caller's VoiceFixer (vf, which stays in the
+    calling process: a worker receives None and builds its own), the engine's precision, weight layout and arena in
+    host shared memory, and the call's arguments over all files."""
+
+    def __init__(self, vf, **kw):
+        self.vf = vf
+        self.__dict__.update(kw)
+
+    def __getstate__(self):
+        return dict(self.__dict__, vf=None)
+
+
+def _restore_shard(device, shard, args):
+    """parallel.run_on_devices' target for restore_files(..., gpus=N): restores the files `shard` (indices into the
+    call's lists) on device with the single-device restore_files, on the caller's VoiceFixer in the calling process and
+    on one around the shared weights in a worker.  Returns None, or (the index of the file it stopped at, the error)."""
+    vf = args.vf
+    if vf is None:
+        torch.cuda.set_device(device)
+        eng = Engine(device=device, precision=args.precision)
+        eng.attach(args.arena.to(f"cuda:{device}"), args.table)
+        vf = VoiceFixer.from_engine(eng)
+    modes = [args.modes[i] for i in shard]
+    seeds = [args.seeds[i] for i in shard] if args.seeds is not None and 2 in modes else None
+    kw = {}
+    if "processing" in args.messages:
+        kw["_on_wave"] = lambda ids: [print(f"Processing {args.inputs[shard[i]]}, mode={modes[i]}", flush=True)
+                                      for i in ids]
+    if "took" in args.messages:
+        kw["_on_wave_done"] = lambda ids, s: print("Restoration took {} s".format(round(s, 1)), flush=True)
+    try:
+        vf.restore_files([args.inputs[i] for i in shard], [args.outputs[i] for i in shard], mode=modes,
+                         dropout_seed=seeds, channels=args.channels, _budget=args.budget, **kw)
+    except Exception as e:                               # noqa: BLE001 - reported by run_on_devices
+        return shard[getattr(e, "vfx_job", None) or 0], e
+    return None
 
 
 def plan_vocoder_many(items, kind, max_items, pack_lengths=None):
@@ -1597,8 +1680,8 @@ class VoiceFixer:
                                for c in range(x.shape[1])])
 
     @torch.no_grad()
-    def restore_files(self, inputs, outputs, mode=0, cuda=True, dropout_seed=None, channels="mix", _budget=None,
-                      _on_wave=None, _on_wave_done=None):
+    def restore_files(self, inputs, outputs, mode=0, cuda=True, dropout_seed=None, channels="mix", gpus=None,
+                      _budget=None, _on_wave=None, _on_wave_done=None, _messages=(), _devices=None):
         """Extension of the reference API: restore(inputs[i], outputs[i]) for many files, the files batched across each
         other.  Output file i is byte for byte what restore(inputs[i], outputs[i], mode=mode_i, channels=channels) writes
         in modes 0 and 1, for .wav and .flac at every rate and channel count the readers take.  In mode 2 with
@@ -1630,9 +1713,52 @@ class VoiceFixer:
         too short for its mode, at a bad rate or (with "keep") with more than 8 channels ValueError, each naming the
         file; such a file cuts its wave short, the files before it in that wave still being restored and written.
 
+        gpus: None or 1 runs everything on this instance's device, as above.  gpus=N (an int, at most
+        torch.cuda.device_count()) spreads the files over N devices: this instance's and the next N - 1 visible ones in
+        index order (wrapping past the last).  Each file is sized from its headers (wavio.probe) and the files are
+        assigned by plan_devices, every occurrence of one input on one device.  One worker process per extra device,
+        started with the spawn method, receives the engine's weights through host shared memory (one copy of its arena
+        from the device, no checkpoint read, so an instance made by from_engine works too), builds an Engine of the same
+        precision on its device and restores its files with the single-device restore_files, its own wave budget and
+        its files' modes and seeds; this instance restores its own device's files meanwhile.  Every output is the same
+        file, byte for byte, as with one device.  Errors: within a device the rule above holds; the other devices go on
+        to finish their own files, and once every device has finished the call raises the error of the lowest-indexed
+        file that failed, with its type and message (a later file on another device may then have been written, the
+        one difference from gpus=1).  A worker that dies raises RuntimeError naming its device.  Every worker process
+        has exited when the call returns or raises.  As with DataLoader workers, a script that calls this with gpus > 1
+        must guard its entry point with `if __name__ == "__main__":`, since the spawned workers import it.
+
         _budget (samples at 44.1 kHz per wave), _on_wave(jobs) (called as a wave starts) and _on_wave_done(jobs,
         seconds) (called as its outputs reach the host, with the GPU time from its upload to its copy back) are for the
-        command line and the tests."""
+        command line and the tests; with gpus > 1 the callbacks cannot reach the workers, so _messages names the
+        command line's lines each device prints itself ("processing", "took").  _devices (the tests') overrides the
+        devices gpus > 1 runs on, e.g. [0, 0] for two processes on one device."""
+        inputs, outputs, modes, seeds, keep = self._check_files(inputs, outputs, mode, cuda, dropout_seed, channels)
+        if gpus is not None:
+            if isinstance(gpus, (bool, np.bool_)) or not isinstance(gpus, numbers.Integral) or gpus < 1:
+                raise ValueError(f"restore_files: gpus is {gpus!r}; it must be a positive int")
+            if _devices is None and gpus > torch.cuda.device_count():
+                raise ValueError(f"restore_files: gpus={gpus}, but {torch.cuda.device_count()} CUDA device(s) are "
+                                 "visible")
+        if (gpus is None or gpus == 1) and _devices is None:
+            return self._restore_files(inputs, outputs, modes, seeds, keep, _budget, _on_wave, _on_wave_done)
+        if _on_wave is not None or _on_wave_done is not None:
+            raise ValueError("restore_files: _on_wave / _on_wave_done run in one process; with gpus > 1 use _messages")
+        eng = self._engine
+        devices = list(_devices) if _devices is not None else \
+            [(eng.device + k) % torch.cuda.device_count() for k in range(int(gpus))]
+        shards = plan_devices(_probe_samples(inputs, modes, keep), inputs, len(devices))
+        arena = torch.empty(eng.arena.numel(), dtype=torch.uint8).share_memory_()
+        arena.copy_(eng.arena)
+        args = _ShardArgs(self, inputs=inputs, outputs=outputs, modes=modes, seeds=seeds,
+                          channels="keep" if keep else "mix", budget=_budget, messages=tuple(_messages),
+                          precision=eng.precision, table=eng.table, arena=arena)
+        from .parallel import run_on_devices
+        run_on_devices([(d, s) for d, s in zip(devices, shards) if s], _restore_shard, args)
+
+    def _check_files(self, inputs, outputs, mode, cuda, dropout_seed, channels):
+        """restore_files' argument checks: (inputs, outputs, modes, seeds, keep) as lists of one entry per file (seeds
+        None without dropout_seed), or ValueError before anything is read."""
         _check_cuda(cuda)
         inputs, outputs = [str(p) for p in inputs], [str(p) for p in outputs]
         n = len(inputs)
@@ -1653,6 +1779,11 @@ class VoiceFixer:
             if 2 not in modes:
                 raise ValueError("restore_files: dropout_seed is mode 2's dropout; no file is restored in mode 2")
             seeds = dropout_seeds(dropout_seed, 2, None, n, "restore_files")
+        return inputs, outputs, modes, seeds, keep
+
+    def _restore_files(self, inputs, outputs, modes, seeds, keep, _budget, _on_wave, _on_wave_done):
+        """restore_files on this instance's device, on checked arguments (_check_files)."""
+        n = len(inputs)
         eng = self._engine
         dev = f"cuda:{eng.device}"
         budget = _budget if _budget is not None else 2 * eng.max_batch(SEG_LENGTH) * SEG_LENGTH
@@ -1713,7 +1844,7 @@ class VoiceFixer:
                 try:
                     wavio.write_pcm16(y[a:b].reshape(-1, C), fname=outputs[i], sample_rate=44100)
                 except Exception as e:
-                    raise RuntimeError(f"restore_files: {outputs[i]}: {e}") from e
+                    raise _stopped_at(RuntimeError(f"restore_files: {outputs[i]}: {e}"), i) from e
 
         try:
             run_waves(inputs, budget, load, restore, write)

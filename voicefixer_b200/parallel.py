@@ -4,7 +4,10 @@ Exactly two collectives, as the north star prescribes: one broadcast of the pack
 from rank 0 at start-up and a gather of the output waveforms to rank 0 per step.  Shard sizes are
 static for a job, so they are exchanged ONCE when a `WaveformGather` is built (start-up, like the
 weight broadcast) and never in the step.  The functions take the process group's backend as given,
-so the same code runs under NCCL on the GPUs and under gloo on CPU tensors in the tests (world_size 2)."""
+so the same code runs under NCCL on the GPUs and under gloo on CPU tensors in the tests (world_size 2).
+
+`run_on_devices` is the other form, with no process group: the caller spawns one worker process per extra device and
+each runs a shard of independent jobs (VoiceFixer.restore_files(..., gpus=N)), reporting only its outcome back."""
 import os
 import torch
 import torch.distributed as dist
@@ -97,3 +100,87 @@ class WaveformGather:
 def gather_waveforms(local_out, dst=0):
     """One-shot convenience form (builds a WaveformGather for this call: the size exchange is then part of it)."""
     return WaveformGather(local_out.shape[0], local_out.shape[1], local_out.dtype, local_out.device, dst)(local_out)
+
+
+def _outcome(target, device, shard, args):
+    """target's outcome on one shard: None when it is done, else (input index, exception type, message, exception).
+    target returns None or (the input index it failed on, the exception); an exception it raises itself counts as a
+    failure at the shard's first input."""
+    try:
+        failed = target(device, shard, args)
+    except Exception as e:                               # noqa: BLE001 - reported to the caller
+        failed = (shard[0], e)
+    if failed is None:
+        return None
+    index, e = failed
+    return int(index), type(e), str(e), e
+
+
+def _worker(target, device, shard, args, conn):
+    """A worker process's body: runs its shard and sends the outcome, without the exception object, to the caller."""
+    outcome = _outcome(target, device, shard, args)
+    if outcome is not None:
+        outcome = outcome[:3]
+    try:
+        conn.send(outcome)
+    except Exception:                                    # noqa: BLE001 - an exception type that does not pickle
+        index, etype, message = outcome
+        conn.send((index, RuntimeError, f"{etype.__name__}: {message}"))
+    conn.close()
+
+
+def run_on_devices(shards, target, args):
+    """Runs target(device, shard, args) for each (device, shard) of shards, one process per shard after the first,
+    started with the spawn method (CUDA cannot be forked), while the calling process runs the first shard itself.
+    target must be a module-level function (the workers import it) and returns None when its shard is done or
+    (failing input index, exception) for the first input it failed on.
+
+    Returns once every shard has finished; every process is joined before this returns or raises, and terminated
+    first if the caller is interrupted.  Then, if any shard failed, raises the failure with the lowest input index: the
+    exception itself for the caller's shard, a new one of the same type and message for a worker's (RuntimeError
+    "<type>: <message>" for a type that cannot be rebuilt from its message).  A worker that exits without reporting
+    raises RuntimeError naming its device and exit code."""
+    import multiprocessing
+    from multiprocessing.connection import wait
+    ctx = multiprocessing.get_context("spawn")
+    procs = []
+    try:
+        for device, shard in shards[1:]:
+            recv, send = ctx.Pipe(duplex=False)
+            p = ctx.Process(target=_worker, args=(target, device, shard, args, send), daemon=True,
+                            name=f"vfx-device-{device}")
+            p.start()
+            send.close()
+            procs.append((device, p, recv))
+        outcomes = [_outcome(target, shards[0][0], shards[0][1], args)] if shards else []
+        for (device, p, recv), (_, shard) in zip(procs, shards[1:]):
+            wait([recv, p.sentinel])
+            try:
+                reported, outcome = recv.poll(), None
+                if reported:
+                    outcome = recv.recv()
+            except EOFError:                             # it died while sending
+                reported = False
+            p.join()
+            if not reported:
+                outcome = (shard[0], RuntimeError,
+                           f"the worker process of device {device} exited with code {p.exitcode} without reporting")
+            outcomes.append(outcome)
+    finally:
+        for _, p, recv in procs:
+            if p.is_alive():
+                p.terminate()
+            p.join()
+            recv.close()
+    failed = [o for o in outcomes if o is not None]
+    if not failed:
+        return
+    first = min(failed, key=lambda o: o[0])
+    if len(first) == 4:
+        raise first[3]
+    _, etype, message = first
+    try:
+        e = etype(message)
+    except Exception:                                    # noqa: BLE001
+        e = RuntimeError(f"{etype.__name__}: {message}")
+    raise e

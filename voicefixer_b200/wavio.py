@@ -86,6 +86,137 @@ def load_native(path):
     return _read_pcm(path)
 
 
+def probe(path):
+    """(frames, channels, rate) of an audio file from its headers, without decoding it: load_native(path)'s
+    (x.shape[0], x.shape[1], sr).  WAV: the RIFF chunks are walked with seeks by _read_riff's rules (padding, extensible
+    format, a `data` size of 0 / 0xFFFFFFFF or past the end meaning "to the end of the file").  FLAC: STREAMINFO's total
+    samples; a stream that leaves it 0 (length unknown) is measured from its last frame's header, or, if no frame header
+    is found there, estimated from the file size as if uncompressed.  Raises RuntimeError for a file that is not one."""
+    import os
+    import struct
+    path = str(path)
+    size = os.path.getsize(path)
+    with open(path, "rb") as f:
+        if path.lower().endswith(".flac"):
+            return _probe_flac(f, size)
+        head = f.read(12)
+        if len(head) < 12 or head[:4] != b"RIFF" or head[8:12] != b"WAVE":
+            raise RuntimeError(f"{path}: not a RIFF/WAVE file")
+        pos, fmt = 12, None
+        while pos + 8 <= size:
+            f.seek(pos)
+            cid, csize = struct.unpack("<4sI", f.read(8))
+            body = pos + 8
+            if cid == b"fmt ":
+                if csize < 16:
+                    raise RuntimeError(f"{path}: short fmt chunk")
+                _, nch, sr, _, _, bits = struct.unpack("<HHIIHH", f.read(16))
+                fmt = (nch, sr, bits)
+            elif cid == b"data":
+                if fmt is None:
+                    break
+                if csize in (0, 0xFFFFFFFF) or body + csize > size:
+                    csize = size - body
+                nch, sr, bits = fmt
+                if nch < 1 or sr < 1:
+                    raise RuntimeError(f"{path}: invalid channel count / sample rate")
+                return csize // ((bits + 7) // 8 * nch), nch, sr
+            pos = body + csize + (csize & 1)
+    raise RuntimeError(f"{path}: missing fmt or data chunk")
+
+
+def _probe_flac(f, size):
+    from . import _hostio
+    n = 1 << 14
+    while True:                                          # the metadata chain, read until STREAMINFO's block is whole
+        f.seek(0)
+        try:
+            info = _hostio.flac_info(f.read(n))
+            break
+        except RuntimeError:
+            if n >= size:
+                raise
+            n *= 8
+    ch, rate, total = int(info.channels), int(info.sample_rate), int(info.total_samples)
+    if total == 0:
+        audio = size - int(info.audio_offset)
+        tail = min(audio, int(info.max_blocksize or 65535) * ch * 5 + 4096)      # more than one frame can take
+        f.seek(size - tail)
+        total = _flac_last_sample(f.read(tail), info)
+        if total is None:
+            total = audio * 8 // (ch * int(info.bits_per_sample))
+    return total, ch, rate
+
+
+def _crc8(data):
+    c = 0
+    for b in data:
+        c ^= b
+        for _ in range(8):
+            c = ((c << 1) ^ 0x07) & 0xFF if c & 0x80 else (c << 1) & 0xFF
+    return c
+
+
+_CRC16 = []
+
+
+def _crc16(data):
+    """FLAC's frame CRC-16 (polynomial 0x8005, initial 0); 0 over a whole frame, footer included."""
+    if not _CRC16:
+        for v in range(256):
+            c = v << 8
+            for _ in range(8):
+                c = ((c << 1) ^ 0x8005) & 0xFFFF if c & 0x8000 else (c << 1) & 0xFFFF
+            _CRC16.append(c)
+    c = 0
+    for b in data:
+        c = ((c << 8) & 0xFFFF) ^ _CRC16[(c >> 8) ^ b]
+    return c
+
+
+def _flac_frame_header(h):
+    """(number, blocksize, header bytes) of the FLAC frame header at the start of h, number being the frame number of
+    a fixed-blocksize stream or the first sample's of a variable one; None if h does not start with a valid one."""
+    if len(h) < 6 or h[0] != 0xFF or h[1] not in (0xF8, 0xF9):
+        return None
+    bs_code, sr_code, ch_code = h[2] >> 4, h[2] & 0x0F, h[3] >> 4
+    if bs_code == 0 or sr_code == 0x0F or ch_code > 10 or h[3] & 1:
+        return None
+    k = 0                                                # the number's UTF-8-style coding: k leading ones, k - 1 more bytes
+    while k < 8 and h[4] & (0x80 >> k):
+        k += 1
+    if k == 1 or k > 7 or 5 + max(k - 1, 0) > len(h):
+        return None
+    number, q = h[4] & (0x7F >> k), 5
+    for _ in range(k - 1):
+        if h[q] & 0xC0 != 0x80:
+            return None
+        number, q = number << 6 | h[q] & 0x3F, q + 1
+    if bs_code in (6, 7):
+        bs, q = int.from_bytes(h[q:q + bs_code - 5], "big") + 1, q + bs_code - 5
+    else:
+        bs = 192 if bs_code == 1 else (576 << (bs_code - 2) if bs_code < 6 else 256 << (bs_code - 8))
+    q += {12: 1, 13: 2, 14: 2}.get(sr_code, 0)
+    if q >= len(h) or _crc8(h[:q]) != h[q]:
+        return None
+    return number, bs, q + 1
+
+
+def _flac_last_sample(tail, info):
+    """One past the last sample of the FLAC frame that ends `tail` (the end of the file): the last offset that holds a
+    frame header (CRC-8 checked) from which the frame's CRC-16 checks to the end; None if there is none."""
+    p = len(tail)
+    while p > 0:
+        p = max(tail.rfind(b"\xff\xf8", 0, p), tail.rfind(b"\xff\xf9", 0, p))
+        if p < 0:
+            return None
+        hdr = _flac_frame_header(tail[p:p + 16])
+        if hdr is not None and _crc16(tail[p:]) == 0:
+            number, bs, _ = hdr
+            return number + bs if tail[p + 1] & 1 else number * int(info.max_blocksize) + bs
+    return None
+
+
 def load_mono_native(path):
     """(x, sr): the file's mono mix (mean over channels), float32, at its own rate sr."""
     x, sr = load_native(path)
