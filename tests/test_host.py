@@ -246,63 +246,51 @@ def test_planning_only_engine_validates_weight_sets_and_sizes_workspace(states, 
     assert rc == -1 and b"planning-only" in lib.vfx_last_error()
 
 
-def test_cli_pipeline_overlaps_io_keeps_order_and_propagates_errors():
-    """run_jobs: reader thread -> GPU stage -> writer thread (SURVEY 8f rank 1: disk -> GPU -> disk must keep up)."""
-    import threading, time as _t
-    from voicefixer_b200.__main__ import run_jobs
-    jobs = [(f"in{i}.wav", f"out{i}.wav", 0) for i in range(6)] + [("in5.wav", "out5-mode1.wav", 1)]
-    log, lock = [], threading.Lock()
+def test_cli_per_file_runs_one_job_per_wave_through_run_waves(tmp_path, monkeypatch, capsys):
+    """execute(batch=False) is run_waves with budget 0: each job a wave of its own, an input that the job before also
+    read (--mode all) decoded once, `Processing` through say and `Restoration took` through print (--silent keeps it),
+    outputs written in job order.  The pipeline's overlap, order and error rules are tested on run_waves itself."""
+    from voicefixer_b200 import api, wavio, __main__ as cli
+    calls, waves = [], []
+    run_waves = api.run_waves
 
-    def rec(*a):
-        with lock:
-            log.append(a)
+    def spy(srcs, budget, load, restore, write):
+        calls.append(("run_waves", list(srcs), budget))
+        return run_waves(srcs, budget, load, restore, lambda ids, out: (waves.append(ids), write(ids, out)))
 
-    def load(src):
-        _t.sleep(0.05); rec("load", src); return src + ":pcm"
+    class StubFixer:
+        def _load_wav(self, path, sample_rate):
+            calls.append(("load", os.path.basename(path), sample_rate))
+            return wavio.load_mono(path, sample_rate)
 
-    def restore(wav, mode):
-        _t.sleep(0.05); rec("gpu", wav, mode); return wav + ":restored%d" % mode
+        def restore_inmem(self, wav, cuda=False, mode=0):
+            calls.append(("restore", len(wav), cuda, mode))
+            return wav[None] * (0.25 * (mode + 1))
 
-    def save(out, dst):
-        _t.sleep(0.05); rec("save", out, dst)
-
-    t0 = _t.time()
-    took = run_jobs(jobs, load, restore, save, say=lambda *a: None)
-    wall = _t.time() - t0
-    assert len(took) == 7 and wall < 0.85 * (6 + 7 + 7) * 0.05                      # stages overlap (serial = 1.0 s)
-    assert [e[1] for e in log if e[0] == "load"] == [f"in{i}.wav" for i in range(6)]  # in5.wav decoded once for two modes
-    assert [e[2] for e in log if e[0] == "save"] == [j[1] for j in jobs]              # results written in job order
-    assert ("save", "in5.wav:pcm:restored1", "out5-mode1.wav") in log
-
-    def bad_load(src):
-        if src == "in2.wav":
-            raise FileNotFoundError(src)
-        return load(src)
-
-    log.clear()
-    with pytest.raises(FileNotFoundError, match="in2.wav"):
-        run_jobs(jobs, bad_load, restore, save, say=lambda *a: None)
-    assert [e[2] for e in log if e[0] == "save"] == ["out0.wav", "out1.wav"]          # finished work is kept, nothing after
-
-    def bad_gpu(wav, mode):
-        if wav.startswith("in3"):
-            raise RuntimeError("device fault")
-        return restore(wav, mode)
-
-    log.clear()
-    with pytest.raises(RuntimeError, match="device fault"):
-        run_jobs(jobs, load, bad_gpu, save, say=lambda *a: None)
-    assert "out3.wav" not in [e[2] for e in log if e[0] == "save"]
-
-    def bad_save(out, dst):
-        if dst == "out1.wav":
-            raise OSError("disk full")
-        save(out, dst)
-
-    with pytest.raises(OSError, match="disk full"):
-        run_jobs(jobs, load, restore, bad_save, say=lambda *a: None)
-    assert threading.active_count() < 10                                             # no leaked pipeline threads
-    assert run_jobs([], load, restore, save) == []
+    monkeypatch.setattr(api, "run_waves", spy)
+    rng = np.random.default_rng(1)
+    srcs = [str(tmp_path / f"in{k}.wav") for k in range(2)]
+    for k, src in enumerate(srcs):
+        wavio.save_wave((0.5 * rng.standard_normal((1, 3000 + k))).clip(-1, 1).astype(np.float32), src)
+    jobs = [(srcs[0], str(tmp_path / f"a{m}.wav"), m) for m in (0, 1, 2)] + [(srcs[1], str(tmp_path / "b.wav"), 1)]
+    for say in (print, lambda *a: None):                                         # default, then --silent
+        del calls[:], waves[:]
+        cli.execute(StubFixer(), jobs, batch=False, cuda=False, say=say)
+        assert calls[0] == ("run_waves", [j[0] for j in jobs], 0) and waves == [[0], [1], [2], [3]]
+        assert [c for c in calls if c[0] == "load"] == [("load", "in0.wav", 44100), ("load", "in1.wav", 44100)]
+        assert [c for c in calls if c[0] == "restore"] == [("restore", 3000 + (j[0] == srcs[1]), False, j[2])
+                                                           for j in jobs]
+        took, lines = "Restoration took 0.0 s", capsys.readouterr().out.splitlines()
+        if say is print:
+            assert lines == [x for src, _, m in jobs for x in ("Processing {}, mode={}".format(src, m), took)]
+        else:
+            assert lines == [took] * 4
+        for src, dst, m in jobs:
+            wavio.save_wave(wavio.load_mono(src)[None] * (0.25 * (m + 1)), tmp_path / "want.wav")
+            assert open(dst, "rb").read() == (tmp_path / "want.wav").read_bytes()
+    calls.clear()
+    cli.execute(StubFixer(), [], batch=False)                                   # no jobs: nothing is read or restored
+    assert calls == [("run_waves", [], 0)] and capsys.readouterr().out == ""
 
 
 def test_cli_main_wiring_folder_mode_all_with_flac_output(tmp_path, monkeypatch, capsys):

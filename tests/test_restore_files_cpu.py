@@ -124,14 +124,17 @@ def _written(log):
 
 def test_run_waves_overlaps_stages_and_keeps_order():
     srcs = [f"in{i}" for i in range(6)] + ["in5"]                              # in5 twice (two modes)
-    t0 = time.time()
-    log, waves = _pipeline(srcs, budget=20, delay=0.05)
-    wall = time.time() - t0
-    assert waves == 4                                                           # [0, 1] [2, 3] [4, 5] [6]
-    assert [e[1] for e in log if e[0] == "gpu"] == [[0, 1], [2, 3], [4, 5], [6]]
-    assert _written(log) == [f"out{i}" for i in range(7)]
-    assert ("write", "out6", "in5:pcm:restored") in log
-    assert wall < 0.85 * (7 + 4 + 4) * 0.05                                     # the stages overlap
+    for budget, gpu in ((20, [[0, 1], [2, 3], [4, 5], [6]]),
+                        (0, [[i] for i in range(7)])):                          # the command line's one file per wave
+        t0 = time.time()
+        log, waves = _pipeline(srcs, budget, delay=0.05)
+        wall = time.time() - t0
+        assert waves == len(gpu)
+        assert [e[1] for e in log if e[0] == "gpu"] == gpu
+        assert _written(log) == [f"out{i}" for i in range(7)]
+        assert ("write", "out6", "in5:pcm:restored") in log
+        assert [e[1] for e in log if e[0] == "read"] == srcs[:6]                # in5 decoded once
+        assert wall < 0.85 * (6 + 2 * len(gpu)) * 0.05                          # the stages overlap
 
 
 def test_run_waves_decodes_an_input_once_per_wave():
@@ -139,9 +142,12 @@ def test_run_waves_decodes_an_input_once_per_wave():
     assert waves == 2                                                           # [0, 1, 2] [3, 4, 5]
     assert [e[1] for e in log if e[0] == "read"] == ["a", "b", "a"]
     assert _written(log) == [f"out{i}" for i in range(6)]
+    log, waves = _pipeline(["a", "a", "b"], budget=0)                          # one job per wave: the reader still
+    assert waves == 3                                                           # holds the job before when it loads
+    assert [e[1] for e in log if e[0] == "read"] == ["a", "b"]
 
 
-@pytest.mark.parametrize("budget", [10, 30, 1000])
+@pytest.mark.parametrize("budget", [0, 10, 30, 1000])
 def test_run_waves_failing_read_keeps_the_files_before_it(budget):
     srcs = [f"in{i}" for i in range(7)]
     log, err = _pipeline(srcs, budget, fail_load="in4")
@@ -152,13 +158,15 @@ def test_run_waves_failing_read_keeps_the_files_before_it(budget):
 
 def test_run_waves_failing_restore_fails_its_wave_only():
     srcs = [f"in{i}" for i in range(7)]
-    log, err = _pipeline(srcs, budget=20, fail_restore="in3")                  # waves [0, 1] [2, 3] ...
-    assert isinstance(err, RuntimeError) and "device fault" in str(err)
-    assert _written(log) == ["out0", "out1"]
-    assert not any(e[0] == "gpu" and 4 in e[1] for e in log)
+    for budget, written in ((20, ["out0", "out1"]),                            # waves [0, 1] [2, 3] ...
+                            (0, ["out0", "out1", "out2"])):                     # one file per wave
+        log, err = _pipeline(srcs, budget, fail_restore="in3")
+        assert isinstance(err, RuntimeError) and "device fault" in str(err)
+        assert _written(log) == written
+        assert not any(e[0] == "gpu" and 4 in e[1] for e in log)
 
 
-@pytest.mark.parametrize("budget", [10, 1000])
+@pytest.mark.parametrize("budget", [0, 10, 1000])
 def test_run_waves_failing_write_keeps_the_files_before_it(budget):
     srcs = [f"in{i}" for i in range(7)]
     log, err = _pipeline(srcs, budget, fail_write="out3")
@@ -168,8 +176,9 @@ def test_run_waves_failing_write_keeps_the_files_before_it(budget):
 
 def test_run_waves_threads_exit():
     before = {t.ident for t in threading.enumerate()}
-    for kw in ({}, {"fail_load": "in2"}, {"fail_restore": "in2"}, {"fail_write": "out2"}):
-        _pipeline([f"in{i}" for i in range(5)], budget=20, **kw)
+    for budget in (0, 20):
+        for kw in ({}, {"fail_load": "in2"}, {"fail_restore": "in2"}, {"fail_write": "out2"}):
+            _pipeline([f"in{i}" for i in range(5)], budget, **kw)
     assert not [t for t in threading.enumerate() if t.ident not in before and t.name.startswith("vfx-wave")]
 
 

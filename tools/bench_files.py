@@ -1,6 +1,7 @@
-"""The command line's two ways through a folder of files, on three seeded folders: one file at a time (`run_jobs`, what
-`python -m voicefixer_b200 --infolder ...` runs) against many files per batch (`VoiceFixer.restore_files`, what it runs
-with `--batch`), both through `__main__.execute`, in one process, alternating, synthetic weights:
+"""The command line's two ways through a folder of files, on three seeded folders: one file at a time (`run_waves` with
+a budget of 0, what `python -m voicefixer_b200 --infolder ...` runs) against many files per batch
+(`VoiceFixer.restore_files`, what it runs with `--batch`), both through `__main__.execute`, in one process, alternating,
+synthetic weights:
 
   short16k:  64 utterances of 1 .. 10 s at 16 kHz, mono 16-bit WAV;
   cli10s:    16 recordings of 10 s at 44.1 kHz, mono 16-bit WAV (bench.py's cli_folder shape);

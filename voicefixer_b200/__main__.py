@@ -5,11 +5,12 @@
 
 Same flags, same output naming (`--mode all` writes `<name>-mode<k><ext>` for k = 0,1,2), same
 `.wav`-only input rule, same messages.  The work is planned first (`plan_jobs`, a pure function) and
-then executed with one VoiceFixer instance as a reader -> GPU -> writer pipeline (`run_jobs`), one
-file at a time; with `--batch` the same jobs run through `VoiceFixer.restore_files`, many files per
-batch (`execute`).  With `--keep-channels` every channel of a file is restored and written (restore(...,
-channels="keep")), on either path, with the same bytes.  With `--gpus N` (N > 1) the jobs run as with `--batch`,
-spread over N GPUs by `VoiceFixer.restore_files(..., gpus=N)`, again with the same bytes."""
+then executed with one VoiceFixer instance (`execute`), one file at a time through the reader -> GPU ->
+writer pipeline of `VoiceFixer.restore_files` (`api.run_waves`); with `--batch` the same jobs run
+through `VoiceFixer.restore_files` itself, many files per batch.  With `--keep-channels` every channel
+of a file is restored and written (restore(..., channels="keep")), on either path, with the same bytes.
+With `--gpus N` (N > 1) the jobs run as with `--batch`, spread over N GPUs by
+`VoiceFixer.restore_files(..., gpus=N)`, again with the same bytes."""
 import argparse
 import os
 import re
@@ -79,104 +80,42 @@ def plan_jobs(args):
     return jobs
 
 
-def run_jobs(jobs, load, restore, save, say=print, depth=2):
-    """Executes [(src, dst, mode)] as a three-stage pipeline so that disk and codec time hide behind GPU time:
-    a reader thread decodes / resamples the next inputs (`load(src)`), the calling thread runs `restore(wav, mode)`
-    on the GPU, a writer thread encodes and writes the previous results (`save(out, dst)`).  At most `depth` decoded
-    inputs and `depth` finished outputs are in flight.  Jobs complete in order; like the sequential loop of the reference,
-    every job before a failing one is still written, nothing after it is started, and the exception is re-raised once
-    the threads have drained.  A source that is
-    used by consecutive jobs (`--mode all`) is decoded once.  Returns the per-job GPU-stage seconds."""
-    import queue
-    import threading
-    loaded, finished, took = queue.Queue(maxsize=depth), queue.Queue(maxsize=depth), []
-    stop, write_errors = threading.Event(), []
-
-    def reader():                                        # failures travel down the queue IN ORDER, so that every
-        last_src, last_wav = None, None                  # job before the failing one still completes
-        try:
-            for job in jobs:
-                if stop.is_set():
-                    break
-                if job[0] != last_src:
-                    last_src, last_wav = job[0], load(job[0])
-                loaded.put((job, last_wav))
-        except BaseException as e:                       # noqa: BLE001 - re-raised by the caller's thread
-            loaded.put(e)
-        finally:
-            loaded.put(None)
-
-    def writer():
-        while True:
-            item = finished.get()
-            if item is None:
-                return
-            if write_errors:
-                continue                                 # drain
-            try:
-                save(item[1], item[0][1])
-            except BaseException as e:                   # noqa: BLE001
-                write_errors.append(e)
-                stop.set()
-
-    threads = [threading.Thread(target=reader, name="vfx-reader", daemon=True),
-               threading.Thread(target=writer, name="vfx-writer", daemon=True)]
-    for t in threads:
-        t.start()
-    failure = None
-    try:
-        while True:
-            item = loaded.get()
-            if item is None:
-                break
-            if failure is not None or stop.is_set():
-                continue                                 # keep draining so the reader can finish
-            if isinstance(item, BaseException):
-                failure = item
-                stop.set()
-                continue
-            (src, dst, mode), wav = item
-            say("Processing {}, mode={}".format(src, mode))
-            t0 = time.time()
-            try:
-                out = restore(wav, mode)
-            except BaseException as e:                   # noqa: BLE001
-                failure = e
-                stop.set()
-                continue
-            took.append(time.time() - t0)
-            print("Restoration took {} s".format(round(took[-1], 1)))
-            finished.put((item[0], out))
-    finally:
-        finished.put(None)
-        for t in threads:
-            t.join()
-    if write_errors:
-        raise write_errors[0]
-    if failure is not None:
-        raise failure
-    return took
-
-
 def execute(vf, jobs, batch=False, cuda=True, say=print, channels="mix", gpus=1):
-    """Runs [(src, dst, mode)] with the VoiceFixer vf: one file at a time through run_jobs, or with batch through
-    vf.restore_files, which prints the same `Processing` line per job as its wave starts and one `Restoration took`
-    line per wave.  channels: restore()'s ("mix" or "keep").  gpus > 1 runs the jobs through
-    vf.restore_files(..., gpus=gpus) whatever batch is; each device then prints its own lines, the `Processing` ones
-    only when say is print, and lines from different devices interleave."""
-    from . import wavio
+    """Runs [(src, dst, mode)] with the VoiceFixer vf: one file at a time, or with batch through vf.restore_files, which
+    prints the same `Processing` line per job as its wave starts and one `Restoration took` line per wave.
+    channels: restore()'s ("mix" or "keep").  gpus > 1 runs the jobs through vf.restore_files(..., gpus=gpus) whatever
+    batch is; each device then prints its own lines, the `Processing` ones only when say is print, and lines from
+    different devices interleave.
+
+    One file at a time is restore_files' pipeline (api.run_waves) with a budget of 0, so that every job is a wave of
+    its own: a reader thread decodes the next inputs, the calling thread restores one job with vf.restore_inmem (or
+    vf.restore_columns), a writer thread writes the previous outputs with wavio.save_wave.  An input that the job before
+    also read (`--mode all`) is decoded once.  Every job before a failing one is written, nothing after it is started."""
+    from . import api, wavio
     if gpus != 1 and jobs:
         vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda,
                          channels=channels, gpus=gpus, _messages=("processing", "took") if say is print else ("took",))
     elif not batch:
         if channels == "keep":                                            # = vf.restore(..., channels="keep") per job
-            load = lambda src: wavio.read_wave(src, 44100)                # noqa: E731
-            restore = lambda wav, mode: vf.restore_columns(wav, cuda=cuda, mode=mode)   # noqa: E731
+            read = lambda src: wavio.read_wave(src, 44100)                # noqa: E731
+            run = vf.restore_columns
         else:                                                             # = vf.restore(input, output, ...) per job
-            load = lambda src: vf._load_wav(src, sample_rate=44100)       # noqa: E731  base.py:141-146, staged
-            restore = lambda wav, mode: vf.restore_inmem(wav, cuda=cuda, mode=mode)     # noqa: E731
-        run_jobs(jobs, load=load, restore=restore,
-                 save=lambda out, dst: wavio.save_wave(out, fname=dst, sample_rate=44100), say=say)
+            read = lambda src: vf._load_wav(src, sample_rate=44100)       # noqa: E731  base.py:141-146, staged
+            run = vf.restore_inmem
+
+        def load(i, prev):                    # length 1: a 0 fits budget 0, and every job would join one wave
+            return (read(jobs[i][0]) if prev is None else prev), 1
+
+        def restore(wave):
+            [(i, wav)] = wave
+            say("Processing {}, mode={}".format(jobs[i][0], jobs[i][2]))
+            t0 = time.time()
+            out = run(wav, cuda=cuda, mode=jobs[i][2])
+            print("Restoration took {} s".format(round(time.time() - t0, 1)))
+            return out
+
+        api.run_waves([j[0] for j in jobs], 0, load, restore,
+                      lambda ids, out: wavio.save_wave(out, fname=jobs[ids[0]][1], sample_rate=44100))
     elif jobs:
         kw = {"channels": channels} if channels != "mix" else {}        # "mix" is restore_files' default
         vf.restore_files([j[0] for j in jobs], [j[1] for j in jobs], mode=[j[2] for j in jobs], cuda=cuda, **kw,

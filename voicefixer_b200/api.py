@@ -161,15 +161,18 @@ def run_waves(srcs, budget, load, restore, write, depth=2):
     """The pipeline of VoiceFixer.restore_files over jobs 0 .. len(srcs) - 1, srcs[i] being job i's input file:
 
     a reader thread calls load(i, prev) -> (item, length at 44.1 kHz) for each job in order and groups the jobs into
-    waves by plan_waves(lengths, budget).  prev is the item load returned for an earlier job of the same wave with the
-    same source, or None: load then checks that item for job i rather than reading the file again.
+    waves by plan_waves(lengths, budget).  prev is the item load returned for an earlier job with the same source that
+    the reader still holds (loaded, its wave not yet handed on), or None: load then checks that item for job i rather
+    than reading the file again.  A wave is handed on only once the next job's length is known, so the reader still
+    holds the job just before i, even when every wave is one job (budget 0): consecutive jobs on one source (the command
+    line's `--mode all`) decode it once.
     The calling thread calls restore(wave) -> result for each wave [(i, item), ...]; it may return before the GPU is done.
     A writer thread calls write([i, ...], result) for each wave, which writes the wave's outputs in order.
 
-    At most `depth` loaded and `depth` restored waves are in flight.  Errors follow run_jobs's order rule: a failing load
-    cuts its wave short (the jobs before it in the wave are restored and written), a failing restore fails its wave,
-    every job before the failure is written and nothing after it is started, and the exception is re-raised once the
-    threads have drained.  The exception's `vfx_job` attribute is then the job it stopped at: the one whose load failed,
+    At most `depth` loaded and `depth` restored waves are in flight.  Errors keep the order of a sequential loop: a
+    failing load cuts its wave short (the jobs before it in the wave are restored and written), a failing restore fails
+    its wave, every job before the failure is written and nothing after it is started, and the exception is re-raised
+    once the threads have drained.  The exception's `vfx_job` attribute is then the job it stopped at: the one whose load failed,
     the first of a failed wave, or for a failed write the job write set it to (else the wave's first).  Returns the
     number of waves restored."""
     import queue
