@@ -285,7 +285,7 @@ __global__ void __launch_bounds__(NT, 1) conv_gemm_wgmma_kernel(const __grid_con
       const bool live = tile_row<TMA>(d, tp, M, mt, ct & 127, b, qh, qw) && row_stored<SEQ>(d, b, qh, qw);
       if (!named_sync_or(2, 256, live)) continue;
     }
-    k_loop<BN, KIND>(ring, acc, k, niter, cw, l, [](int, uint32_t sa) { return sa; }, released);
+    k_loop<BN, KIND>(acc, niter, cw, ring_feed(ring, k, l, [](int, uint32_t sa) { return sa; }, StageB{}, released));
     k += niter;
 
     // ---- epilogue: accumulator element (j, h, e) of lane l in warp w of consumer warpgroup cw is

@@ -93,62 +93,103 @@ template <class P> struct Ring {
   }
 };
 
-// The consumers' K loop of one tile, for consumer warpgroup cw and lane l: acc = the sum of the tile's niter slices,
-// ring slices k0 ... k0 + niter - 1.  Slice it is 4 m64nBN wgmma (32 bytes of K each) of the A tile at
-// a_tile(it, stage address), from row cw * 64 on, by the BN weight rows that follow the stage's A tile, into a zeroed
-// partial: the tensor core's accumulator adds truncate, so the partials are added to acc in slice order with
-// round-to-nearest fp32 adds, and the error of long reductions (9 taps x 768 channels) does not build up as a bias.
-// One group is in flight: slice it goes into partial it & 1 while slice it - 1 is added.  released(it) runs once slice
-// it's stage has been handed back, before its partial is added.
+// The consumers' K loop of one tile, for consumer warpgroup cw: acc = the sum of the tile's niter K slices, which the
+// feed f describes.  Slice it is 4 m64nBN wgmma (32 bytes of K each) into a zeroed partial: the tensor core's accumulator
+// adds truncate, so the partials are added to acc in slice order with round-to-nearest fp32 adds, and the error of long
+// reductions (9 taps x 768 channels) does not build up as a bias.  One group is in flight: slice it goes into partial
+// it & 1 while slice it - 1 is added.
+// The feed: wait(it) before slice it is read; b(it), the address of its BN weight rows (K-major, 128-byte swizzle);
+// its A operand, either (REG_A false) a(it), the address of its 128-row A tile, of which warpgroup cw reads rows
+// cw * 64 on by descriptor, or (REG_A true) a_frag(it, fr), which loads this warp's 16 x (32 bytes of K) register
+// fragment of each of the 4 wgmma; release(it) once slice it's wgmma group has retired, before its partial is added.
+// The register fragments of the group in flight are not overwritten before its wgmma_wait: two sets alternate.
 // niter is a runtime value on purpose: with a compile-time count, ptxas peels the loop and serialises its wgmma groups
 // (C7514), and a fully unrolled loop spills.
-template <int BN, int KIND, class P, class ATile, class Released>
-__device__ __forceinline__ void k_loop(const Ring<P>& ring, float (&acc)[BN / 2], uint32_t k0, int niter, int cw, int l,
-                                       ATile a_tile, Released released) {
+template <int BN, int KIND, class Feed>
+__device__ __forceinline__ void k_loop(float (&acc)[BN / 2], int niter, int cw, const Feed& f) {
   float p0[BN / 2], p1[BN / 2];
-  auto issue = [&](float (&p)[BN / 2], int it) {
-    ring.wait_full(k0 + it);
+  uint32_t f0[4][4], f1[4][4];                    // register A fragments (Feed::REG_A only)
+  auto issue = [&](float (&p)[BN / 2], uint32_t (&fr)[4][4], int it) {
+    f.wait(it);
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) p[i] = 0.f;
-    const uint32_t sa = ring.stage(k0 + it);
-    const uint64_t da = sw128_desc(a_tile(it, sa) + cw * 64 * 128), db = sw128_desc(sa + A_BYTES);
-    wgmma_fence();
+    const uint64_t db = sw128_desc(f.b(it));
+    if constexpr (Feed::REG_A) {
+      f.a_frag(it, fr);
+      wgmma_fence();
 #pragma unroll
-    for (int q = 0; q < 4; ++q) Wgmma<BN, KIND>::mma(p, da + 2 * q, db + 2 * q);
+      for (int q = 0; q < 4; ++q) Wgmma<BN, KIND>::mma(p, fr[q], db + 2 * q);
+    } else {
+      const uint64_t da = sw128_desc(f.a(it) + cw * 64 * 128);
+      wgmma_fence();
+#pragma unroll
+      for (int q = 0; q < 4; ++q) Wgmma<BN, KIND>::mma(p, da + 2 * q, db + 2 * q);
+    }
     wgmma_commit();
   };
-  auto retire = [&](float (&p)[BN / 2], int it) {
+  auto retire = [&](float (&p)[BN / 2], uint32_t (&fr)[4][4], int it) {
     wgmma_fence_operand(p);                       // the reads of p below stay after the wgmma_wait that precedes
-    ring.release(k0 + it, l);
-    released(it);
+    if constexpr (Feed::REG_A) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) wgmma_fence_operand(fr[q]);   // fr stays allocated until its group has retired
+    }
+    f.release(it);
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] += p[i];
     wgmma_fence_operand(acc);                     // the adds stay here, before the next slice is issued: p is reused
   };
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  issue(p0, 0);
+  issue(p0, f0, 0);
   int it = 1;
 #pragma unroll 1
   for (; it + 1 < niter; it += 2) {
-    issue(p1, it);
+    issue(p1, f1, it);
     wgmma_wait<1>();
-    retire(p0, it - 1);
-    issue(p0, it + 1);
+    retire(p0, f0, it - 1);
+    issue(p0, f0, it + 1);
     wgmma_wait<1>();
-    retire(p1, it);
+    retire(p1, f1, it);
   }
   if (it < niter) {
-    issue(p1, it);
+    issue(p1, f1, it);
     wgmma_wait<1>();
-    retire(p0, it - 1);
+    retire(p0, f0, it - 1);
     wgmma_wait<0>();
-    retire(p1, it);
+    retire(p1, f1, it);
   } else {
     wgmma_wait<0>();
-    retire(p0, it - 1);
+    retire(p0, f0, it - 1);
   }
 }
+
+// The feed of K slices k0, k0 + 1, ... of a ring: slice it's A tile is a_tile(it, stage address), its weight rows
+// b_tile(it, stage address); its stage is handed back by lane l's warp once read, then released(it) runs.
+template <class P, class ATile, class BTile, class Released> struct RingFeed {
+  static constexpr bool REG_A = false;
+  const Ring<P>& ring;
+  uint32_t k0;
+  int l;
+  ATile a_tile;
+  BTile b_tile;
+  Released released;
+  __device__ __forceinline__ void wait(int it) const { ring.wait_full(k0 + it); }
+  __device__ __forceinline__ uint32_t a(int it) const { return a_tile(it, ring.stage(k0 + it)); }
+  __device__ __forceinline__ uint32_t b(int it) const { return b_tile(it, ring.stage(k0 + it)); }
+  __device__ __forceinline__ void release(int it) const {
+    ring.release(k0 + it, l);
+    released(it);
+  }
+};
+template <class P, class ATile, class BTile, class Released>
+__device__ __forceinline__ RingFeed<P, ATile, BTile, Released> ring_feed(const Ring<P>& ring, uint32_t k0, int l,
+                                                                         ATile a_tile, BTile b_tile, Released released) {
+  return {ring, k0, l, a_tile, b_tile, released};
+}
+// the weight rows of a stage that carries them: they follow its A tile
+struct StageB {
+  __device__ __forceinline__ uint32_t operator()(int, uint32_t sa) const { return sa + A_BYTES; }
+};
 
 // ---- host
 

@@ -1,6 +1,6 @@
 // PTX wrappers of the Hopper tensor-core path (conv_gemm_tc.cu, resstack_pair.cu): TMA tile loads and stores, cp.async operand
-// staging with zero fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups
-// and the shared-memory matrix descriptor; on the host, the SM count and the tensor-map encoder their launches use.
+// staging with zero fill, the generic -> async proxy fence, mbarriers, named barriers, setmaxnreg, wgmma fences / groups,
+// ldmatrix and the shared-memory matrix descriptor; on the host, the SM count and the tensor-map encoder their launches use.
 #pragma once
 #include <atomic>
 #include <cuda.h>      // CUtensorMap and the types of its encoder; the encoder itself is looked up at run time
@@ -79,6 +79,17 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int N> __device__ __forceinline__ void wgmma_fence_operand(float (&r)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// ... and on a register A fragment, which the tensor core reads until its group has retired
+template <int N> __device__ __forceinline__ void wgmma_fence_operand(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
+// four 8 x 8 b16 matrices from shared memory: lanes 8i ... 8i + 7 give the addresses of matrix i's rows (16 bytes each),
+// and lane l receives bytes 4 (l % 4) ... + 3 of row l / 4 of matrix i in r[i]
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
 }
 
 // K-major operand tile with 128-byte rows in the 128-byte swizzle (16-byte chunk c of row r stored at chunk c ^ (r & 7)),
